@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 sparse hot path.
+"""bench.py -- headline benchmark of the sparse hot path on an H100.
 
 Metric (BASELINE.json): SpMV effective GFLOP/s (2*nnz/t) + achieved HBM GB/s, fp64 CrsMatrix.
 Workload at N=1 (BASELINE.json configs[1]): 10M x 10M, ~60 nnz/row, 27-point Laplacian family ->
@@ -72,7 +72,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -201,30 +201,6 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm), "window": "warm-up + timed region", "source": "nvidia-smi -lms 100"}
-
-
-def ncu_traffic(files=("r02c15_spmv_tile_ncu_key_metrics.csv", "r01_spmv_tile_c2_ncu_key_metrics.csv"), kernel=None):
-    """(DRAM bytes per launch, file) of a kernel from the newest committed `ncu --set full` capture of it on the bench workload
-    (profiles/*key_metrics*: lines `metric,unit,value`; files holding several kernels separate them by a `Kernel Name` line) --
-    a CONSTANT of the repository, not a measurement of this run; (None, None) if absent."""
-    for name in files:
-        path = os.path.join(ROOT, "profiles", name)
-        try:
-            vals, active = {}, kernel is None
-            for ln in open(path):
-                f = ln.strip().split(",")
-                if len(f) >= 3 and f[0] == "Kernel Name":
-                    active = kernel is None or kernel in ln
-                    continue
-                if not active or len(f) != 3:
-                    continue
-                scale = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}.get(f[1])
-                if scale and f[0] not in vals:
-                    vals[f[0]] = float(f[2]) * scale
-            return int(vals["dram__bytes_read.sum"] + vals["dram__bytes_write.sum"]), name
-        except Exception:
-            continue
-    return None, None
 
 
 def alg_bytes(nnz, nrows, ncols, beta_nonzero=False):
@@ -356,7 +332,7 @@ def run_reference(args, emit):
 # ---------------------------------------------------------------------------------------------------------------------
 # secondary workloads (N = 1): BASELINE.json configs[2] (SpMM) and configs[3] (SpGEMM), reported inside the one JSON line
 # ---------------------------------------------------------------------------------------------------------------------
-def secondary_spmm(dev, scale=23, k=16, iters=10):
+def secondary_spmm(dev, scale=23, k=16, iters=10, dump_dir=None):
     """configs[2]: spmv fp32 CrsMatrix, R-MAT scale 23 (Graph500 parameters, edge factor 16, duplicates merged), 16-column
     multivector (LayoutRight), alpha = 1, beta = 0."""
     import torch
@@ -384,6 +360,8 @@ def secondary_spmm(dev, scale=23, k=16, iters=10):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / iters
+    if dump_dir:
+        dump_outputs(dump_dir, "spmm_Y", {"spmm_Y": Yd})
     # the same product on LayoutLeft operands (the Kokkos default for a multivector in CudaSpace): relayout + kernel + relayout
     Xl, Yl = Xd.t().contiguous().t(), torch.full((k, n), float("nan"), dtype=torch.float32, device=dev).t()
     hl = sp.SPMVHandle()
@@ -461,8 +439,6 @@ def secondary_spmm(dev, scale=23, k=16, iters=10):
         "roofline": {"bound": "hbm", "achieved": round(balg / ms / 1e6, 1), "peak": peak, "unit": "GB/s", "frac": round(balg / ms / 1e6 / peak, 4),
                      "algorithmic_bytes_per_launch": balg, "gather_model_bytes": bgather,
                      "frac_gather_model": round(bgather / ms / 1e6 / peak, 4),
-                     "traffic": ncu_traffic(("r02c15_spmm_coop_key_metrics.txt", "r02c8_spmm_coop_key_metrics.txt"), "spmm_item_coop_kernel")[0],
-                     "traffic_unit": "DRAM bytes of the item kernel per launch, a constant from the committed ncu --set full capture at this size (profiles/r02c*_spmm_coop_key_metrics.txt)",
                      "peak_source": peak_src},
         "cpu_baseline": {"value": round(cpu_gf, 2), "unit": "GFLOP/s", "cores": threads, "kind": "port",
                          "sample": f"oracle O4 (CPU multivector strips, spmv_impl.hpp:745-926, OpenMP over rows), first {srows} rows "
@@ -559,7 +535,7 @@ def next_rows_bench(dev):
     return out
 
 
-def secondary_spgemm(dev, n=2_000_000, deg=32, reps=2):
+def secondary_spgemm(dev, n=2_000_000, deg=32, reps=2, dump_dir=None):
     """configs[3]: spgemm_symbolic + spgemm_numeric fp64, C = A*A, A = 2M x 2M with exactly 32 distinct uniform-random columns
     per row (seed 4), values U(1,50)."""
     import torch
@@ -608,6 +584,9 @@ def secondary_spgemm(dev, n=2_000_000, deg=32, reps=2):
         del row_mapC, entriesC, valuesC
         kh.destroy_spgemm_handle()
     c_nnz = C.nnz()
+    if dump_dir:
+        dump_outputs(dump_dir, "spgemm_row_map", {"spgemm_row_map": C.row_map})
+        dump_outputs(dump_dir, "spgemm_C", {"spgemm_entries": C.entries, "spgemm_values": C.values})
     # parity: blocks of rows vs the oracle (reference SPGEMM_DEBUG + sort), structure AND values bit-exact
     orc = oracle_lib.Oracle()
     rpC = C.row_map.cpu().numpy()
@@ -681,8 +660,6 @@ def secondary_spgemm(dev, n=2_000_000, deg=32, reps=2):
                      "unit": "GB/s", "frac": round(b_num / ms_num / 1e6 / peak, 4), "algorithmic_bytes_per_launch": b_num,
                      "gather_model_bytes": b_gather, "frac_gather_model": round(b_gather / ms_num / 1e6 / peak, 4),
                      "symbolic_GBs": round(b_sym / ms_sym / 1e6, 1),
-                     "traffic": ncu_traffic(("r02c9_esc_key_metrics.txt",), "esc_num_kernel")[0],
-                     "traffic_unit": "DRAM bytes of the numeric kernel per launch, a constant from the committed ncu --set full capture at this size (profiles/r02c9_esc_key_metrics.txt)",
                      "peak_source": peak_src},
         "cpu_baseline": {"value": round(cpu_gf, 3), "unit": "GFLOP/s", "cores": threads, "kind": "port",
                          "sample": f"oracle O6 (spgemm_debug symbolic + numeric + row sort, impl_seq.hpp:23-182), rows dealt to {threads} "
@@ -724,9 +701,8 @@ class near_gpu:
     """with near_gpu(i): allocations made inside (pinned host buffers are placed by first touch) land on the NUMA node of GPU i."""
 
     def __init__(self, dev_index):
-        # opt-in (B200SP_BENCH_NUMA=1): on the B200 boxes measured, the GPU's own node did not help -- at N = 1 the stream-ordered
-        # host-vector step went from 2.00 to 2.73 ms (a node of a sub-NUMA-clustered socket has a fraction of the memory channels),
-        # and at N = 8 the bound is the PCIe uplink two GPUs share (~26 GB/s each way per GPU), not the placement
+        # opt-in (B200SP_BENCH_NUMA=1): the GPU's own node is not always faster -- a node of a sub-NUMA-clustered socket has a
+        # fraction of the memory channels, and with several GPUs a PCIe uplink two GPUs share can be the bound, not the placement
         self.cpus = gpu_local_cpus(dev_index) if os.environ.get("B200SP_BENCH_NUMA") == "1" else None
         self.saved = None
 
@@ -746,6 +722,34 @@ class near_gpu:
             except OSError:
                 pass
         return False
+
+
+# --dump-outputs: bytes each result may take (60 MB in all, under a 64 MB cap), in float64 values plus sampled positions
+DUMP_BYTES = {"y": 24_000_000, "spmm_Y": 16_000_000, "spgemm_row_map": 4_000_000, "spgemm_C": 16_000_000}
+
+
+def dump_outputs(out_dir, name, arrays):
+    """Write what a timed call returned, as float64 .npy files under out_dir.  `arrays` maps file names to tensors of one flat
+    length (row-major).  When they fit in DUMP_BYTES[name] they are written whole, DIR/<key>.npy; otherwise all of them at
+    the same positions, drawn with a fixed seed from the length alone (the same positions for the same arguments, run after
+    run), which go to DIR/<name>_rows.npy.  Positions are gathered on the tensors' device: only the sample is copied."""
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    flat = {k: v.detach().reshape(-1) for k, v in arrays.items()}
+    length = {int(v.numel()) for v in flat.values()}
+    assert len(length) == 1, f"dump {name}: arrays of different lengths"
+    length = length.pop()
+    limit = DUMP_BYTES[name]
+    rows = None
+    if length * 8 * len(flat) > limit:
+        rows = np.unique(np.random.default_rng(0).integers(0, length, limit // (8 * (len(flat) + 1))))
+        np.save(os.path.join(out_dir, f"{name}_rows.npy"), rows.astype(np.float64))
+    for k, v in flat.items():
+        if rows is not None:
+            v = v[torch.from_numpy(rows).to(v.device)]
+        np.save(os.path.join(out_dir, f"{k}.npy"), v.to("cpu", torch.float64).numpy())
+    log(f"[dump] {name}: " + (f"{len(rows)} of {length} positions" if rows is not None else f"all {length} values") + f" -> {out_dir}")
 
 
 def verify_transport(op, x, n_total, world, rank, dev):
@@ -810,6 +814,10 @@ def main():
                          "SpMV kernel itself (fused / multicast), or NCCL after it")
     ap.add_argument("--chunks", type=int, default=8)
     ap.add_argument("--push-ctas", type=int, default=32)
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write what the timed calls computed to DIR/*.npy (float64; a fixed, seeded sample of positions where "
+                         "a result is large; 60 MB at most): y of the last timed step and, with the secondary workloads, SpMM's Y "
+                         "and SpGEMM's C -- so that two builds can be compared output for output")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -838,7 +846,7 @@ def main():
     assert torch.cuda.is_available(), "bench.py needs a CUDA device (no CPU fallback)"
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
-    assert kk._lib.sparse().b200sp_device_ok() == 1, "not a compute-capability 10.x (B200) device"
+    assert kk._lib.sparse().b200sp_device_ok() == 1, "not a compute-capability 9.0 (H100) device"
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
 
@@ -931,10 +939,11 @@ def main():
             sp.spmv(h, "N", 1.0, A, x, 0.0, y)
 
     def step():
+        """One timed step; returns the vector a caller receives: y = A x here, the gathered next x over all ranks for N > 1."""
         if op is not None:
-            op.step(x)
-        else:
-            sp.spmv(h, "N", 1.0, A, x, 0.0, y)
+            return op.step(x)
+        sp.spmv(h, "N", 1.0, A, x, 0.0, y)
+        return y
 
     # ---- parity on this rank's shard: sampled rows vs the oracle's Serial path (O1)
     step()
@@ -997,10 +1006,12 @@ def main():
     sampler.mark_begin()
     e0.record()
     for _ in range(args.steps):
-        step()
+        result = step()
     e1.record()
     torch.cuda.synchronize()
     sampler.mark_end()
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, "y", {"y": result})
     if world > 1:
         dist.barrier()
     launches = lib.b200sp_launch_count() - launches0
@@ -1132,7 +1143,7 @@ def main():
         secondary = []
         for fn in (secondary_spmm, secondary_spgemm):
             try:
-                secondary.append(fn(dev))
+                secondary.append(fn(dev, dump_dir=args.dump_outputs))
             except AssertionError:
                 raise
             except Exception as exc:
@@ -1157,15 +1168,12 @@ def main():
                             f"{n_total} rows, {total_nnz} nnz ({total_nnz / n_total:.1f}/row), alpha=1 beta=0, single vector"
                             + (f", row-partitioned over {world} GPUs, all-gather of y each step ({collective})" if world > 1 else ""),
                 "baseline_config": "configs[1]" if world == 1 else "configs[4]",
-                "cache": "inputs (matrix %.1f GB per GPU) exceed the 126 MB L2; no flush needed" % (nnz * 12 / 1e9),
+                "cache": "inputs (matrix %.1f GB per GPU) exceed the 50 MB L2; no flush needed" % (nnz * 12 / 1e9),
                 "kernel": kernel_name, "parity_max_scaled_err": check, "collective": collective,
                 "statistic": "mean over the timed steps",
             },
             "roofline": {"bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
                          "frac": round(achieved / peak, 4),
-                         "traffic": ncu_traffic()[0] if (world == 1 and args.grid == GRID) else None,
-                         "traffic_unit": "DRAM bytes per launch, a CONSTANT read from the committed ncu --set full capture of this kernel on "
-                                         f"this workload (profiles/{ncu_traffic()[1]}), not measured by this run",
                          "peak_source": peak_src,
                          "kernel_ms": round(kern_ms, 5), "algorithmic_bytes_per_launch": balg},
             "e2e": dict({"value": round(e2e_gflops, 2), "unit": "GFLOP/s", "h2d_bytes_per_step": h2d,

@@ -1,5 +1,5 @@
 /*
- * b200sparse.h -- C ABI of libb200sparse: B200 (sm_100a) SpMV / SpMM / SpGEMM
+ * b200sparse.h -- C ABI of libb200sparse: H100 (sm_90a) SpMV / SpMM / SpGEMM
  * for CrsMatrix data, the drop-in behind Kokkos Kernels' TPL slot for
  * Kokkos::Cuda (SURVEY.md section 8b).
  *
@@ -57,7 +57,7 @@ typedef struct b200sp_spgemm_plan b200sp_spgemm_plan; /* lives in SPGEMMHandle (
 
 const char* b200sp_last_error_string(void);
 int b200sp_version(void);
-/* 1 when a CUDA device of compute capability 10.x is current, else 0. */
+/* 1 when a CUDA device of compute capability 9.x (H100, sm_90a) is current, else 0. */
 int b200sp_device_ok(void);
 
 /* ---- SpMV plan ---------------------------------------------------------- */
@@ -383,7 +383,7 @@ const char* b200sp_bsr_last_kernel(const b200sp_bsr_plan* plan);
 /* The handle's algorithm (sparse/src/KokkosSparse_spmv_handle.hpp: SPMV_BSR_V41 / V42 / TC).  For no-transpose multivector
  * products in double with 2 <= bs <= 16 there are two kernels: the mma.sync m8n8k4 kernel -- what SPMV_BSR_TC selects in the
  * reference (sparse/impl/KokkosSparse_spmv_bsrmatrix_spec.hpp:165-245, ..._impl.hpp:74-459: wmma fragments of the same
- * shape) -- and a scalar one.  DEFAULT picks the tensor-core kernel from 4 columns on (measured 3-14x faster on a B200),
+ * shape) -- and a scalar one.  DEFAULT picks the tensor-core kernel from 4 columns on (several times faster where measured),
  * TENSOR_CORES always, SCALAR never (SPMV_BSR_V41 / V42 requests); every other call takes the default kernels, as the
  * reference falls back when its functor is unavailable. */
 #define B200SP_BSR_ALGO_DEFAULT 0

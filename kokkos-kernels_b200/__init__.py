@@ -1,4 +1,4 @@
-"""kokkos-kernels_b200: B200-native (sm_100a) drop-in for Kokkos Kernels' sparse
+"""kokkos-kernels_b200: H100-native (sm_90a) drop-in for Kokkos Kernels' sparse
 hot path -- KokkosSparse::spmv on CrsMatrix (rank-1, rank-2) and
 spgemm_symbolic / spgemm_numeric.  See DESIGN.md and include/b200sparse.h."""
 from . import _lib, build  # noqa: F401

@@ -133,7 +133,7 @@ def _load(path, api, what):
     if not os.path.exists(path):
         raise ImportError(
             f"{what} not built: {path} is missing. Run `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(there is no CPU or PyTorch fallback for the B200 sparse kernels)."
+            "(there is no CPU or PyTorch fallback for the CUDA sparse kernels)."
         )
     lib = C.CDLL(path)
     for name, (res, args) in api.items():

@@ -1,7 +1,7 @@
 """In-tree build of the native libraries (no JIT cache: the .so files travel
 with the repo snapshot to the GPU box).
 
-  lib/libb200sparse.so   CUDA kernels + C ABI (include/b200sparse.h), sm_100a
+  lib/libb200sparse.so   CUDA kernels + C ABI (include/b200sparse.h), sm_90a (H100)
   lib/libb200matgen.so   host-side synthetic matrix generators (C + OpenMP)
 """
 import os
@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 CU_SOURCES = ["spmv.cu", "spmv64.cu", "spmm.cu", "spgemm.cu", "crs_utils.cu", "bsr.cu", "cg.cu", "gmres.cu", "gs.cu", "gs2.cu", "sptrsv.cu", "crs_io.cpp"]
@@ -63,7 +63,7 @@ def _build_locked(force, verbose):
         for p, cmd in procs:
             if p.wait() != 0:
                 raise RuntimeError("nvcc failed: " + " ".join(cmd))
-        cmd = [_nvcc(), "-shared", "-o", out] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [_nvcc(), "-shared", "-o", out] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         if verbose:
             print("[build]", " ".join(cmd), flush=True)
         subprocess.check_call(cmd)

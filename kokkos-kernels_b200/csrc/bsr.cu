@@ -1,4 +1,4 @@
-// bsr.cu -- BsrMatrix SpMV / SpMM for sm_100a (SURVEY.md section 8f rank 3; DESIGN.md section 7c).
+// bsr.cu -- BsrMatrix SpMV / SpMM for sm_90a (SURVEY.md section 8f rank 3; DESIGN.md section 7c).
 //
 // Replaces, behind the C ABI (include/b200sparse.h, b200sp_bsr_*):
 //   SPMV_BSRMATRIX<Cuda,...>::spmv_bsrmatrix        sparse/impl/KokkosSparse_spmv_bsrmatrix_spec.hpp:165-283
@@ -835,8 +835,8 @@ int bsr_spmv_impl(b200sp_bsr_plan* p, cudaStream_t st, char mode, int mb, int nb
       default: break;
     }
   }
-  // The run-time block size ("walk") tile kernel loses to the row-vector kernel from bs = 5 on (B200, lap27 pattern, 6.9 M blocks:
-  // bs = 5: 1.13 vs 0.84 ms, bs = 8: 5.91 vs 1.90 ms, profiles/r02c6_bsr_big_*.log): it serves bs <= 4 and explicit requests only.
+  // The run-time block size ("walk") tile kernel lost to the row-vector kernel from bs = 5 on when it was tuned (lap27 pattern,
+  // 6.9 M blocks): it serves bs <= 4 and explicit requests only.
   if constexpr (sizeof(S) == 8) {
     // bs 6..16 in double: the tensor-core multivector kernel with ONE column (x contiguous: row stride 1).  Seven of the eight
     // columns of each MMA are zeros, but the MMA is not what bounds the product -- the loads of the blocks are, and the fragment
@@ -896,8 +896,8 @@ int bsr_spmm_impl(b200sp_bsr_plan* p, cudaStream_t st, char mode, int mb, int nb
   if constexpr (sizeof(S) == 8) {
     // SPMV_BSR_TC (spmv_bsrmatrix_spec.hpp:176-245): no-transpose multivector products in double; anything else falls back,
     // as the reference does when its tensor-core functor is unavailable.  B200SP_BSR_MM=tc|scalar overrides the plan.
-    // Default = tensor cores from 4 columns on: measured 2.9x (bs = 4) to 14x (bs = 16) faster than the scalar kernel at k = 16
-    // (profiles/r02c8_bsr_mm.log; differences between the two at the 1e-14 level, far inside the reference's tolerance law).
+    // Default = tensor cores from 4 columns on, several times faster than the scalar kernel at k = 16 when it was tuned
+    // (differences between the two at the 1e-14 level, far inside the reference's tolerance law).
     const char* fm = getenv("B200SP_BSR_MM");
     const bool tc = fm ? !strcmp(fm, "tc") : (p->algo == B200SP_BSR_ALGO_TENSOR_CORES || (p->algo == B200SP_BSR_ALGO_DEFAULT && k >= 4));
     if (tc && bs >= 2 && bs <= 16) {

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers of libb200sparse (sm_100a only).
+// common.cuh -- shared helpers of libb200sparse (sm_90a only).
 #pragma once
 #ifdef B200SP_EMU
 #include "cuda_emu.h"  // tools/emu: CUDA-on-CPU emulation of the kernels (test infrastructure)
@@ -48,8 +48,7 @@ extern std::atomic<long long> g_launches;
 int sm_count();  // SMs of the current device (cached per device)
 // Scratch is allocated with cudaMallocAsync.  The default pool hands unused memory back to the driver at every synchronisation
 // point (release threshold 0), and the symbolic phases synchronise by contract (they return counts to the host): each call would
-// then map its scratch again, which costs more than its kernels (spadd_symbolic: 24-100 ms instead of ~1, profiles/README.md call
-// 27).  Keeps the pool's memory (once per device); called by every scratch allocation scope (DevTmp) and by the plans that own
+// then map its scratch again, which can cost more than its kernels (spadd_symbolic most of all).  Keeps the pool's memory (once per device); called by every scratch allocation scope (DevTmp) and by the plans that own
 // stream-ordered memory.
 void keep_async_pool_memory();
 

@@ -1,4 +1,4 @@
-// crs_utils.cu -- the CrsMatrix utilities either side of the SpMV / SpGEMM hot path on B200
+// crs_utils.cu -- the CrsMatrix utilities either side of the SpMV / SpGEMM hot path on H100
 // (SURVEY.md section 8f): in-row sort, sort-and-merge, sparse add, transpose.
 //
 // Replaces the reference's Kokkos::Cuda legs
@@ -389,8 +389,8 @@ __global__ void __launch_bounds__(256)
 }
 
 // ---- sorted spadd by a GROUP of lanes per row -------------------------------------------------------------------------------
-// One thread per row walks two sorted rows in a serial chain of dependent loads (446 GB/s of the ~36 bytes per entry on a B200,
-// profiles/README.md).  Rows WITHOUT a repeated column inside A_i or inside B_i (any merged matrix) need no walk: the place of an
+// One thread per row walks two sorted rows in a serial chain of dependent loads (latency-bound, far from the HBM roof).
+// Rows WITHOUT a repeated column inside A_i or inside B_i (any merged matrix) need no walk: the place of an
 // entry in C_i is its rank in the union,
 //     pos(a_k) = k + |{b in B_i : b < a_k}| - |{j < k : a_j in B_i}|,      pos(b_k) likewise, written only when b_k is not in A_i,
 // found by one binary search in the other row per entry (the rows were just read: the probes hit L1) and a ballot / popc prefix
@@ -550,9 +550,10 @@ static int spadd_group(int m, int64_t nnzA, int64_t nnzB) {
     const int g = atoi(e);
     if (g == 0 || g == 8 || g == 32) return g;
   }
-  // measured (call 27, 54 + 54 entries per row): 8 lanes 0.41 ms, 32 lanes 0.50 ms, one thread per row 3.49 ms -- more rows in
-  // flight beat wider batches until the rows are long
-  return (double)(nnzA + nnzB) / (double)std::max(m, 1) > 512.0 ? 32 : 8;
+  // tools/bench_spadd.py on an H100 (400 W), 54 + 54 entries per row: numeric 0.60-0.69 ms with 32 lanes, 1.0-1.9 ms with 8,
+  // 6.6-7.3 ms with one thread per row (symbolic 0.39-0.44 vs 0.33-0.40 ms), same bits.  Rows this long fill a warp; shorter
+  // rows keep 8 lanes (more rows in flight), a choice not re-measured on the H100.
+  return (double)(nnzA + nnzB) / (double)std::max(m, 1) >= 64.0 ? 32 : 8;
 }
 
 __global__ void __launch_bounds__(256)

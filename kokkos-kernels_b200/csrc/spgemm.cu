@@ -1,4 +1,4 @@
-// spgemm.cu -- C = A*B on CrsMatrix data for B200 (sm_100a): symbolic + numeric.
+// spgemm.cu -- C = A*B on CrsMatrix data for H100 (sm_90a): symbolic + numeric.
 //
 // Replaces the reference's Kokkos::Cuda SpGEMM legs
 //   native  KokkosSPGEMM symbolic (compression + StructureC hash kernels)
@@ -1244,7 +1244,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
     int esc_cfg = 0;
     if (const char* e = getenv("B200SP_ESC_CFG")) esc_cfg = atoi(e);
     if ((rc = launch_esc_num<S, 32, 8, 9, 32>(st, p, 0, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
-    switch (esc_cfg) {  // bin 1; default measured best (round 2: 18.7 ms on config 4 against 22.7 for <128, 8, 11>)
+    switch (esc_cfg) {  // bin 1; the default was the fastest on config 4 when it was tuned (B200-era, not re-tuned on the H100)
       case 1: rc = launch_esc_num<S, 256, 4, 11, 6>(st, p, 1, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC); break;
       case 2: rc = launch_esc_num<S, 128, 8, 10, 8>(st, p, 1, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC); break;
       case 4: rc = launch_esc_num<S, 256, 4, 10, 5>(st, p, 1, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC); break;
@@ -1525,8 +1525,8 @@ int b200sp_spgemm_symbolic_i32(b200sp_spgemm_plan* p, void* stream, int m, int n
   if (sym_variant >= 3) {
     const int* er = p->esc_rows;
     const int* eo = p->esc_off;
-    // bin 1 (<= 1024 products, config 4's bin): 256 threads x 4 products, 1024 buckets measured best on a B200
-    // (profiles/README.md, round 2); B200SP_ESC_SYM_CFG selects the alternatives for A/B runs
+    // bin 1 (<= 1024 products, config 4's bin): 256 threads x 4 products, 1024 buckets (the best of the alternatives when
+    // the kernel was tuned); B200SP_ESC_SYM_CFG selects the alternatives for A/B runs
     int sym_cfg = 0;
     if (const char* e = getenv("B200SP_ESC_SYM_CFG")) sym_cfg = atoi(e);
     if ((rc = launch_esc_sym<32, 8, 9, 1>(st, eo[1] - eo[0], er + eo[0], rpA, ciA, rpB, ciB, flops, p->cmin, p->cmax, row_nnz))) return rc;

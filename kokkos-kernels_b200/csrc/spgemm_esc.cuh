@@ -240,8 +240,8 @@ __device__ __forceinline__ int esc_stage_row(int a0, int nA, int f, const int* _
 // ---- row pipeline of the persistent kernels -------------------------------------------------------------------------
 // A CTA works through the rows r = blockIdx.x, blockIdx.x + gridDim.x, ... of its bin ("sequence" k = 0, 1, ...).  What a
 // row needs before its first gather is a chain of four dependent global loads (row list -> row header -> A's columns ->
-// B's row pointers): ~3 us that a one-row-per-CTA launch pays once per row (ncu capture r02c6: 40-60 % of all stall
-// samples of both kernels sit on that chain and on the barrier behind it).  The chain therefore runs as a software
+// B's row pointers) that a one-row-per-CTA launch pays once per row (stall sampling put most of both kernels' stalls on
+// that chain and on the barrier behind it).  The chain therefore runs as a software
 // pipeline, one stage per row built: at the top of row k the B row pointers of row k+1, the A entries of row k+2, the
 // header of row k+3 and the list entry of row k+4 are requested, each from what the previous row's requests brought.
 // The requests are cp.async copies global -> shared memory (LDGSTS): no register is held while they are in flight.

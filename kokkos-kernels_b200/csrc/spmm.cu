@@ -734,8 +734,8 @@ static int launch_split(b200sp_spmv_plan* p, cudaStream_t st, int m, int k, int6
     constexpr int VW = 16 / (int)sizeof(S);
     const bool vec_ok = (k % VW == 0) && (ldx % VW == 0) && (ldy % VW == 0) &&
                         ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0 && getenv("B200SP_SPMM_VEC") != nullptr;
-    // opt-in: measured 6.6 ms vs 5.2 ms for the scalar-lane kernel on config 3 (profiles/r01_spmm.md) -- fewer
-    // lanes per chunk means fewer chunks in flight per SM at its register count; kept for the tuning round
+    // opt-in: slower than the scalar-lane kernel on config 3 when it was tuned -- fewer lanes per chunk means fewer
+    // chunks in flight per SM at its register count; kept for the tuning round
     if (vec_ok) {
       int KTv = 1;
       while (KTv * VW < k && KTv < 32) KTv <<= 1;
@@ -1098,7 +1098,7 @@ __global__ void __launch_bounds__(256)
 // group reads a batch of EB consecutive entries with ONE load per lane (adjacent lanes, adjacent entries: the group's
 // EB/KTL loads cover a contiguous 32..64-byte run) and passes them round with shuffles, which run on a different
 // pipe: 1 + 2 * 4/32 wavefronts per nonzero for k = 16 fp32, with EB gathers of X in flight per lane (EB = 4: 40 registers,
-// 6 CTAs per SM; EB = 8: 80 registers, 3 CTAs -- the same number of gathers in flight per SM, and 4 measured faster).
+// 6 CTAs per SM; EB = 8: 80 registers, 3 CTAs -- the same number of gathers in flight per SM, and 4 was faster when tuned).
 template <typename S, int VW, int KTL, int EB /* entries per batch: 4 or 8 */>
 __global__ void __launch_bounds__(256)
     spmm_item_coop_kernel(int n_items, const int4* __restrict__ items, int k, const int* __restrict__ col_idx,
@@ -1227,8 +1227,8 @@ __global__ void __launch_bounds__(256)
 // rows of several pieces: Y(row, :) = beta * Y(row, :) + alpha * (sum of the pieces).  One WARP per row: the lanes are
 // KC columns x 32/KC interleaved piece subsequences (k = 16: lane = (piece parity, column)); a lane adds its subsequence in
 // piece order, a fixed xor tree joins the subsequences -- the order of additions depends on the row alone, so the result is
-// reproducible run to run.  (One thread per (row, column) made the longest row of R-MAT scale 23, 2388 pieces, a 0.5 ms tail:
-// 20 % of the whole product, profiles/r02c9_spmm_launches.csv.)
+// reproducible run to run.  (One thread per (row, column) made the longest row of R-MAT scale 23, 2388 pieces, a tail that
+// took a fifth of the whole product.)
 template <typename S>
 __global__ void __launch_bounds__(256)
     spmm_item_reduce_kernel(int n_multi, const int4* __restrict__ multi, int k, const S* __restrict__ partial, S* __restrict__ Y,
@@ -1294,7 +1294,7 @@ __global__ void __launch_bounds__(256)
 template <typename S>
 static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m, int k, int64_t nnz, const int* row_ptr,
                            const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
-  int LMAX = 64;  // entries per item (B200SP_SPMM_ITEM_LMAX: 16..256); measured on R-MAT scale 23: 32: 3.22, 64: 2.94, 128: 3.36, 256: 3.66 ms
+  int LMAX = 64;  // entries per item (B200SP_SPMM_ITEM_LMAX: 16..256); 64 was the best of 32..256 on R-MAT scale 23 when tuned
   if (const char* e = getenv("B200SP_SPMM_ITEM_LMAX")) {
     const int v = atoi(e);
     if (v >= 16 && v <= MMI_MAXL) LMAX = v;
@@ -1319,7 +1319,7 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   if (grid > 0) {
     static const int coop = [] {  // B200SP_SPMM_ITEM_COOP=0: every lane reads (col, val) itself (the first item kernel); 4 (default) | 8: batch
       const char* e = getenv("B200SP_SPMM_ITEM_COOP");
-      return e && e[0] == '0' ? 0 : (e && e[0] == '8' ? 8 : 4);  // measured on R-MAT scale 23 x 16: 2.27 (4), 2.49 (8), 2.95 ms (0)
+      return e && e[0] == '0' ? 0 : (e && e[0] == '8' ? 8 : 4);  // 4 was the fastest of 0 / 4 / 8 on R-MAT scale 23 x 16 when tuned
     }();
 #define B200SP_MMI(V, L)                                                                                                   \
   case L:                                                                                                                  \
@@ -1355,8 +1355,8 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   return B200SP_OK;
 }
 
-// which rank-2 kernel: 0 = row per group, 1 = nnz-split, 2 = tile, 3 = tile with 16-byte X loads (default:
-// measured 1.74 ms vs 4.01 ms for the split kernel on R-MAT scale 21 x 16 columns, profiles/README.md).
+// which rank-2 kernel: 0 = row per group, 1 = nnz-split, 2 = tile, 3 = tile with 16-byte X loads (default: about twice
+// as fast as the split kernel on R-MAT scale 21 x 16 columns when it was tuned).
 // B200SP_SPMM_KERNEL=row|split|tile|tilev overrides.
 static int mm_kernel_choice(b200sp_spmv_plan* p) {
   if (!p) return 0;  // the others need a plan (chunk table / tile analysis)

@@ -1,4 +1,4 @@
-// spmv.cu -- rank-1 CrsMatrix SpMV for B200 (sm_100a): y = beta*y + alpha*op(A)*x.
+// spmv.cu -- rank-1 CrsMatrix SpMV for H100 (sm_90a): y = beta*y + alpha*op(A)*x.
 //
 // Replaces the reference's Kokkos::Cuda SpMV legs:
 //   native  SPMV_Functor team kernel   sparse/impl/KokkosSparse_spmv_impl.hpp:134-165,337-379
@@ -47,11 +47,11 @@ int sm_count() {
   static std::once_flag once;
   std::call_once(once, [] { memset(cached, 0, sizeof(cached)); });
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -473,9 +473,9 @@ __global__ void __launch_bounds__((NW + 1) * 32)
       }
       __syncwarp();
       if (forward) {
-        // Software-pipelined by one tile: the values of the tile that just left are only LOADED here (L2, ~0.7 us) and stored
-        // when the next tile comes round -- with ~1.2 us per tile and CTA on config 2 a load-then-store in one go made the
-        // producer warp the bottleneck of the kernel (+12 % on one GPU, profiles/r02c20_forward.log).  Tiles of more than 64
+        // Software-pipelined by one tile: the values of the tile that just left are only LOADED here (from L2) and stored
+        // when the next tile comes round -- a load-then-store in one go made the producer warp the bottleneck of the
+        // kernel.  Tiles of more than 64
         // rows are forwarded in one go.
         S* dst = static_cast<S*>(ex.p[0]);
         if (fr1 > fr0) {
@@ -594,8 +594,8 @@ static constexpr int kNumCfgs = sizeof(kCfgs) / sizeof(kCfgs[0]);
 
 // ---------------------------------------------------------------------------
 // Push a finished piece of y to the NVSwitch multicast mapping of the next-x buffer with 16-byte stores
-// (on sm_100 a plain st.global to a multicast address IS multimem.st: the switch replicates it into every
-// GPU's copy).  A few CTAs are enough (80 MB per step); they co-reside with the persistent SpMV CTAs.
+// (on sm_90, as the SASS of this kernel shows, multimem.st to a multicast address is a plain STG: the switch replicates
+// it into every GPU's copy, so store_y and the forwarding kernel write the multicast mapping with plain stores).  A few CTAs are enough (80 MB per step); they co-reside with the persistent SpMV CTAs.
 // ---------------------------------------------------------------------------
 // 16-byte store to a multicast address: multimem.st (the switch writes the value into every GPU's copy)
 __device__ __forceinline__ void mc_store16(double2* dst, const double2& v) {
@@ -971,7 +971,7 @@ int spmv_lanes_per_row(int64_t m, int64_t nnz);
 static int pick_lpr(int m, int64_t nnz) { return spmv_lanes_per_row(m, nnz); }
 int spmv_lanes_per_row(int64_t m, int64_t nnz) {  // also used by spmv64.cu: one choice for all windows of a matrix
   const double avg = m > 0 ? (double)nnz / (double)m : 0.0;
-  // measured on B200 (profiles/r01_tune_spmv.csv): fewer lanes per row win until rows get long
+  // tuned by tools/tune_spmv.py: fewer lanes per row win until rows get long
   if (avg <= 8.0) return 2;
   if (avg <= 96.0) return 4;
   if (avg <= 384.0) return 8;
@@ -1267,7 +1267,7 @@ int b200sp_device_ok(void) {
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   int major = 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }
 
 int b200sp_spmv_plan_create(b200sp_spmv_plan** plan, int algo) {

@@ -12,8 +12,8 @@
 //             loop of the oracle (oracle/kk_oracle_sptrsv.c: okk_sptrsv), so the result is bit-identical to it whatever the level
 //             schedule is.  The lanes of a group load a batch of the row's (column, value, x[column]) and form the products IN
 //             PARALLEL (each product is rounded on its own either way); only the chain of subtractions runs in order, on values
-//             passed by shuffle.  One thread per row (the first version, 17 us per level on the 27-point operator,
-//             profiles/README.md call 24) spent its time in ~14 serial rounds of dependent loads per row; a group needs three
+//             passed by shuffle.  One thread per row (the first version) spends its time in ~14 serial rounds of dependent
+//             loads per row on the 27-point operator; a group needs three
 //             (row record -> columns / values -> x).  The row record (row, begin, end) is stored with the level lists.
 //             The Gauss-Seidel form solves with the lower (upper) triangle of a general matrix: the entries on the other side and
 //             the ghost columns are skipped (`filter`), no copy of the triangle is made; with a caller-supplied inverse diagonal

@@ -3,7 +3,7 @@
 // Install: copy this directory into kokkos-kernels/sparse/tpls/, add
 // KOKKOSKERNELS_ENABLE_TPL_B200SPARSE to KokkosKernels_config.h.in, include the
 // *_avail.hpp / *_decl.hpp files next to the cuSPARSE ones (INTEGRATION.md lists
-// the exact lines), link -lb200sparse.  The B200 specialisations occupy the slot
+// the exact lines), link -lb200sparse.  The TPL_B200 specialisations occupy the slot
 // of the cuSPARSE ones (same template arguments), so build with
 // KokkosKernels_ENABLE_TPL_CUSPARSE=OFF.
 #ifndef KOKKOSSPARSE_B200_UTILS_HPP_

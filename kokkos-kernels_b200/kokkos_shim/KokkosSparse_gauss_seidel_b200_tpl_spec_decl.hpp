@@ -80,7 +80,6 @@ inline int b200_gs_kind(KernelHandle* handle) {  // 0 point, 1 two-stage (inner 
   template <>                                                                                                          \
   struct GAUSS_SEIDEL_SYMBOLIC<Kokkos::Cuda, KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE), KOKKOSSPARSE_B200_IV(const int, MEMSPACE), \
                                KOKKOSSPARSE_B200_IV(const int, MEMSPACE), true, ETI_AVAIL> {                           \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     using KernelHandle = KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE);                                                       \
     using c_int_view_t = KOKKOSSPARSE_B200_IV(const int, MEMSPACE);                                                    \
     static void gauss_seidel_symbolic(const Kokkos::Cuda& exec, KernelHandle* handle, typename KernelHandle::const_nnz_lno_t num_rows, \
@@ -114,7 +113,6 @@ inline int b200_gs_kind(KernelHandle* handle) {  // 0 point, 1 two-stage (inner 
   struct GAUSS_SEIDEL_NUMERIC<Kokkos::Cuda, KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE), KokkosSparse::SparseMatrixFormat::CRS, \
                               KOKKOSSPARSE_B200_IV(const int, MEMSPACE), KOKKOSSPARSE_B200_IV(const int, MEMSPACE),   \
                               KOKKOSSPARSE_B200_IV(const SCALAR, MEMSPACE), true, ETI_AVAIL> {                         \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     using KernelHandle    = KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE);                                                    \
     using c_int_view_t    = KOKKOSSPARSE_B200_IV(const int, MEMSPACE);                                                 \
     using c_scalar_view_t = KOKKOSSPARSE_B200_IV(const SCALAR, MEMSPACE);                                              \
@@ -154,7 +152,6 @@ inline int b200_gs_kind(KernelHandle* handle) {  // 0 point, 1 two-stage (inner 
                             KOKKOSSPARSE_B200_IV(const int, MEMSPACE), KOKKOSSPARSE_B200_IV(const int, MEMSPACE),     \
                             KOKKOSSPARSE_B200_IV(const SCALAR, MEMSPACE), KOKKOSSPARSE_B200_MV(SCALAR, MEMSPACE),     \
                             KOKKOSSPARSE_B200_MV(const SCALAR, MEMSPACE), true, ETI_AVAIL> {                           \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     using KernelHandle    = KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE);                                                    \
     using c_int_view_t    = KOKKOSSPARSE_B200_IV(const int, MEMSPACE);                                                 \
     using c_scalar_view_t = KOKKOSSPARSE_B200_IV(const SCALAR, MEMSPACE);                                              \

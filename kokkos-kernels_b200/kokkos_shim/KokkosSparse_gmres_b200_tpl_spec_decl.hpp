@@ -40,7 +40,6 @@ inline int b200_call_gmres_bsr(b200sp_bsr_plan* p, void* s, int mb, int64_t nnzb
   struct GMRES<KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE), const SCALAR, const int, Kokkos::Device<Kokkos::Cuda, MEMSPACE>, \
                Kokkos::MemoryTraits<Kokkos::Unmanaged>, const int, KOKKOSSPARSE_B200_GMRES_VEC(const SCALAR, MEMSPACE), \
                KOKKOSSPARSE_B200_GMRES_VEC(SCALAR, MEMSPACE), true, ETI_AVAIL> {                                       \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     using KernelHandle = KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE);                                                       \
     using device_type  = Kokkos::Device<Kokkos::Cuda, MEMSPACE>;                                                       \
     using AMatrix  = CrsMatrix<const SCALAR, const int, device_type, Kokkos::MemoryTraits<Kokkos::Unmanaged>, const int>; \

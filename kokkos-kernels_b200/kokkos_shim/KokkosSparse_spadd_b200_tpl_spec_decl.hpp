@@ -34,7 +34,6 @@ inline int b200_call_spadd_numeric(b200sp_spadd_plan* p, void* s, int m, int n, 
   struct SPADD_SYMBOLIC<Kokkos::Cuda, KOKKOSSPARSE_B200_AKH(SCALAR), KOKKOSSPARSE_B200_AV(const int),                  \
                         KOKKOSSPARSE_B200_AV(const int), KOKKOSSPARSE_B200_AV(const int),                              \
                         KOKKOSSPARSE_B200_AV(const int), KOKKOSSPARSE_B200_AV(int), true, ETI_SPEC_AVAIL> {            \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     using kernelhandle_t          = KOKKOSSPARSE_B200_AKH(SCALAR);                                                     \
     using rowmap_view_t           = KOKKOSSPARSE_B200_AV(const int);                                                   \
     using non_const_rowmap_view_t = KOKKOSSPARSE_B200_AV(int);                                                         \
@@ -67,7 +66,6 @@ inline int b200_call_spadd_numeric(b200sp_spadd_plan* p, void* s, int m, int n, 
                        KOKKOSSPARSE_B200_AV(const int), KOKKOSSPARSE_B200_AV(const int),                               \
                        KOKKOSSPARSE_B200_AV(const SCALAR), KOKKOSSPARSE_B200_AV(const int), KOKKOSSPARSE_B200_AV(int), \
                        KOKKOSSPARSE_B200_AV(SCALAR), true, ETI_SPEC_AVAIL> {                                           \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     using kernelhandle_t           = KOKKOSSPARSE_B200_AKH(SCALAR);                                                    \
     using rowmap_view_t            = KOKKOSSPARSE_B200_AV(const int);                                                  \
     using colidx_view_t            = KOKKOSSPARSE_B200_AV(const int);                                                  \

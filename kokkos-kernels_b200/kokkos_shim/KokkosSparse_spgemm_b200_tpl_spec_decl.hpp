@@ -67,7 +67,6 @@ void spgemm_numeric_b200(SpgemmHandle* sh, int m, int n, int k, const CIV& rowma
     using KernelHandle = KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE);                                                       \
     using c_int_view_t = KOKKOSSPARSE_B200_IV(const int, MEMSPACE);                                                    \
     using int_view_t   = KOKKOSSPARSE_B200_IV(int, MEMSPACE);                                                          \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     static void spgemm_symbolic(KernelHandle* handle, typename KernelHandle::nnz_lno_t m,                              \
                                 typename KernelHandle::nnz_lno_t n, typename KernelHandle::nnz_lno_t k,                \
                                 c_int_view_t row_mapA, c_int_view_t entriesA, bool, c_int_view_t row_mapB,             \
@@ -89,7 +88,6 @@ void spgemm_numeric_b200(SpgemmHandle* sh, int m, int n, int k, const CIV& rowma
     using int_view_t      = KOKKOSSPARSE_B200_IV(int, MEMSPACE);                                                       \
     using c_scalar_view_t = KOKKOSSPARSE_B200_IV(const SCALAR, MEMSPACE);                                              \
     using scalar_view_t   = KOKKOSSPARSE_B200_IV(SCALAR, MEMSPACE);                                                    \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     static void spgemm_numeric(KernelHandle* handle, typename KernelHandle::nnz_lno_t m,                               \
                                typename KernelHandle::nnz_lno_t n, typename KernelHandle::nnz_lno_t k,                 \
                                c_int_view_t row_mapA, c_int_view_t entriesA, c_scalar_view_t valuesA, bool,            \

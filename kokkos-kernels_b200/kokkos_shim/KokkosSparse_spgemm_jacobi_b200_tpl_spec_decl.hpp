@@ -31,7 +31,6 @@ inline int b200_call_jacobi(b200sp_spgemm_plan* p, void* s, int m, int n, int k,
                        KOKKOSSPARSE_B200_IV(const SCALAR, MEMSPACE), KOKKOSSPARSE_B200_IV(int, MEMSPACE),              \
                        KOKKOSSPARSE_B200_IV(int, MEMSPACE), KOKKOSSPARSE_B200_IV(SCALAR, MEMSPACE),                    \
                        KOKKOSSPARSE_B200_DINV(SCALAR, MEMSPACE), true, ETI_AVAIL> {                                    \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     using KernelHandle    = KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE);                                                    \
     using c_int_view_t    = KOKKOSSPARSE_B200_IV(const int, MEMSPACE);                                                 \
     using int_view_t      = KOKKOSSPARSE_B200_IV(int, MEMSPACE);                                                       \

@@ -61,7 +61,6 @@ inline int b200_call_spmm(b200sp_spmv_plan* p, void* s, char mode, int m, int n,
                                  Kokkos::MemoryTraits<Kokkos::Unmanaged | Kokkos::RandomAccess>>;                    \
     using YVector = Kokkos::View<SCALAR*, LAYOUT, device_type, Kokkos::MemoryTraits<Kokkos::Unmanaged>>;             \
     using coefficient_type = typename YVector::non_const_value_type;                                                 \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */       \
     static void spmv(const Kokkos::Cuda& exec, Handle* handle, const char mode[], const coefficient_type& alpha,     \
                      const AMatrix& A, const XVector& x, const coefficient_type& beta, const YVector& y) {           \
       Kokkos::Profiling::pushRegion("KokkosSparse::spmv[TPL_B200," + Kokkos::ArithTraits<SCALAR>::name() + "]");     \
@@ -90,7 +89,6 @@ inline int b200_call_spmm(b200sp_spmv_plan* p, void* s, char mode, int m, int n,
                                  Kokkos::MemoryTraits<Kokkos::Unmanaged | Kokkos::RandomAccess>>;                    \
     using YVector = Kokkos::View<SCALAR**, YL, device_type, Kokkos::MemoryTraits<Kokkos::Unmanaged>>;                \
     using coefficient_type = typename YVector::non_const_value_type;                                                 \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */       \
     static void spmv_mv(const Kokkos::Cuda& exec, Handle* handle, const char mode[], const coefficient_type& alpha,  \
                         const AMatrix& A, const XVector& X, const coefficient_type& beta, const YVector& Y) {        \
       Kokkos::Profiling::pushRegion("KokkosSparse::spmv[TPL_B200," + Kokkos::ArithTraits<SCALAR>::name() + "]");     \
@@ -173,7 +171,6 @@ inline int b200_call_spmm64(b200sp_spmv64_plan* p, void* s, char mode, int64_t m
                                  Kokkos::MemoryTraits<Kokkos::Unmanaged | Kokkos::RandomAccess>>;                    \
     using YVector = Kokkos::View<SCALAR*, LAYOUT, device_type, Kokkos::MemoryTraits<Kokkos::Unmanaged>>;             \
     using coefficient_type = typename YVector::non_const_value_type;                                                 \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */       \
     static void spmv(const Kokkos::Cuda& exec, Handle* handle, const char mode[], const coefficient_type& alpha,     \
                      const AMatrix& A, const XVector& x, const coefficient_type& beta, const YVector& y) {           \
       Kokkos::Profiling::pushRegion("KokkosSparse::spmv[TPL_B200," + Kokkos::ArithTraits<SCALAR>::name() + "]");     \
@@ -204,7 +201,6 @@ inline int b200_call_spmm64(b200sp_spmv64_plan* p, void* s, char mode, int64_t m
                                  Kokkos::MemoryTraits<Kokkos::Unmanaged | Kokkos::RandomAccess>>;                    \
     using YVector = Kokkos::View<SCALAR**, YL, device_type, Kokkos::MemoryTraits<Kokkos::Unmanaged>>;                \
     using coefficient_type = typename YVector::non_const_value_type;                                                 \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */       \
     static void spmv_mv(const Kokkos::Cuda& exec, Handle* handle, const char mode[], const coefficient_type& alpha,  \
                         const AMatrix& A, const XVector& X, const coefficient_type& beta, const YVector& Y) {        \
       Kokkos::Profiling::pushRegion("KokkosSparse::spmv[TPL_B200," + Kokkos::ArithTraits<SCALAR>::name() + "]");     \

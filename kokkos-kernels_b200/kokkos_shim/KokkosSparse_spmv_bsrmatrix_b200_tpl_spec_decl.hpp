@@ -69,7 +69,6 @@ inline int b200_call_bsr_spmm(b200sp_bsr_plan* p, void* s, char mode, int mb, in
                    Kokkos::MemoryTraits<Kokkos::Unmanaged | Kokkos::RandomAccess>>,                                   \
       Kokkos::View<SCALAR*, LAYOUT, Kokkos::Device<Kokkos::Cuda, MEMSPACE>, Kokkos::MemoryTraits<Kokkos::Unmanaged>>, \
       true> { /* eti: the default argument, as the cuSPARSE specialisation leaves it (tpl_spec_decl.hpp:470) */     \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */        \
     using device_type = Kokkos::Device<Kokkos::Cuda, MEMSPACE>;                                                       \
     using Handle      = SPMVHandleImpl<Kokkos::Cuda, MEMSPACE, SCALAR, int, int>;                                     \
     using AMatrix     = ::KokkosSparse::Experimental::BsrMatrix<SCALAR const, int const, device_type,                 \
@@ -98,7 +97,6 @@ inline int b200_call_bsr_spmm(b200sp_bsr_plan* p, void* s, char mode, int mb, in
                    Kokkos::MemoryTraits<Kokkos::Unmanaged | Kokkos::RandomAccess>>,                                   \
       Kokkos::View<SCALAR**, LAYOUT, Kokkos::Device<Kokkos::Cuda, MEMSPACE>, Kokkos::MemoryTraits<Kokkos::Unmanaged>>, \
       false, true> { /* eti: the default argument */                                                                  \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */        \
     using device_type = Kokkos::Device<Kokkos::Cuda, MEMSPACE>;                                                       \
     using Handle      = SPMVHandleImpl<Kokkos::Cuda, MEMSPACE, SCALAR, int, int>;                                     \
     using AMatrix     = ::KokkosSparse::Experimental::BsrMatrix<SCALAR const, int const, device_type,                 \

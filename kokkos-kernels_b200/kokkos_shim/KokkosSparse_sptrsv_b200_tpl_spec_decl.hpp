@@ -28,7 +28,6 @@ inline int b200_call_sptrsv_solve(b200sp_sptrsv_plan* p, void* s, int n, const i
   template <>                                                                                                          \
   struct SPTRSV_SYMBOLIC<Kokkos::Cuda, KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE), KOKKOSSPARSE_B200_RAV(const int, MEMSPACE), \
                          KOKKOSSPARSE_B200_RAV(const int, MEMSPACE), true, ETI_AVAIL> {                                \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */         \
     using KernelHandle = KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE);                                                       \
     using c_int_view_t = KOKKOSSPARSE_B200_RAV(const int, MEMSPACE);                                                   \
     static void sptrsv_symbolic(const Kokkos::Cuda& space, KernelHandle* handle, const c_int_view_t row_map,           \
@@ -45,7 +44,6 @@ inline int b200_call_sptrsv_solve(b200sp_sptrsv_plan* p, void* s, int n, const i
   struct SPTRSV_SOLVE<Kokkos::Cuda, KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE), KOKKOSSPARSE_B200_RAV(const int, MEMSPACE), \
                       KOKKOSSPARSE_B200_RAV(const int, MEMSPACE), KOKKOSSPARSE_B200_RAV(const SCALAR, MEMSPACE),       \
                       KOKKOSSPARSE_B200_RAV(const SCALAR, MEMSPACE), KOKKOSSPARSE_B200_IV(SCALAR, MEMSPACE), true, ETI_AVAIL> { \
-    enum : bool { is_b200sparse = true }; /* tests/shim_ref: proves this specialisation is the one selected */                  \
     using KernelHandle    = KOKKOSSPARSE_B200_KH(SCALAR, MEMSPACE);                                                    \
     using c_int_view_t    = KOKKOSSPARSE_B200_RAV(const int, MEMSPACE);                                                \
     using c_scalar_view_t = KOKKOSSPARSE_B200_RAV(const SCALAR, MEMSPACE);                                             \

@@ -10,9 +10,9 @@ to the single-GPU SpMV (same kernel, same per-row order).
 
 modes: "pipelined" (default), "fused" (P2P stores issued by the SpMV kernel itself,
 b200sp_spmv_scatter_f64_i32), "multicast" (as fused, but ONE store per y value to the NVSwitch multicast
-address of the symmetric buffer -- on sm_100 multimem.st is a plain st.global to a multicast mapping, the
+address of the symmetric buffer -- on sm_90 multimem.st is a plain st.global to a multicast mapping, the
 switch replicates it into all 8 copies, so every GPU sends its 80 MB once instead of 7 times; falls back
-to "fused" when the symmetric-memory handle has no multicast pointer; first measurements: round 2),
+to "fused" when the symmetric-memory handle has no multicast pointer; not yet measured on H100 machines),
 "pipelined_mc" (pieces like "pipelined", but each finished piece is pushed ONCE to the multicast address by a
 small SM kernel with 16-byte stores, b200sp_multicast_push, on one communication stream; falls back to
 "pipelined" without a multicast pointer),

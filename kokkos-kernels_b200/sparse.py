@@ -810,7 +810,7 @@ class KokkosKernelsHandle:
 
 def spgemm_symbolic_views(kh, m, n, k, row_mapA, entriesA, transposeA, row_mapB, entriesB, transposeB, row_mapC,
                           computeRowptrs=False):
-    """View-level spgemm_symbolic (sparse/src/KokkosSparse_spgemm_symbolic.hpp:25-182).  The B200
+    """View-level spgemm_symbolic (sparse/src/KokkosSparse_spgemm_symbolic.hpp:25-182).  The CUDA
     path always fills row_mapC (computeRowptrs is implied)."""
     if transposeA or transposeB:  # :61-65
         raise B200SparseError("KokkosSparse::spgemm_symbolic: transposing A or B is not supported")

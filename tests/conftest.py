@@ -10,8 +10,8 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    config.addinivalue_line("markers", "gpu_next: GPU tests of code that has not had its first run on a B200 yet "
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
+    config.addinivalue_line("markers", "gpu_next: GPU tests of code that has not had its first run on an H100 yet "
                                        "(validated with tools/gpu_check first, then promoted to `gpu`)")
 
 
@@ -78,5 +78,5 @@ def cuda():
         pytest.skip("no CUDA device")
     import kokkos_kernels_b200 as kk
 
-    assert kk._lib.sparse().b200sp_device_ok() == 1, "libb200sparse needs a compute-capability 10.x device"
+    assert kk._lib.sparse().b200sp_device_ok() == 1, "libb200sparse needs a compute-capability 9.0 (H100) device"
     return torch.device("cuda:0")

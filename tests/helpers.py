@@ -1,8 +1,52 @@
 """Shared test helpers: inputs as the reference's tests define them, and its
 acceptance laws."""
+import hashlib
+import json
+import os
+
 import numpy as np
 
 from kokkos_kernels_b200 import matgen
+
+REFERENCE_DIGESTS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_digests.json")
+
+
+class ReferenceOutputs:
+    """Arrays a test requires to be, bit for bit, what the reference's own code returns on the same inputs.  What the
+    reference returned is stored as one SHA-256 digest per test under `key` in tests/golden/reference_digests.json, so the
+    comparison needs no reference build: add() every result in order, then check().  With KKREF_RECORD=1 (and oracle/_ref
+    built from the reference tree, see oracle/Makefile) add() also runs `ref()`, the reference's code, compares its arrays
+    with the results directly, and check() records the digest.  Without KKREF_RECORD the reference library is never called,
+    even where oracle/_ref exists: the digests stand for its outputs, bit for bit."""
+
+    def __init__(self, key):
+        self.key = key
+        self.hash = hashlib.sha256()
+        self.record = os.environ.get("KKREF_RECORD") == "1"
+
+    def add(self, got, ref, what=""):
+        if self.record:
+            want = ref()
+            assert len(want) == len(got), (self.key, what)
+            for a, b in zip(got, want):
+                a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
+                assert a.dtype == b.dtype and a.shape == b.shape and a.tobytes() == b.tobytes(), (self.key, what)
+        for a in got:
+            a = np.ascontiguousarray(a)
+            self.hash.update(f"{a.dtype.str}{a.shape}".encode())
+            self.hash.update(a.tobytes())
+
+    def check(self):
+        digest = self.hash.hexdigest()
+        stored = json.load(open(REFERENCE_DIGESTS)) if os.path.exists(REFERENCE_DIGESTS) else {}
+        if self.record:
+            stored[self.key] = digest
+            with open(REFERENCE_DIGESTS, "w") as f:
+                json.dump(stored, f, indent=0, sort_keys=True)
+                f.write("\n")
+            return
+        assert self.key in stored, f"no stored reference output for {self.key}"
+        assert digest == stored[self.key], f"{self.key}: differs from the reference's output"
 
 
 def kk_matrix(nrows, ncols, nnz, variance, bandwidth, dtype=np.float64, seed=13718, lo=0.0, hi=1.0, sort=False, oracle=None):

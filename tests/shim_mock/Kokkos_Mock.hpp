@@ -1,5 +1,5 @@
 // Kokkos_Mock.hpp -- the smallest stand-in for the Kokkos / Kokkos Kernels declarations that the
-// B200 shim headers (kokkos-kernels_b200/kokkos_shim/*.hpp) specialise, so the shim can be
+// TPL_B200 shim headers (kokkos-kernels_b200/kokkos_shim/*.hpp) specialise, so the shim can be
 // compiled and RUN without Kokkos (>= 4.6.02 is not available in this image, SURVEY.md 8c).
 // Names, template parameter lists and member names follow the reference:
 //   SPMVHandleImpl / TPL_SpMV_Data   sparse/src/KokkosSparse_spmv_handle.hpp:90-107,217-253
@@ -178,7 +178,6 @@ struct SPMVHandleImpl {
   TPL_SpMV_Data<ExecutionSpace>* tpl_rank2 = nullptr;
 };
 
-#ifndef B200_SHIM_REFERENCE_SPEC  // tests/shim_ref: the reference's own declarations of these are included in place instead
 template <class ExecutionSpace, class Handle, class AMatrix, class XVector, class YVector>
 struct spmv_tpl_spec_avail {
   enum : bool { value = false };
@@ -194,9 +193,7 @@ template <class ExecutionSpace, class Handle, class AMatrix, class XVector, clas
           bool tpl_spec_avail = spmv_mv_tpl_spec_avail<ExecutionSpace, Handle, AMatrix, XVector, YVector>::value>
 struct SPMV_MV;
 
-#endif  // B200_SHIM_REFERENCE_SPEC
 
-#ifndef B200_SHIM_REFERENCE_SPEC
 // sparse/tpls/KokkosSparse_spmv_bsrmatrix_tpl_spec_avail.hpp:27-30,121-124 and
 // sparse/impl/KokkosSparse_spmv_bsrmatrix_spec.hpp:89-112 (eti always true in the mock, as in a library build)
 template <class ExecutionSpace, class Handle, class AMatrix, class XVector, class YVector>
@@ -215,7 +212,6 @@ template <class ExecutionSpace, class Handle, class AMatrix, class XVector, clas
           bool tpl_spec_avail = spmv_mv_bsrmatrix_tpl_spec_avail<ExecutionSpace, Handle, AMatrix, XVector, YVector>::value,
           bool eti_spec_avail = true>
 struct SPMV_MV_BSRMATRIX;
-#endif  // B200_SHIM_REFERENCE_SPEC
 }  // namespace Impl
 }  // namespace KokkosSparse
 
@@ -482,7 +478,6 @@ struct KokkosKernelsHandle {
 
 namespace KokkosSparse {
 namespace Impl {
-#ifndef B200_SHIM_REFERENCE_SPEC
 template <class KH, class a_r, class a_e, class b_r, class b_e, class c_r>
 struct spgemm_symbolic_tpl_spec_avail {
   enum : bool { value = false };
@@ -491,8 +486,6 @@ template <class KH, class a_r, class a_e, class a_v, class b_r, class b_e, class
 struct spgemm_numeric_tpl_spec_avail {
   enum : bool { value = false };
 };
-#endif  // B200_SHIM_REFERENCE_SPEC
-#ifndef B200_SHIM_REFERENCE_SPEC
 // sparse/tpls/KokkosSparse_sptrsv_{symbolic,solve}_tpl_spec_avail.hpp, sparse/impl/KokkosSparse_sptrsv_{symbolic,solve}_spec.hpp
 template <class KH, class a_r, class a_e>
 struct sptrsv_symbolic_tpl_spec_avail {
@@ -537,7 +530,7 @@ template <class Exec, class KH, KokkosSparse::SparseMatrixFormat format, class a
           bool tpl = gauss_seidel_apply_tpl_spec_avail<KH, a_r, a_e, a_v, x_v, y_v>::value, bool eti = true>
 struct GAUSS_SEIDEL_APPLY;
 // the native bodies (tpl = false; sparse/impl/KokkosSparse_gauss_seidel_spec.hpp:153-262): stand-ins that count their calls -- the
-// B200 specialisations forward what they do not serve (cluster Gauss-Seidel)
+// TPL_B200 specialisations forward what they do not serve (cluster Gauss-Seidel)
 inline int& mock_native_gs_calls() {
   static int n = 0;
   return n;
@@ -572,20 +565,16 @@ struct spgemm_jacobi_tpl_spec_avail {
 template <class KH, class a_r, class a_e, class a_v, class b_r, class b_e, class b_v, class c_r, class c_e, class c_v, class dinv_v,
           bool tpl = spgemm_jacobi_tpl_spec_avail<KH, a_r, a_e, a_v, b_r, b_e, b_v, c_r, c_e, c_v, dinv_v>::value, bool eti = true>
 struct SPGEMM_JACOBI;
-#endif  // B200_SHIM_REFERENCE_SPEC
-#ifndef B200_SHIM_REFERENCE_SPEC
 template <class KH, class a_r, class a_e, class b_r, class b_e, class c_r, bool tpl, bool eti>
 struct SPGEMM_SYMBOLIC;
 template <class KH, class a_r, class a_e, class a_v, class b_r, class b_e, class b_v, class c_r, class c_e, class c_v,
           bool tpl, bool eti>
 struct SPGEMM_NUMERIC;
-#endif  // B200_SHIM_REFERENCE_SPEC
 }  // namespace Impl
 }  // namespace KokkosSparse
 
 namespace KokkosSparse {
 namespace Impl {
-#ifndef B200_SHIM_REFERENCE_SPEC
 template <class ExecSpace, class KH, class a_r, class a_e, class b_r, class b_e, class c_r>
 struct spadd_symbolic_tpl_spec_avail {
   enum : bool { value = false };
@@ -600,6 +589,5 @@ struct SPADD_SYMBOLIC;
 template <class ExecSpace, class KH, class a_r, class a_e, class a_v, class b_r, class b_e, class b_v, class c_r, class c_e,
           class c_v, bool tpl, bool eti>
 struct SPADD_NUMERIC;
-#endif  // B200_SHIM_REFERENCE_SPEC
 }  // namespace Impl
 }  // namespace KokkosSparse

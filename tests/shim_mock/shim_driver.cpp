@@ -1,4 +1,4 @@
-// shim_driver.cpp -- instantiates the B200 TPL specialisations exactly as KokkosSparse::spmv /
+// shim_driver.cpp -- instantiates the TPL_B200 specialisations exactly as KokkosSparse::spmv /
 // spgemm_symbolic / spgemm_numeric would (Kokkos_Mock.hpp standing in for Kokkos), runs them on the
 // GPU through libb200sparse and checks the results on the host.  Exit code 0 = all checks passed.
 #define KOKKOSKERNELS_ENABLE_TPL_B200SPARSE
@@ -78,7 +78,7 @@ T* to_dev(const std::vector<T>& h) {
 }
 
 int main(int argc, char** argv) {
-  // --bsr: also run the BsrMatrix specialisations (not part of the default run until their first pass on a B200)
+  // --bsr: also run the BsrMatrix specialisations (not part of the default run)
   bool with_bsr = false, with_jacobi = false, with_gs = false, with_gmres = false;  // --jacobi, --gs: likewise for spgemm_jacobi / Gauss-Seidel
   int n_arg = 50000;                                                                 // --n N: rows of the test matrix (the CPU emulation runs a smaller one)
   bool with_sptrsv = false;                                                          // --sptrsv: SPTRSV_SYMBOLIC / SPTRSV_SOLVE

@@ -2,7 +2,7 @@
 operation, run under the CPU emulation with EVERY array (inputs, outputs, the library's temporaries) fenced by
 inaccessible pages, results compared with the oracle.  A kernel that reads or writes one element outside an array
 faults (the seed is printed before each case); on a GPU the same access is usually silent.  Longer campaigns:
-`python tools/emu/fuzz_guard.py --seeds 0:3000` (profiles/README.md records the ones run)."""
+`python tools/emu/fuzz_guard.py --seeds 0:3000`."""
 import os
 import subprocess
 import sys

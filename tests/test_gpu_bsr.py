@@ -8,7 +8,6 @@ import torch
 
 from bsr_cases import BLOCK_SIZES, COEFS_ALPHA, COEFS_BETA, PRIME_CASE, SHAPES, bsr_random, op_max_nnz_per_row, tolerance
 
-# first run on a B200: round 2 (profiles/r02_pytest_gpu_next_first_run.log); part of `pytest -m gpu` since
 pytestmark = pytest.mark.gpu
 
 CASES = [(bs, mb, nb) for (mb, nb) in SHAPES for bs in BLOCK_SIZES] + [PRIME_CASE]
@@ -161,7 +160,7 @@ def test_tile_kernel_every_block_size(cuda, oracle, bs, force, monkeypatch):
     else:
         monkeypatch.delenv("B200SP_BSR_KERNEL", raising=False)
 
-    mb = max(20000, 4000000 // (bs * bs))  # enough tiles per CTA to wrap the ring on 148 SMs
+    mb = max(20000, 4000000 // (bs * bs))  # enough tiles per CTA to wrap the ring on 132 SMs
     nb = mb + 13
     rp, ci, v = bsr_random(bs, mb, nb, seed=bs, min_blocks=0, max_blocks=12, sort=False)
     A = to_dev(sp, cuda, bs, nb, rp, ci, v)

@@ -10,7 +10,6 @@ import torch
 from crs_cases import MERGE_CASES, random_matrix, spadd_dense_check
 from helpers import kk_matrix
 
-# first B200 run: profiles/r01_gpu_check_a.log (C ABI vs oracle) and profiles/r01_pytest_b.log (this file, 58 passed)
 pytestmark = pytest.mark.gpu
 
 

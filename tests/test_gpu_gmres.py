@@ -8,7 +8,6 @@ import torch
 
 from gmres_cases import crs_to_bsr, gmres_matrix, true_rel_res
 
-# first run on a B200: round 2 (profiles/r02_pytest_gpu_next_first_run.log); part of `pytest -m gpu` since
 pytestmark = pytest.mark.gpu
 
 

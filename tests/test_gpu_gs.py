@@ -9,7 +9,6 @@ from gmres_cases import gmres_matrix
 from test_emulated_gs import check_coloring, symmetrize
 from test_oracle_cg import spd_lap27
 
-# first run on a B200: round 2 (profiles/r02_pytest_gpu_next_first_run.log); part of `pytest -m gpu` since
 pytestmark = pytest.mark.gpu
 
 

@@ -9,7 +9,6 @@ import torch
 
 from test_oracle_gs2 import dd_matrix
 
-# first run on a B200: round 2 (profiles/r02_pytest_gpu_next_first_run.log); part of `pytest -m gpu` since
 pytestmark = pytest.mark.gpu
 
 

@@ -8,7 +8,6 @@ import torch
 
 from helpers import kk_matrix
 
-# first run on a B200: round 2 (profiles/r02_pytest_gpu_next_first_run.log); part of `pytest -m gpu` since
 pytestmark = pytest.mark.gpu
 
 

@@ -10,7 +10,6 @@ import torch
 
 from test_emulated_spmv64 import random_crs
 
-# first run on a B200: round 2 (profiles/r02_pytest_gpu_next_first_run.log); part of `pytest -m gpu` since
 pytestmark = pytest.mark.gpu
 
 

@@ -1,11 +1,12 @@
 """Pins oracle/kk_oracle_bsr.c (BsrMatrix SpMV): the restatement of the reference's mode-N functor must equal
-(a) the reference's own functor compiled from the reference tree (oracle/_ref/libkkref.so) and (b) the pinned
+(a) the reference's own functor (its outputs stored as digests, see helpers.ReferenceOutputs) and (b) the pinned
 CrsMatrix functor order on bsr_to_crs(A), bit for bit; the host functors (all four modes) by the unit test's law
 (sparse/unit_test/Test_Sparse_spmv_bsr.hpp:142-213,351-456)."""
 import numpy as np
 import pytest
 
 from bsr_cases import BLOCK_SIZES, COEFS_ALPHA, COEFS_BETA, PRIME_CASE, SHAPES, bsr_random, op_max_nnz_per_row, tolerance
+from helpers import ReferenceOutputs
 
 CASES = [(bs, mb, nb) for (mb, nb) in SHAPES for bs in BLOCK_SIZES] + [PRIME_CASE]
 
@@ -18,8 +19,7 @@ def vectors(rng, n, k, dtype, order="F"):
 @pytest.mark.parametrize("bs,mb,nb", CASES)
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
 def test_v42_restatement_equals_reference_functor(oracle, bs, mb, nb, dtype):
-    if oracle.ref is None or not hasattr(oracle.ref, "kkref_bsr_spmv_v42_f64"):
-        pytest.skip("oracle/_ref not built")
+    reference = ReferenceOutputs(f"bsr_v42/{np.dtype(dtype).name}/{bs}/{mb}x{nb}")
     rp, ci, v = bsr_random(bs, mb, nb, seed=bs * 100 + mb, dtype=dtype, sort=False)
     rng = np.random.default_rng(5)
     for k, order in ((1, "F"), (3, "F"), (4, "C")):
@@ -31,9 +31,10 @@ def test_v42_restatement_equals_reference_functor(oracle, bs, mb, nb, dtype):
                 if beta == 0.0:
                     Y0n[::3] = np.nan
                 a = oracle.bsr_spmv_v42(bs, rp, ci, v, X, Y0n.copy(order=order), alpha, beta)
-                b = oracle.bsr_spmv_v42(bs, rp, ci, v, X, Y0n.copy(order=order), alpha, beta, ref=True)
-                assert np.array_equal(a, b), (k, order, alpha, beta)
+                reference.add((a,), lambda: (oracle.bsr_spmv_v42(bs, rp, ci, v, X, Y0n.copy(order=order), alpha, beta, ref=True),),
+                              (k, order, alpha, beta))
                 assert not np.isnan(a).any()
+    reference.check()
 
 
 @pytest.mark.parametrize("bs,mb,nb", CASES)

@@ -5,7 +5,7 @@ C = (I - omega * diag(dinv) * A) * B on the pattern of A*B, with the reference t
 import numpy as np
 import pytest
 
-from helpers import dense_from_csr
+from helpers import ReferenceOutputs, dense_from_csr
 
 
 def diag_dominant(n, per, seed):
@@ -45,13 +45,12 @@ def test_jacobi_matches_dense(oracle, n, per, dtype, tol):
 @pytest.mark.parametrize("n,per", [(60, 4), (500, 9), (3000, 7)])
 def test_jacobi_restatement_equals_reference_seq(oracle, n, per):
     """The restatement equals the reference's own spgemm_jacobi_seq -- sparse/impl/KokkosSparse_spgemm_jacobi_seq_impl.hpp
-    compiled from the reference tree in place (oracle/_ref) -- bit for bit: entries in first-touch order, values."""
-    if oracle.ref is None or not hasattr(oracle.ref, "kkref_spgemm_jacobi_f64"):
-        pytest.skip("oracle/_ref not built")
+    (its output stored as a digest, see helpers.ReferenceOutputs) -- bit for bit: entries in first-touch order, values."""
     rp, ci, v = diag_dominant(n, per, n + 1)
     rng = np.random.default_rng(n)
     vB = rng.uniform(-1, 1, len(ci))
     dinv = rng.uniform(0.5, 1.5, n)
     got = oracle.spgemm_jacobi(rp, ci, v, rp, ci, vB, n, 0.7, dinv, sort=False)
-    ref = oracle.ref_spgemm_jacobi(rp, ci, v, rp, ci, vB, n, 0.7, dinv)
-    assert np.array_equal(got[0], ref[0]) and np.array_equal(got[1], ref[1]) and np.array_equal(got[2], ref[2])
+    reference = ReferenceOutputs(f"jacobi/{n}/{per}")
+    reference.add(got, lambda: oracle.ref_spgemm_jacobi(rp, ci, v, rp, ci, vB, n, 0.7, dinv))
+    reference.check()

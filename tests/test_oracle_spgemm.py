@@ -1,13 +1,13 @@
 """Pins the SpGEMM oracle: the C restatement must equal, bit for bit, the
-REFERENCE's own spgemm_debug_symbolic/numeric compiled from the reference tree
-(oracle/_ref/libkkref.so, see oracle/Makefile), plus the reference's fixtures
-and degenerate shapes (Test_Sparse_spgemm.hpp:483-511)."""
+REFERENCE's own spgemm_debug_symbolic/numeric (its outputs stored as digests, see
+helpers.ReferenceOutputs), plus the reference's fixtures and degenerate
+shapes (Test_Sparse_spgemm.hpp:483-511)."""
 import os
 
 import numpy as np
 import pytest
 
-from helpers import dense_from_csr, kk_matrix
+from helpers import ReferenceOutputs, dense_from_csr, kk_matrix
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "issue402.npz")
 
@@ -20,13 +20,12 @@ def _ab(oracle, m, k, n, nnz, bw, var):
 
 @pytest.mark.parametrize("m,k,n,nnz", [(1000, 500, 1600, 20000), (2500, 2000, 1500, 40000)])
 def test_restatement_equals_reference_build(oracle, m, k, n, nnz):
-    if oracle.ref is None:
-        pytest.skip("oracle/_ref not built (reference tree absent and no prebuilt library)")
     A, B = _ab(oracle, m, k, n, nnz, 500, 10)
-    rpC, ciC, vC = oracle.spgemm(*A, *B, n, sort=False)
-    rrp, rci, rv = oracle.ref_spgemm(*A, k, *B, n)
-    assert np.array_equal(rpC, rrp) and np.array_equal(ciC, rci)
-    assert np.array_equal(vC, rv)  # same operation order -> same bits
+    got = oracle.spgemm(*A, *B, n, sort=False)
+    # same operation order -> same bits
+    reference = ReferenceOutputs(f"spgemm/{m}x{k}x{n}/{nnz}")
+    reference.add(got, lambda: oracle.ref_spgemm(*A, k, *B, n))
+    reference.check()
 
 
 def test_against_dense(oracle):
@@ -63,10 +62,15 @@ def test_issue402_fixture(oracle):
     oracle.sort_crs(rp, ci, v)
     oracle.sort_crs(trp, tci, tv)
     rpC, ciC, vC = oracle.spgemm(rp, ci, v, trp, tci, tv, n)
-    if oracle.ref is not None:
+
+    def ref():
         rrp, rci, rv = oracle.ref_spgemm(rp, ci, v, n, trp, tci, tv, n)
         oracle.sort_crs(rrp, rci, rv)
-        assert np.array_equal(rpC, rrp) and np.array_equal(ciC, rci) and np.array_equal(vC, rv)
+        return rrp, rci, rv
+
+    reference = ReferenceOutputs("spgemm/issue402")
+    reference.add((rpC, ciC, vC), ref)
+    reference.check()
     Cd = dense_from_csr(rpC, ciC, vC, n)
     assert np.allclose(Cd, Cd.T, rtol=1e-9, atol=1e-18)
     Ad = dense_from_csr(rp, ci, v, n)

@@ -3,7 +3,7 @@ known-answer tests and checks its variants against each other (CPU only)."""
 import numpy as np
 import pytest
 
-from helpers import dense_from_csr, kk_matrix, spmv_tolerance
+from helpers import ReferenceOutputs, dense_from_csr, kk_matrix, spmv_tolerance
 
 EPS_F = np.finfo(np.float32).eps
 
@@ -158,12 +158,12 @@ def test_fma_build_brackets(oracle):
 @pytest.mark.parametrize("rows,per,bw,var", [(1000, 3, 200, 10), (1000, 20, 100, 5), (5000, 3, 100, 10), (300, 61, 250, 40)])
 def test_o1_o2_equal_the_reference_code_bit_for_bit(oracle, dtype, rows, per, bw, var):
     """O1 (the Serial loop north_star names as the parity oracle) and O2 (the generic functor) against the reference's OWN code:
-    sparse/impl/KokkosSparse_spmv_impl.hpp compiled from the reference tree in place (oracle/_ref, oracle/kkref_spmv.cpp) and
-    run through its own dispatch on dobeta.  Every alpha x beta of the reference's sweep (Test_Sparse_spmv.hpp:1060-1068 +
-    the dobeta = -1 branch), rows with 0..60+ entries (the 4-way unrolled loop with every remainder), NaN in y for beta = 0."""
-    if oracle.ref is None or not hasattr(oracle.ref, "kkref_spmv_serial_f64"):
-        pytest.skip("oracle/_ref not built")
+    sparse/impl/KokkosSparse_spmv_impl.hpp (oracle/kkref_spmv.cpp; its outputs stored as digests, see
+    helpers.ReferenceOutputs), run through its own dispatch on dobeta.  Every alpha x beta of the reference's sweep
+    (Test_Sparse_spmv.hpp:1060-1068 + the dobeta = -1 branch), rows with 0..60+ entries (the 4-way unrolled loop with every
+    remainder), NaN in y for beta = 0."""
     rp, ci, v = kk_matrix(rows, rows, rows * per, var, bw, dtype=dtype)
+    reference = ReferenceOutputs(f"spmv_o1_o2/{np.dtype(dtype).name}/{rows}x{per}/{bw}/{var}")
     rng = np.random.default_rng(13718)
     x = rng.random(rows).astype(dtype)
     y0 = rng.random(rows).astype(dtype)
@@ -173,20 +173,18 @@ def test_o1_o2_equal_the_reference_code_bit_for_bit(oracle, dtype, rows, per, bw
             if beta == 0.0:
                 yin[::19] = np.nan
             a = oracle.spmv_serial(rp, ci, v, x, yin.copy(), alpha, beta)
-            b = oracle.ref_spmv("serial", rp, ci, v, x, yin.copy(), alpha, beta)
-            assert np.array_equal(a, b, equal_nan=True), ("O1", alpha, beta)
+            reference.add((a,), lambda: (oracle.ref_spmv("serial", rp, ci, v, x, yin.copy(), alpha, beta),), ("O1", alpha, beta))
             c = oracle.spmv_functor(rp, ci, v, rows, x, yin.copy(), alpha, beta)
-            d = oracle.ref_spmv("functor", rp, ci, v, x, yin.copy(), alpha, beta)
-            assert np.array_equal(c, d, equal_nan=True), ("O2", alpha, beta)
+            reference.add((c,), lambda: (oracle.ref_spmv("functor", rp, ci, v, x, yin.copy(), alpha, beta),), ("O2", alpha, beta))
+    reference.check()
 
 
 @pytest.mark.parametrize("rows,cols,per", [(1000, 1000, 7), (800, 300, 21), (300, 2000, 5)])
 def test_o5_equals_the_reference_transpose_code(oracle, rows, cols, per):
     """O5 (Serial transpose: y scaled first, then the order-preserving unrolled scatter) against the reference's own
-    spmv_beta_transpose compiled in place (sparse/impl/KokkosSparse_spmv_impl.hpp:383-460), bit for bit."""
-    if oracle.ref is None or not hasattr(oracle.ref, "kkref_spmv_transpose_f64"):
-        pytest.skip("oracle/_ref not built")
+    spmv_beta_transpose (sparse/impl/KokkosSparse_spmv_impl.hpp:383-460; its outputs stored as digests), bit for bit."""
     rp, ci, v = kk_matrix(rows, cols, rows * per, 6, min(cols, 200))
+    reference = ReferenceOutputs(f"spmv_o5/{rows}x{cols}x{per}")
     rng = np.random.default_rng(5)
     x = rng.random(rows)
     y0 = rng.random(cols)
@@ -196,20 +194,19 @@ def test_o5_equals_the_reference_transpose_code(oracle, rows, cols, per):
             if beta == 0.0:
                 yin[::23] = np.nan
             a = oracle.spmv_transpose(rp, ci, v, cols, x, yin.copy(), alpha, beta)
-            b = oracle.ref_spmv("transpose", rp, ci, v, x, yin.copy(), alpha, beta)
-            assert np.array_equal(a, b), (alpha, beta)
+            reference.add((a,), lambda: (oracle.ref_spmv("transpose", rp, ci, v, x, yin.copy(), alpha, beta),), (alpha, beta))
+    reference.check()
 
 
 @pytest.mark.parametrize("order", ["F", "C"])
 @pytest.mark.parametrize("k", [1, 3, 16, 17, 33])
 def test_o4_equals_the_reference_multivector_code(oracle, order, k):
     """O4 (CPU multivector strips, alpha folded per term when alpha is not 0 / +-1, dobeta = -1 as -y + sum) and the multivector
-    transpose against the reference's own spmv_alpha_mv compiled in place (sparse/impl/KokkosSparse_spmv_impl.hpp:547-1270),
-    bit for bit, for every alpha x beta, column counts around the strip widths (16 / 17) and both layouts."""
-    if oracle.ref is None or not hasattr(oracle.ref, "kkref_spmv_mv_f64"):
-        pytest.skip("oracle/_ref not built")
+    transpose against the reference's own spmv_alpha_mv (sparse/impl/KokkosSparse_spmv_impl.hpp:547-1270; its outputs stored
+    as digests), bit for bit, for every alpha x beta, column counts around the strip widths (16 / 17) and both layouts."""
     rows, cols = 700, 500
     rp, ci, v = kk_matrix(rows, cols, rows * 9, 8, 150)
+    reference = ReferenceOutputs(f"spmv_o4/{order}/{k}")
     rng = np.random.default_rng(k)
     for mode in ("N", "T"):
         nx, ny = (rows, cols) if mode == "T" else (cols, rows)
@@ -224,8 +221,9 @@ def test_o4_equals_the_reference_multivector_code(oracle, order, k):
                     a = oracle.spmv_mv(rp, ci, v, cols, X, Yin.copy(order=order), alpha, beta)
                 else:
                     a = oracle.spmv_mv_transpose(rp, ci, v, cols, X, Yin.copy(order=order), alpha, beta)
-                b = oracle.ref_spmv_mv(mode, rp, ci, v, cols, X, Yin.copy(order=order), alpha, beta)
-                assert np.array_equal(a, b), (mode, alpha, beta)
+                reference.add((a,), lambda: (oracle.ref_spmv_mv(mode, rp, ci, v, cols, X, Yin.copy(order=order), alpha, beta),),
+                              (mode, alpha, beta))
+    reference.check()
 
 
 def test_raw_openmp_path_a8(oracle):

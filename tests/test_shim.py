@@ -28,7 +28,7 @@ def test_shim_runs_on_gpu(cuda):
 
 @pytest.mark.gpu
 def test_shim_bsr_runs_on_gpu(cuda):
-    """SPMV_BSRMATRIX / SPMV_MV_BSRMATRIX / SPGEMM_JACOBI specialisations (on the B200 since round 2, see tests/test_gpu_bsr.py)."""
+    """SPMV_BSRMATRIX / SPMV_MV_BSRMATRIX / SPGEMM_JACOBI specialisations (run on the GPU by tests/test_gpu_bsr.py)."""
     out = subprocess.run([DRV, "--bsr", "--jacobi", "--gs", "--gmres", "--spmv64", "--sptrsv"], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0, out.stdout + out.stderr
     assert "SHIM DRIVER OK" in out.stdout and "BsrMatrix spmv through" in out.stdout and "spgemm_jacobi through" in out.stdout and \

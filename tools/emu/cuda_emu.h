@@ -64,7 +64,7 @@ static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 static inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 static inline cudaError_t cudaGetDeviceCount(int* n) { *n = 1; return cudaSuccess; }
 static inline cudaError_t cudaDeviceGetAttribute(int* v, int attr, int) {
-  *v = attr == cudaDevAttrMultiProcessorCount ? 4 : (attr == cudaDevAttrComputeCapabilityMajor ? 10 : 0);
+  *v = attr == cudaDevAttrMultiProcessorCount ? 4 : (attr == cudaDevAttrComputeCapabilityMajor ? 9 : 0);
   return cudaSuccess;
 }
 static inline cudaError_t cudaMalloc(void** p, size_t n) { *p = b200emu::device_alloc(n); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }

@@ -6,8 +6,7 @@ instruction count comes from.  Uses the object files of the in-tree build (compi
   python tools/sass_lines.py spmm spmm_tile_kernel 'float, (int)4, (int)4'
 
 Prints `line  #instructions  source text` for the kernel whose demangled name contains every given substring
-(first match), plus totals per opcode class.  Weigh the lines with the trip counts of the case at hand (see
-profiles/r01_spgemm_num_v1_sass_accounting.md for an example)."""
+(first match), plus totals per opcode class.  Weigh the lines with the trip counts of the case at hand."""
 import collections
 import os
 import re
