@@ -314,6 +314,12 @@ struct Acc {
   S a[VW];
 };
 
+// beta*y + alpha*acc as alpha*acc rounded, then one fused multiply-add.  Written out so that every instantiation rounds the
+// same way: left to the compiler, the contraction of this expression differed between the 16-byte-load (VW > 1) and the
+// scalar variants of the item and tile kernels, and misaligned operands then gave other bits than aligned ones.
+__device__ __forceinline__ float axpby_rn(float alpha, float acc, float beta, float y) { return fmaf(beta, y, __fmul_rn(alpha, acc)); }
+__device__ __forceinline__ double axpby_rn(double alpha, double acc, double beta, double y) { return fma(beta, y, __dmul_rn(alpha, acc)); }
+
 template <typename S, int VW>
 __device__ __forceinline__ Acc<S, VW> load_x(const S* __restrict__ p) {
   static_assert(VW == 1 || VW == VecOf<S>::W, "VW is 1 or the 16-byte vector width");
@@ -418,7 +424,7 @@ __global__ void __launch_bounds__((NW + 1) * 32)
           } else {
             const Acc<S, VW> old = load_x<S, VW>(yp);
 #pragma unroll
-            for (int q = 0; q < VW; ++q) o[q] = beta * old.a[q] + alpha * acc.a[q];
+            for (int q = 0; q < VW; ++q) o[q] = axpby_rn(alpha, acc.a[q], beta, old.a[q]);
           }
           if constexpr (VW == 1) {
             yp[0] = o[0];
@@ -719,7 +725,8 @@ int plan_chunk_rows(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, co
 
 template <typename S>
 static int launch_split(b200sp_spmv_plan* p, cudaStream_t st, int m, int k, int64_t nnz, const int* row_ptr,
-                        const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
+                        const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta,
+                        const char** name) {
   const int Q = 256;
   int* chunk_row = nullptr;
   int n_chunks = 0;
@@ -736,6 +743,7 @@ static int launch_split(b200sp_spmv_plan* p, cudaStream_t st, int m, int k, int6
                         ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0 && getenv("B200SP_SPMM_VEC") != nullptr;
     // opt-in: slower than the scalar-lane kernel on config 3 when it was tuned -- fewer lanes per chunk means fewer
     // chunks in flight per SM at its register count; kept for the tuning round
+    *name = vec_ok ? "split_vec" : "split";
     if (vec_ok) {
       int KTv = 1;
       while (KTv * VW < k && KTv < 32) KTv <<= 1;
@@ -825,7 +833,8 @@ static int launch_mm_tile_cfg(int cfg, cudaStream_t st, const MMTileView& tv, in
 
 template <typename S>
 static int launch_mm_tile(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m, int k, int64_t nnz, const int* row_ptr,
-                          const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
+                          const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta,
+                          const char** name) {
   constexpr int SEG = 2048;
   int cfg = 0;
   if (const char* e = getenv("B200SP_SPMM_CFG")) cfg = atoi(e);
@@ -862,9 +871,11 @@ static int launch_mm_tile(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m,
   const int grid = sm_count() * 4;
   spmm_seg_prescale_kernel<S><<<grid, 256, 0, st>>>(tv.segs, tv.n_seg, k, beta, Y, ldy);
   B200SP_LAUNCH_CHECK();
+  *name = vec ? "tile_vec" : "tile";
   if (vec) {
     const char* e = getenv("B200SP_SPMM_SEG");
     if (e && e[0] == 'v') {
+      *name = "tile_vec+seg_vec";
 #define B200SP_SEGV(L)                                                                                               \
   case L:                                                                                                            \
     spmm_seg_vec_kernel<S, L><<<grid, 256, 0, st>>>(tv.segs, tv.n_seg, k, col_idx, vals, X, ldx, Y, ldy, alpha, beta); \
@@ -1075,7 +1086,7 @@ __global__ void __launch_bounds__(256)
       } else {
         const Acc<S, VW> old = load_x<S, VW>(dst);
 #pragma unroll
-        for (int cc = 0; cc < VW; ++cc) o[cc] = beta * old.a[cc] + alpha * acc.a[cc];
+        for (int cc = 0; cc < VW; ++cc) o[cc] = axpby_rn(alpha, acc.a[cc], beta, old.a[cc]);
       }
     } else {
       dst = partial + (int64_t)slot * k + j;  // raw sums; alpha and beta are applied by the reduce kernel
@@ -1208,7 +1219,7 @@ __global__ void __launch_bounds__(256)
       } else {
         const Acc<S, VW> old = load_x<S, VW>(dst);
 #pragma unroll
-        for (int cc = 0; cc < VW; ++cc) o[cc] = beta * old.a[cc] + alpha * acc.a[cc];
+        for (int cc = 0; cc < VW; ++cc) o[cc] = axpby_rn(alpha, acc.a[cc], beta, old.a[cc]);
       }
     } else {
       dst = partial + (int64_t)slot * k + j;  // raw sums; alpha and beta are applied by the reduce kernel
@@ -1422,15 +1433,22 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
       plan_set_last_kernel(p, vec ? "spmm_items_vec" : "spmm_items");
       return launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
     }
+    const char* name = "rowmajor";
+    int rc;
     if (choice >= 2 && (((uintptr_t)vals | (uintptr_t)col_idx | (uintptr_t)row_ptr) & 15u) == 0) {
       constexpr int W = VecOf<S>::W;
       const bool vec = choice == 3 && (k % W == 0) && (ldx % W == 0) && (ldy % W == 0) && ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0;
-      plan_set_last_kernel(p, vec ? "spmm_tile_vec" : "spmm_tile");
-      return launch_mm_tile<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
+      rc = launch_mm_tile<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta, &name);
+    } else if (split) {
+      rc = launch_split<S>(p, st, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta, &name);
+    } else {
+      rc = launch_rowmajor<S>(st, m, k, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
     }
-    plan_set_last_kernel(p, split ? "spmm_split" : "spmm_rowmajor");
-    if (split) return launch_split<S>(p, st, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
-    return launch_rowmajor<S>(st, m, k, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
+    if (rc) return rc;
+    char label[48];
+    snprintf(label, sizeof(label), "spmm_%s", name);
+    plan_set_last_kernel(p, label);
+    return B200SP_OK;
   }
   // LayoutLeft operands: with a plan and k >= 4, relayout to row-major scratch and use the row-major kernel
   if (p && k >= 4) {
@@ -1460,6 +1478,7 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
       }
     }
     const bool tile_ok = choice >= 2 && (choice == 4 || (((uintptr_t)vals | (uintptr_t)col_idx | (uintptr_t)row_ptr) & 15u) == 0);
+    const char* name = choice == 4 ? "items" : split ? "split" : "rowmajor";
     if (choice == 4) {
       constexpr int W = VecOf<S>::W;
       const bool vec = (k % W == 0) && (ldxr % W == 0) && (ldyr % W == 0) && ((((uintptr_t)Xr) | ((uintptr_t)Yr)) & 15u) == 0;
@@ -1467,9 +1486,9 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
     } else if (tile_ok) {
       constexpr int W = VecOf<S>::W;
       const bool vec = choice == 3 && (k % W == 0) && (ldxr % W == 0) && (ldyr % W == 0) && ((((uintptr_t)Xr) | ((uintptr_t)Yr)) & 15u) == 0;
-      rc = launch_mm_tile<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta);
+      rc = launch_mm_tile<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta, &name);
     } else {
-      rc = split ? launch_split<S>(p, st, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta)
+      rc = split ? launch_split<S>(p, st, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta, &name)
                  : launch_rowmajor<S>(st, m, k, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta);
     }
     if (rc) return rc;
@@ -1477,7 +1496,9 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
       relayout_kernel<S, false><<<rl_grid(yrows), tb, 0, st>>>(yrows, k, Yr, nullptr, Y, yr, yc);
       B200SP_LAUNCH_CHECK();
     }
-    plan_set_last_kernel(p, choice == 4 ? "spmm_relayout+items" : tile_ok ? "spmm_relayout+tile" : (split ? "spmm_relayout+split" : "spmm_relayout+rowmajor"));
+    char label[48];
+    snprintf(label, sizeof(label), "spmm_relayout+%s", name);
+    plan_set_last_kernel(p, label);
     return B200SP_OK;
   }
   const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);

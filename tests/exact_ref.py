@@ -1,0 +1,180 @@
+"""Exact reference and per-entry rounding-error bound of rank-2 SpMV, Y = beta*Y0 + alpha*op(A)*X.
+
+The oracle (oracle_lib.Oracle.spmv_mv) computes in the kernel's own precision, so its rounding error is about as large as
+the error it is meant to detect.  spmm_exact computes the same product in a wider format (float64 for fp32 data,
+np.longdouble for fp64 data), and spmm_bound gives, for every entry of Y, how far a correctly implemented kernel may be
+from it.  assert_within checks a kernel's output entry by entry against that bound."""
+import numpy as np
+
+assert np.finfo(np.longdouble).nmant >= 63, "the fp64 reference needs an x87-extended or quad np.longdouble"
+
+_CHUNK = 1 << 23  # products held at once (entries x columns): keeps the wide temporaries to a few hundred MB
+
+
+def wide(dtype):
+    """The reference's working format: fp32 products are exact in float64, fp64 products nearly so in long double."""
+    return np.float64 if np.dtype(dtype) == np.float32 else np.longdouble
+
+
+def unit_roundoff(dtype):
+    return float(np.finfo(dtype).eps) / 2
+
+
+def gamma(n, u):
+    """Higham's gamma_n = n*u / (1 - n*u): bound on |prod (1 + d_i)^(+-1) - 1| over n roundings with |d_i| <= u."""
+    n = np.asarray(n, dtype=np.float64)
+    return n * u / (1.0 - n * u)
+
+
+def _op_rows(rp, ci, ncols, trans):
+    """Rows of op(A) as (start offsets, row of A of each entry, column of X of each entry, permutation of the entries).
+    For T/H the entries are stably sorted by column, so row c of op(A) is column c of A in storage order."""
+    rp = np.asarray(rp, dtype=np.int64)
+    ci = np.asarray(ci, dtype=np.int64)
+    m = len(rp) - 1
+    arow = np.repeat(np.arange(m, dtype=np.int64), np.diff(rp))
+    if not trans:
+        return rp, arow, ci, None
+    order = np.argsort(ci, kind="stable")
+    starts = np.zeros(ncols + 1, dtype=np.int64)
+    np.cumsum(np.bincount(ci, minlength=ncols), out=starts[1:])
+    return starts, ci[order], arow[order], order
+
+
+def _segment_sums(starts, xrow, w, X, dt):
+    """out[r, :] = sum over entries e of row r of w[e] * X[xrow[e], :], in dt; rows without entries give 0.
+    np.add.reduceat over the non-empty rows only (it returns the element itself, not 0, for an empty segment)."""
+    nrows = len(starts) - 1
+    k = X.shape[1]
+    out = np.zeros((nrows, k), dtype=dt)
+    lens = np.diff(starts)
+    nz = np.flatnonzero(lens > 0)
+    if len(nz) == 0 or k == 0:
+        return out
+    step = max(1, _CHUNK // max(k, 1))
+    i = 0
+    while i < len(nz):
+        # a block of non-empty rows whose entries fit in one chunk (at least one row, however long)
+        e0 = starts[nz[i]]
+        j = int(np.searchsorted(starts[nz + 1], e0 + step, side="right"))
+        j = max(j, i + 1)
+        rows = nz[i:j]
+        e1 = starts[rows[-1] + 1]
+        prod = w[e0:e1, None].astype(dt) * X[xrow[e0:e1]].astype(dt)
+        out[rows] = np.add.reduceat(prod, starts[rows] - e0, axis=0)
+        i = j
+    return out
+
+
+def _check_args(rp, ci, v, X, Y0):
+    X = np.asarray(X)
+    Y0 = np.asarray(Y0)
+    if X.ndim == 1:
+        X = X[:, None]
+    if Y0.ndim == 1:
+        Y0 = Y0[:, None]
+    assert X.shape[1] == Y0.shape[1], (X.shape, Y0.shape)
+    assert len(ci) == len(v) == int(rp[-1]) - int(rp[0]) and int(rp[0]) == 0
+    return X, Y0
+
+
+def spmm_exact(rp, ci, v, X, Y0, alpha, beta, trans=False):
+    """beta*Y0 + alpha*op(A)*X in the wide format of v's dtype (float64 for fp32, np.longdouble for fp64).
+
+    A is (rp, ci, v) with as many columns as op(A)'s shape needs: rows of Y0 are the rows of op(A), rows of X its columns.
+    alpha and beta are first rounded to v's dtype, as the library receives them.  beta == 0 ignores Y0 (NaN included);
+    alpha == 0 gives beta*Y0 without reading X (KokkosSparse_spmv.hpp:145-154).  The product of two fp32 numbers is exact in
+    float64 and of two fp64 numbers nearly so in long double, and the sums carry about len*2^-53 resp. len*2^-64 relative
+    error -- spmm_bound adds that in as well."""
+    X, Y0 = _check_args(rp, ci, v, X, Y0)
+    dt = wide(v.dtype)
+    a = dt(np.asarray(alpha, dtype=v.dtype))
+    b = dt(np.asarray(beta, dtype=v.dtype))
+    out = np.zeros(Y0.shape, dtype=dt)
+    if b != 0:
+        out += b * Y0.astype(dt)
+    if a == 0:
+        return out
+    starts, _, xrow, order = _op_rows(rp, ci, Y0.shape[0] if trans else None, trans)
+    w = v if order is None else v[order]
+    with np.errstate(invalid="ignore"):  # an Inf in X times a zero of A is NaN, as on the device
+        out += a * _segment_sums(starts, xrow, w, X, dt)
+    return out
+
+
+def op_row_lengths(rp, ci, nrows_out, trans=False):
+    """Entries in each row of op(A), duplicates counted."""
+    if not trans:
+        return np.diff(np.asarray(rp, dtype=np.int64))
+    return np.bincount(np.asarray(ci, dtype=np.int64), minlength=nrows_out)
+
+
+def spmm_bound(rp, ci, v, X, Y0, alpha, beta, trans=False):
+    """Per entry of Y: gamma(len_i + 4) * (|alpha| * sum_j |a_ij||x_jc| + |beta||y0_ic|) + the reference's own error.
+
+    gamma(n) = n*u / (1 - n*u), u = eps/2 of v's dtype, len_i the length of row i of op(A) (not the matrix maximum).
+
+    Derivation (Higham, Accuracy and Stability of Numerical Algorithms, 2nd ed., sections 3.1 and 3.3).  The computed entry
+    is a sum of len_i + 1 terms: beta*y0 and the len_i products alpha*a_ij*x_jc.  Whatever the order or tree of the
+    additions, an addition tree over len_i + 1 leaves has at most len_i levels, so each term passes through at most len_i
+    rounded additions -- a split of the row into pieces or segments, a shuffle or shared-memory reduce, an atomicAdd onto a
+    pre-scaled beta*y0 are all such trees.  A product a_ij*x_jc is rounded at most once (not at all when it is fused into
+    an FMA).  alpha is applied with at most two roundings: once to a partial sum (or to a_ij, or to the product) and once
+    more when a kernel folds it into a partial before the final multiply-add.  beta*y0 is rounded once, and the final
+    multiply-add beta*y0 + alpha*s adds at most one rounding that the addition count above already includes.  So every
+    term carries a factor (1 + theta) with |theta| <= gamma(len_i + 3) (Higham lemma 3.1, which also covers FMA: a fused
+    multiply-add is one rounding of the exact a*b + c), and the error is at most gamma(len_i + 3) times the sum of the
+    terms' magnitudes.  The bound uses len_i + 4, one spare rounding; it still fails any kernel that drops a term larger
+    than about (len_i + 4)*u of the row's scale.  Underflow is not modelled: the test data keep products far from the
+    subnormal range.
+
+    The reference itself is off from the exact value by at most gamma_w(len_i + 2) times the same scale, with u_w the
+    unit roundoff of its wide format (2^-53 for fp32 data, 2^-64 for fp64 data); that is added so the bound holds against
+    the reference, not only against the exact product."""
+    scale = spmm_scale(rp, ci, v, X, Y0, alpha, beta, trans)
+    lens = op_row_lengths(rp, ci, scale.shape[0], trans).astype(np.float64)
+    u = unit_roundoff(v.dtype)
+    uw = unit_roundoff(wide(v.dtype))
+    factor = gamma(lens + 4, u) + gamma(lens + 2, uw)
+    # the scale is summed in float64: at most (len + 1)*2^-53 relative error, far below the spare rounding above
+    return factor[:, None] * scale
+
+
+def spmm_scale(rp, ci, v, X, Y0, alpha, beta, trans=False):
+    """|alpha| * sum_j |a_ij||x_jc| + |beta||y0_ic| in float64 (the Y0 term only for beta != 0, the A term only for
+    alpha != 0, as the product reads them)."""
+    X, Y0 = _check_args(rp, ci, v, X, Y0)
+    a = abs(float(np.asarray(alpha, dtype=v.dtype)))
+    b = abs(float(np.asarray(beta, dtype=v.dtype)))
+    scale = np.zeros(Y0.shape, dtype=np.float64)
+    if b != 0:
+        scale += b * np.abs(Y0.astype(np.float64))
+    if a != 0:
+        starts, _, xrow, order = _op_rows(rp, ci, Y0.shape[0] if trans else None, trans)
+        w = np.abs(v if order is None else v[order]).astype(np.float64)
+        with np.errstate(invalid="ignore"):  # 0 * Inf where X holds an Inf: that entry's exact value is not finite either
+            scale += a * _segment_sums(starts, xrow, w, np.abs(X.astype(np.float64)), np.float64)
+    return scale
+
+
+def assert_within(got, exact, bound, what):
+    """Fail on the first entry (row-major order) of `got` that is further than `bound` from `exact`, or that is NaN/Inf
+    where `exact` is finite.  Where `exact` is NaN, `got` must be NaN; where it is +-Inf, `got` must be the same Inf.
+    `what` names the call (the tests put the handle's last_kernel() in it)."""
+    got = np.asarray(got)
+    exact = np.asarray(exact)
+    if got.ndim == 1:
+        got = got[:, None]
+    if exact.ndim == 1:
+        exact = exact[:, None]
+    bound = np.broadcast_to(np.asarray(bound, dtype=np.float64).reshape(exact.shape[0], -1), exact.shape)
+    assert got.shape == exact.shape, f"{what}: shape {got.shape} != {exact.shape}"
+    gw = got.astype(exact.dtype)
+    fin = np.isfinite(exact)
+    with np.errstate(invalid="ignore", over="ignore"):
+        err = np.abs(gw - exact)
+        bad = np.where(fin, ~(err <= bound), ~((np.isnan(exact) & np.isnan(gw)) | (gw == exact)))
+    if bad.any():
+        r, c = (int(t) for t in np.argwhere(bad)[0])
+        raise AssertionError(f"{what}: {int(bad.sum())} entries off; first at row {r}, column {c}: got {got[r, c]!r}, "
+                             f"exact {exact[r, c]!r}, error {float(err[r, c]):.3e}, bound {float(bound[r, c]):.3e}")

@@ -1,0 +1,172 @@
+"""The exact rank-2 SpMV reference and its per-entry bound (tests/exact_ref.py): the reference is exact enough, the bound
+holds for a correct implementation (the oracle's, in the kernel's precision) and fails for subtly wrong ones."""
+from fractions import Fraction
+
+import numpy as np
+import pytest
+
+import exact_ref as R
+import spmm_cases
+
+DTYPES = [np.float64, np.float32]
+
+
+def _oracle_mv(oracle, rp, ci, v, ncols, X, Y0, alpha, beta, trans):
+    Y = Y0.copy()
+    if trans:
+        return oracle.spmv_mv_transpose(rp, ci, v, ncols, X, Y, alpha, beta)
+    if beta == 0:
+        Y = np.zeros_like(Y0)  # the oracle's functor scales a NaN by 0; the library overwrites
+    return oracle.spmv_mv(rp, ci, v, ncols, X, Y, alpha, beta)
+
+
+def _random_case(rng, dtype):
+    m, n = int(rng.integers(1, 60)), int(rng.integers(1, 60))
+    lens = rng.integers(0, 3 * n, m) * (rng.random(m) < 0.85)
+    rp, ci, v = spmm_cases.from_lengths(lens, n, rng, dtype)
+    for i in np.flatnonzero(rng.random(m) < 0.2):  # cancelling rows: +a and -a at one column, a up to 2^12
+        s, e = rp[i], rp[i + 1]
+        h = (e - s) // 2
+        if h:
+            ci[s + h:s + 2 * h] = ci[s:s + h]
+            v[s:s + h] *= dtype(4096.0)
+            v[s + h:s + 2 * h] = -v[s:s + h]
+    return rp, ci, v, n
+
+
+def test_exact_matches_rational_arithmetic():
+    """The reference against Fractions on small cases: within its own stated error (len*2^-53 resp. 2^-64 relative)."""
+    rng = np.random.default_rng(3)
+    for dtype in DTYPES:
+        for trans in (False, True):
+            rp, ci, v, n = _random_case(rng, dtype)
+            m = len(rp) - 1
+            rows_out, rows_in = (n, m) if trans else (m, n)
+            X = spmm_cases.dense_operands(rng, rows_in, 3, dtype)
+            Y0 = spmm_cases.dense_operands(rng, rows_out, 3, dtype)
+            alpha, beta = -1.5, 0.25
+            got = R.spmm_exact(rp, ci, v, X, Y0, alpha, beta, trans)
+            assert got.dtype == R.wide(dtype)
+            scale = R.spmm_scale(rp, ci, v, X, Y0, alpha, beta, trans)
+            lens = R.op_row_lengths(rp, ci, rows_out, trans)
+            arow = np.repeat(np.arange(m), np.diff(rp))
+            orow, xrow = (ci, arow) if trans else (arow, ci)
+            ex = [[Fraction(beta) * Fraction(float(Y0[i, c])) for c in range(3)] for i in range(rows_out)]
+            for e in range(len(ci)):
+                for c in range(3):
+                    ex[orow[e]][c] += Fraction(alpha) * Fraction(float(v[e])) * Fraction(float(X[xrow[e], c]))
+            for i in range(rows_out):
+                for c in range(3):
+                    err = abs(Fraction(*got[i, c].as_integer_ratio()) - ex[i][c])
+                    assert err <= float(R.gamma(lens[i] + 2, R.unit_roundoff(R.wide(dtype)))) * scale[i, c], (dtype, trans, i, c)
+
+
+def test_exact_special_scalars():
+    rp, ci, v, n = spmm_cases.small(1, np.float64)
+    m = len(rp) - 1
+    X = np.full((n, 2), np.nan)
+    Y0 = np.full((m, 2), 3.0)
+    assert np.array_equal(R.spmm_exact(rp, ci, v, X, Y0, 0.0, 2.5), np.full((m, 2), 7.5))  # X never read
+    Y0[::3] = np.nan
+    X = np.ones((n, 2))
+    out = R.spmm_exact(rp, ci, v, X, Y0, 1.0, 0.0)  # Y0 ignored
+    assert np.isfinite(out).all()
+    assert not R.spmm_exact(rp, ci, v, X, Y0, 0.0, 0.0).any()
+    # empty rows give 0 (np.add.reduceat would repeat the next element)
+    empty = np.diff(rp) == 0
+    assert empty.any() and not out[empty].any()
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("trans", [False, True])
+def test_bound_holds_for_the_oracle(oracle, dtype, trans):
+    """A few hundred random products in the kernel's own precision, mixed signs, cancelling rows: all within the bound."""
+    rng = np.random.default_rng(20 + trans)
+    worst = 0.0
+    for _ in range(150):
+        rp, ci, v, n = _random_case(rng, dtype)
+        m = len(rp) - 1
+        k = int(rng.integers(1, 6))
+        rows_out, rows_in = (n, m) if trans else (m, n)
+        X = spmm_cases.dense_operands(rng, rows_in, k, dtype)
+        Y0 = spmm_cases.dense_operands(rng, rows_out, k, dtype)
+        alpha, beta = [(1.0, 0.0), (-1.0, 1.0), (2.5, -0.5), (0.0, 2.5), (1.0, 1.0), (0.0, 0.0)][int(rng.integers(0, 6))]
+        got = _oracle_mv(oracle, rp, ci, v, n, X, Y0, alpha, beta, trans)
+        exact = R.spmm_exact(rp, ci, v, X, Y0, alpha, beta, trans)
+        bound = R.spmm_bound(rp, ci, v, X, Y0, alpha, beta, trans)
+        R.assert_within(got, exact, bound, f"oracle {dtype.__name__} trans={trans}")
+        with np.errstate(invalid="ignore", divide="ignore"):
+            r = np.abs(got.astype(exact.dtype) - exact) / bound
+        worst = max(worst, float(np.nanmax(np.where(bound > 0, r, 0))))
+    assert worst > 0.01  # the bound is not vacuous either: real rounding errors use a visible part of it
+
+
+@pytest.mark.parametrize("trans", [False, True])
+def test_bound_catches_a_dropped_term(oracle, trans):
+    """Removing one entry whose |alpha*a*x| exceeds 64u of its row's scale, in a row of at most 12 entries."""
+    rng = np.random.default_rng(7)
+    caught = 0
+    for dtype in DTYPES:
+        u = R.unit_roundoff(dtype)
+        for _ in range(80):
+            rp, ci, v, n = _random_case(rng, dtype)
+            m = len(rp) - 1
+            rows_out, rows_in = (n, m) if trans else (m, n)
+            X = spmm_cases.dense_operands(rng, rows_in, 2, dtype)
+            Y0 = spmm_cases.dense_operands(rng, rows_out, 2, dtype)
+            alpha, beta = 1.5, -0.5
+            lens = R.op_row_lengths(rp, ci, rows_out, trans)
+            scale = R.spmm_scale(rp, ci, v, X, Y0, alpha, beta, trans)
+            arow = np.repeat(np.arange(m), np.diff(rp))
+            orow, xrow = (ci, arow) if trans else (arow, ci)
+            term = np.abs(alpha * v.astype(np.float64) * X[xrow, 0].astype(np.float64))
+            ok = (lens[orow] <= 12) & (term > 64 * u * scale[orow, 0])
+            if not ok.any():
+                continue
+            e = int(np.flatnonzero(ok)[0])
+            keep = np.ones(len(ci), bool)
+            keep[e] = False
+            rp2 = rp.copy()
+            rp2[arow[e] + 1:] -= 1
+            got = _oracle_mv(oracle, rp2, ci[keep], v[keep], n, X, Y0, alpha, beta, trans)
+            with pytest.raises(AssertionError, match=f"row {orow[e]}, column 0"):
+                R.assert_within(got, R.spmm_exact(rp, ci, v, X, Y0, alpha, beta, trans), R.spmm_bound(rp, ci, v, X, Y0, alpha, beta, trans), "dropped")
+            caught += 1
+    assert caught >= 20
+
+
+def test_bound_catches_fp32_accumulation_of_fp64_data(oracle):
+    """One row of an fp64 product computed from fp32-rounded data."""
+    rng = np.random.default_rng(9)
+    for _ in range(20):
+        rp, ci, v, n = _random_case(rng, np.float64)
+        m = len(rp) - 1
+        X = spmm_cases.dense_operands(rng, n, 2, np.float64) * (1 + rng.random((n, 2)))
+        Y0 = spmm_cases.dense_operands(rng, m, 2, np.float64)
+        got = _oracle_mv(oracle, rp, ci, v, n, X, Y0, 1.0, 1.0, False)
+        got32 = _oracle_mv(oracle, rp, ci, v.astype(np.float32), n, X.astype(np.float32), Y0.astype(np.float32), 1.0, 1.0, False)
+        i = int(np.argmax(np.diff(rp)))
+        got[i] = got32[i]
+        with pytest.raises(AssertionError, match=f"row {i}, "):
+            R.assert_within(got, R.spmm_exact(rp, ci, v, X, Y0, 1.0, 1.0), R.spmm_bound(rp, ci, v, X, Y0, 1.0, 1.0), "fp32 row")
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_bound_catches_swapped_columns(oracle, dtype):
+    rng = np.random.default_rng(11)
+    rp, ci, v, n = spmm_cases.small(2, dtype)
+    m = len(rp) - 1
+    X = spmm_cases.dense_operands(rng, n, 4, dtype)
+    Y0 = spmm_cases.dense_operands(rng, m, 4, dtype)
+    got = _oracle_mv(oracle, rp, ci, v, n, np.ascontiguousarray(X[:, [0, 2, 1, 3]]), Y0, 1.0, 0.0, False)
+    with pytest.raises(AssertionError, match="column 1"):
+        R.assert_within(got, R.spmm_exact(rp, ci, v, X, Y0, 1.0, 0.0), R.spmm_bound(rp, ci, v, X, Y0, 1.0, 0.0), "swapped")
+
+
+def test_assert_within_special_values():
+    exact = np.array([[1.0, np.inf, np.nan]], dtype=np.longdouble)
+    bound = np.zeros((1, 3))
+    R.assert_within(np.array([[1.0, np.inf, np.nan]]), exact, bound, "ok")
+    for bad in ([[np.nan, np.inf, np.nan]], [[1.0, -np.inf, np.nan]], [[1.0, np.inf, 0.0]], [[np.inf, np.inf, np.nan]]):
+        with pytest.raises(AssertionError, match="row 0"):
+            R.assert_within(np.array(bad), exact, bound, "special")

@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 import torch
 
+import exact_ref as R
 from helpers import kk_matrix, spmv_tolerance
 
 pytestmark = pytest.mark.gpu
@@ -43,11 +44,16 @@ def test_spmm_sweep(cuda, oracle, rows, per, bw, var, nv, dtype):
             got = Yd.cpu().numpy()
             assert not np.isnan(got).any()
             assert np.max(np.abs(got - exp)) <= tol, (xrm, yrm, alpha, beta, np.max(np.abs(got - exp)), tol)
+            what = f"{h.last_kernel() if (xrm, yrm) != (True, False) else 'no plan'} {(xrm, yrm)} a={alpha} b={beta}"
+            R.assert_within(got, R.spmm_exact(rp, ci, v, X, Y0, alpha, beta), R.spmm_bound(rp, ci, v, X, Y0, alpha, beta), what)
             # transpose
             Ytd = _mk(cuda, Yt0, yrm)
             sp.spmv(h, "T", alpha, A, _mk(cuda, Xt, xrm), beta, Ytd)
             expt = oracle.spmv_mv_transpose(rp, ci, v, ncols, Xt, Yt0.copy(), alpha, beta)
-            assert np.max(np.abs(Ytd.cpu().numpy() - expt)) <= 4 * tol + 1e-300
+            gott = Ytd.cpu().numpy()
+            assert np.max(np.abs(gott - expt)) <= 4 * tol + 1e-300
+            R.assert_within(gott, R.spmm_exact(rp, ci, v, Xt, Yt0, alpha, beta, trans=True),
+                            R.spmm_bound(rp, ci, v, Xt, Yt0, alpha, beta, trans=True), f"{h.last_kernel()} T {(xrm, yrm)} a={alpha} b={beta}")
 
 
 @pytest.mark.parametrize("dtype,k", [(np.float32, 16), (np.float64, 5), (np.float32, 40)])
@@ -69,6 +75,7 @@ def test_spmm_hub_rows(cuda, oracle, dtype, k):
     A = sp.CrsMatrix(torch.from_numpy(rp).to(cuda), torch.from_numpy(ci).to(cuda), torch.from_numpy(v).to(cuda), n)
     exp = oracle.spmv_mv(rp, ci, v, n, X, Y0.copy(), 1.5, -0.5)
     tol = 10 * np.finfo(dtype).eps * 9000 * 1.5
+    exact, bound = R.spmm_exact(rp, ci, v, X, Y0, 1.5, -0.5), R.spmm_bound(rp, ci, v, X, Y0, 1.5, -0.5)
     h = sp.SPMVHandle()
     outs = []
     for _ in range(2):
@@ -76,6 +83,7 @@ def test_spmm_hub_rows(cuda, oracle, dtype, k):
         sp.spmv(h, "N", 1.5, A, _mk(cuda, X, True), -0.5, Y)
         outs.append(Y.cpu().numpy())
         assert np.max(np.abs(outs[-1] - exp)) <= tol
+        R.assert_within(outs[-1], exact, bound, h.last_kernel())
     assert np.array_equal(outs[0], outs[1])
     assert h.last_kernel().startswith("spmm_items"), h.last_kernel()
 
@@ -91,18 +99,25 @@ def test_spmm_powerlaw_rows(cuda, oracle):
     A = sp.CrsMatrix(torch.from_numpy(rp).to(cuda), torch.from_numpy(ci).to(cuda), torch.from_numpy(v).to(cuda), n)
     exp = oracle.spmv_mv(rp, ci, v, n, X, np.zeros((n, 16), dtype=np.float32), 1.0, 0.0)
     maxrow = int(np.diff(rp).max())
+    Y0 = np.zeros((n, 16), dtype=np.float32)
+    exact, bound = R.spmm_exact(rp, ci, v, X, Y0, 1.0, 0.0), R.spmm_bound(rp, ci, v, X, Y0, 1.0, 0.0)
     for rowmajor in (True, False):
         Y = _mk(cuda, np.full((n, 16), np.nan, dtype=np.float32), rowmajor)
-        sp.spmv(sp.SPMVHandle(), "N", 1.0, A, _mk(cuda, X, rowmajor), 0.0, Y)
-        err = np.max(np.abs(Y.cpu().numpy() - exp))
+        h = sp.SPMVHandle()
+        sp.spmv(h, "N", 1.0, A, _mk(cuda, X, rowmajor), 0.0, Y)
+        got = Y.cpu().numpy()
+        err = np.max(np.abs(got - exp))
         assert err <= 10 * np.finfo(np.float32).eps * maxrow
+        R.assert_within(got, exact, bound, f"{h.last_kernel()} rowmajor={rowmajor}")
 
 
 def test_config3_full_size(cuda, oracle):
     """BASELINE.json configs[2] at full size: R-MAT scale 23 (8,388,608 rows, 1.3e8 entries, longest row 152,801), fp32,
     16-column multivector, both layouts -- EVERY row against the oracle's CPU multivector loop (O4, spmv_impl.hpp:745-926;
     OpenMP over rows changes no bit of a row).  Criterion (SURVEY.md section 8d): component-wise error scaled by
-    |alpha| sum_j |a_ij||x_jc| + |beta||y0_ic| at most 1e-4 (fp32); alpha = 1.5, beta = 0.5 and the beta == 0 / NaN case."""
+    |alpha| sum_j |a_ij||x_jc| + |beta||y0_ic| at most 1e-4 (fp32); alpha = 1.5, beta = 0.5 and the beta == 0 / NaN case.
+    In addition, 200,000 rows chosen by a fixed seed plus every row of more than 4,096 entries are held to the exact
+    product's per-entry bound (tests/exact_ref.py)."""
     import os
 
     from kokkos_kernels_b200 import matgen, sparse as sp
@@ -117,6 +132,11 @@ def test_config3_full_size(cuda, oracle):
     A = sp.CrsMatrix(torch.from_numpy(rp).to(cuda), torch.from_numpy(ci).to(cuda), torch.from_numpy(v).to(cuda), n)
     h = sp.SPMVHandle()
     scale_a = oracle.spmv_mv(rp, ci, np.abs(v), n, np.abs(X), np.zeros((n, k), dtype=np.float32), 1.0, 0.0, threads=threads)
+    lens = np.diff(rp)
+    sample = np.union1d(np.random.default_rng(8).choice(n, 200000, replace=False), np.flatnonzero(lens > 4096))
+    rp_s = np.concatenate([[0], np.cumsum(lens[sample])]).astype(np.int32)
+    take = np.concatenate([np.arange(rp[r], rp[r + 1]) for r in sample])
+    ci_s, v_s = ci[take], v[take]
     for alpha, beta, rowmajor in ((1.0, 0.0, True), (1.5, 0.5, True), (1.5, 0.5, False)):
         y_in = Y0.copy()
         if beta == 0.0:
@@ -129,3 +149,5 @@ def test_config3_full_size(cuda, oracle):
         scale = abs(alpha) * scale_a.astype(np.float64) + abs(beta) * np.abs(Y0).astype(np.float64)
         err = np.abs(got.astype(np.float64) - exp.astype(np.float64)) / np.maximum(scale, 1e-30)
         assert float(err.max()) <= 1e-4, (alpha, beta, rowmajor, float(err.max()), int(err.argmax()) // k)
+        R.assert_within(got[sample], R.spmm_exact(rp_s, ci_s, v_s, X, Y0[sample], alpha, beta),
+                        R.spmm_bound(rp_s, ci_s, v_s, X, Y0[sample], alpha, beta), f"{h.last_kernel()} rowmajor={rowmajor} (row = index in the sample)")
