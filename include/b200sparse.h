@@ -556,8 +556,9 @@ const char* b200sp_spmv_last_kernel(const b200sp_spmv_plan* plan);
 /* Override the tiled kernel's configuration for this plan before its first
  * use: cfg = index into the built-in table (see DESIGN.md), grid_mult = CTAs
  * per SM (0 = default).  Returns B200SP_ERR_INVALID_ARGUMENT if out of range. */
-/* The analysis a plan caches (tiles, long-row lists, rank-2 work items, chunk tables, cached transpose, host-vector piece
- * bounds) is keyed on (row_ptr pointer, m, n, nnz): a DIFFERENT matrix that reuses the same address with the same shape -- a
+/* The analysis a plan caches (tiles, long-row lists, the tiled kernel's 16-bit column stream, rank-2 work items, chunk tables,
+ * cached transpose, host-vector piece bounds) is keyed on (row_ptr pointer, m, n, nnz), the column stream and the cached
+ * transpose also on the col_idx pointer: a DIFFERENT matrix that reuses the same address with the same shape -- a
  * caching allocator hands the block out again, or row_ptr is edited in place -- would find a stale analysis.  Call this after
  * such a change ("all calls with one handle must use the same matrix", sparse/src/KokkosSparse_spmv_handle.hpp:276-277, is
  * the reference's contract; this is the escape hatch).  Stream-ordered; buffers that depend only on sizes are kept. */

@@ -13,6 +13,8 @@
 //                       NW consumer warps do sub-warp-per-row dot products out of
 //                       shared memory, x gathered through L1 (ld.global.nc),
 //                       warp-shuffle reduction, fused alpha/beta epilogue.
+//                       IDX16 form: col_idx is replaced by the plan's 16-bit in-row
+//                       column deltas + one 32-bit anchor column per row (section 3.5).
 //   spmv_longrow_kernel rows longer than the tile's row limit: one CTA per row (default), or -- opt-in,
 //                       B200SP_SPMV_LONGROWS=seg -- segments of <= 4096 entries + ordered combine.
 //   spmv_vector_kernel  no-analysis fallback (FAST_SETUP, tiny or misaligned
@@ -341,7 +343,9 @@ __global__ void build_tiles_kernel(int m, const int* __restrict__ row_ptr, int n
   if (r1 > r0) {
     s = row_ptr[r0];
     e = row_ptr[r1];
-    // every row but the last ends before (b+1)*T; only a long (> LMAX) last row can exceed the stage
+    // every row but the last ends before (b+1)*T; only a long (> LMAX) last row can exceed the stage.  The clamp also holds
+    // for the 16-bit column form, whose stages start at s & ~7: cap_end <= (s & ~7) + CAP, and every row <= LMAX ends at
+    // most at s + T + LMAX - 1 = s + CAP - 9 < cap_end.
     const int cap_end = (s & ~3) + CAP - 4;
     if (e > cap_end) e = cap_end;
   }
@@ -355,6 +359,31 @@ __global__ void find_long_rows_kernel(int m, const int* __restrict__ row_ptr, in
     if (row_ptr[r + 1] - row_ptr[r] > LMAX) long_rows[atomicAdd(n_long, 1)] = r;
 }
 
+// 16-bit column form of the tiled kernel (DESIGN.md section 3.5): d[j] = col_idx[j] - col_idx[j-1] inside a row, 0 for the
+// first entry of a row; anchor[r] = col_idx[row_ptr[r]], 0 for an empty row.  *bad is set when a row the tiled kernel reads
+// (<= LMAX entries) has an in-row delta outside [0, 65535] (unsorted, or a gap too wide); longer rows go to the long-row
+// kernel, which reads col_idx.  The differences are taken modulo 2^32, so the kernel's anchor + sum of deltas is col_idx[j]
+// exactly whenever no delta was flagged.  8 lanes per row.
+__global__ void build_idx16_kernel(int m, const int* __restrict__ row_ptr, const int* __restrict__ col_idx, int LMAX,
+                                   uint16_t* __restrict__ d, int* __restrict__ anchor, int* __restrict__ bad) {
+  constexpr int G = 8;
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int sl = (int)(t % G);
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x / G;
+  bool wide = false;
+  for (int64_t r = t / G; r < m; r += stride) {
+    const int rs = row_ptr[r], re = row_ptr[r + 1];
+    if (sl == 0) anchor[r] = re > rs ? col_idx[rs] : 0;
+    const bool checked = re - rs <= LMAX;
+    for (int j = rs + sl; j < re; j += G) {
+      const unsigned dl = j == rs ? 0u : (unsigned)col_idx[j] - (unsigned)col_idx[j - 1];
+      wide |= checked && dl > 65535u;
+      d[j] = (uint16_t)dl;
+    }
+  }
+  if (wide) *bad = 1;
+}
+
 // ---------------------------------------------------------------------------
 // the TMA-tiled kernel
 // ---------------------------------------------------------------------------
@@ -365,6 +394,7 @@ template <typename S, int CAP, int STAGES>
 struct TileSmem {
   static constexpr int RCAP = CAP / 2;  // staged row_ptr entries per tile
   alignas(128) S vals[STAGES][CAP];
+  // 32-bit columns; in the 16-bit form the same 4*CAP bytes hold CAP column deltas (uint16) followed by RCAP anchors (int)
   alignas(128) int cols[STAGES][CAP];
   alignas(128) int rows[STAGES][RCAP];
   int4 desc[STAGES];
@@ -372,17 +402,33 @@ struct TileSmem {
   alignas(8) uint64_t empty[STAGES];
 };
 
+// CTAs per SM with 56 registers per thread and the kernel's ring.  Both column forms are held to it: left alone, the compiler
+// gives the 16-bit form's decode up to 91 registers, and the 32-bit form 80 once both share this kernel -- one CTA per SM
+// instead of two in the default configuration.
+template <typename S, int NW, int STAGES, int CAP>
+constexpr int tile_ctas_per_sm() {
+  const int by_regs = 65536 / ((NW + 1) * 32 * 56);
+  const int by_smem = (227 * 1024) / (int)(sizeof(TileSmem<S, CAP, STAGES>) + 128 + 1024);
+  const int c = by_regs < by_smem ? by_regs : by_smem;
+  return c > 1 ? c : 1;
+}
+
 // FWD: the fused all-gather form (b200sp_spmv_forward_f64_i32): the producer warp forwards finished tiles of y to ex.p[0].
 // A template parameter, so that the plain kernel -- the one every roofline number of this repository is measured on -- carries
 // no trace of it.
-template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, bool FWD = false>
-__global__ void __launch_bounds__((NW + 1) * 32)
+// IDX16: columns come from dcol / anchor (build_idx16_kernel) instead of col_idx: 2 bytes per entry plus 4 per row instead of
+// 4 per entry.  Same lanes, same entries per lane, same order: the same bits as the 32-bit form.
+template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, bool IDX16 = false, bool FWD = false>
+__global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES, CAP>())
     spmv_tile_kernel(int m, int64_t nnz, int n_tiles, int LMAX, const int4* __restrict__ tiles,
                      const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
+                     const uint16_t* __restrict__ dcol, const int* __restrict__ anchor,
                      const S* __restrict__ vals, const S* __restrict__ x, S* __restrict__ y, S alpha,
                      S beta, YExtra ex) {
   using Smem = TileSmem<S, CAP, STAGES>;
   constexpr int RCAP = Smem::RCAP;
+  // a stage starts at an entry that is a multiple of EAL: 16 bytes of the narrowest entry stream (bulk-copy alignment)
+  constexpr int EAL = IDX16 ? 8 : 4;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
 
@@ -436,21 +482,26 @@ __global__ void __launch_bounds__((NW + 1) * 32)
       S* sv = sm.vals[stage];
       int* sc = sm.cols[stage];
       int* sr = sm.rows[stage];
-      // entries [s_al, e) -> smem[0 ..); bulk part [s_al, bulk_end), tail by plain loads
-      const int s_al = s & ~3;
-      const int e_up = (e + 3) & ~3;
+      uint16_t* sd = reinterpret_cast<uint16_t*>(sc);  // IDX16: deltas, then anchors
+      int* sa = reinterpret_cast<int*>(sd + CAP);
+      // entries [s_al, e) -> smem[0 ..); bulk part [s_al, bulk_end), tail by plain loads.  nnz_al is a multiple of 4 and
+      // s_al of EAL, so every bulk length is a multiple of 16 bytes.  The delta stream is padded to a multiple of 8 entries
+      // by the plan: its copy [s_al, e_up) is always whole.
+      const int s_al = s & ~(EAL - 1);
+      const int e_up = (e + EAL - 1) & ~(EAL - 1);
       const int bulk_end = (int)dmin64(e_up, nnz_al);
       const int nb = (r1 > r0 && bulk_end > s_al) ? bulk_end - s_al : 0;
+      const int nd = (IDX16 && r1 > r0) ? e_up - s_al : 0;
       if (r1 > r0 && (int64_t)e > nnz_al) {
         const int t0 = (int)dmax64(s_al, nnz_al);
         for (int i = t0 + lane; i < e; i += 32) {
           sv[i - s_al] = vals[i];
-          sc[i - s_al] = col_idx[i];
+          if (!IDX16) sc[i - s_al] = col_idx[i];
         }
       }
       // row_ptr[r0_al .. r1] -> rows[0 ..], at most RCAP entries
       const int r0_al = r0 & ~3;
-      int nrp = 0;
+      int nrp = 0, na = 0;
       if (r1 > r0) {
         const int want_end = min(r1 + 1, r0_al + RCAP);  // exclusive
         const int want_up = (want_end + 3) & ~3;
@@ -460,15 +511,20 @@ __global__ void __launch_bounds__((NW + 1) * 32)
           const int t0 = max(r0_al, rp_al_end);
           for (int i = t0 + lane; i < want_end; i += 32) sr[i - r0_al] = row_ptr[i];
         }
+        // anchors of rows [r0_al, r1), at most RCAP; the plan pads the anchor stream to a multiple of 4 rows
+        if (IDX16) na = min((r1 + 3) & ~3, r0_al + RCAP) - r0_al;
       }
       __syncwarp();
       if (lane == 0) {
         sm.desc[stage] = d;
-        mbar_arrive_expect_tx(&sm.full[stage], (uint32_t)(nb * (sizeof(S) + 4) + nrp * 4));
+        const uint32_t col_bytes = IDX16 ? (uint32_t)(nd * 2 + na * 4) : (uint32_t)(nb * 4);
+        mbar_arrive_expect_tx(&sm.full[stage], (uint32_t)(nb * sizeof(S)) + col_bytes + (uint32_t)(nrp * 4));
         if (nb > 0) {
           bulk_g2s(sv, vals + s_al, (uint32_t)(nb * sizeof(S)), &sm.full[stage], pol);
-          bulk_g2s(sc, col_idx + s_al, (uint32_t)(nb * 4), &sm.full[stage], pol);
+          if (!IDX16) bulk_g2s(sc, col_idx + s_al, (uint32_t)(nb * 4), &sm.full[stage], pol);
         }
+        if (nd > 0) bulk_g2s(sd, dcol + s_al, (uint32_t)(nd * 2), &sm.full[stage], pol);
+        if (na > 0) bulk_g2s(sa, anchor + r0_al, (uint32_t)(na * 4), &sm.full[stage], pol);
         if (nrp > 0) bulk_g2s(sr, row_ptr + r0_al, (uint32_t)(nrp * 4), &sm.full[stage], pol);
       }
       __syncwarp();
@@ -519,10 +575,12 @@ __global__ void __launch_bounds__((NW + 1) * 32)
       mbar_wait(&sm.full[stage], ph);
       const int4 d = sm.desc[stage];
       const int r0 = d.x, r1 = d.y;
-      const int s_al = d.z & ~3;
+      const int s_al = d.z & ~(EAL - 1);
       const int r0_al = r0 & ~3;
       const S* sv = sm.vals[stage];
       const int* sc = sm.cols[stage];
+      const uint16_t* sd = reinterpret_cast<const uint16_t*>(sc);
+      const int* sa = reinterpret_cast<const int*>(sd + CAP);
       const int* sr = sm.rows[stage];
       // absolute row groups of RPW rows are dealt round-robin to the warps
       const int g_first = r0 / RPW;
@@ -530,37 +588,79 @@ __global__ void __launch_bounds__((NW + 1) * 32)
       for (; g * RPW < r1; g += NW) {
         const int r = g * RPW + sub;
         const bool valid = (r >= r0) && (r < r1);
-        int rs = 0, re = 0;
+        int rs = 0, re = 0, col = 0;
         if (valid) {
           const int o = r - r0_al;
           if (o + 1 < RCAP) {
             rs = sr[o];
             re = sr[o + 1];
+            if (IDX16) col = sa[o];
           } else {
             rs = row_ptr[r];
             re = row_ptr[r + 1];
+            if (IDX16) col = anchor[r];
           }
         }
         const bool is_long = (re - rs) > LMAX;
         if (is_long) re = rs;
         S sum = S(0);
         const int jend = re - s_al;
-        // UNR predicated entries per lane per pass: all gathers of a row (<= UNR*LPR entries) are
-        // in flight together -- one memory latency per row instead of one per remainder step
-        for (int j0 = rs + sl - s_al; j0 < jend; j0 += UNR * LPR) {
-          int c[UNR];
-          S av[UNR], xv[UNR];
+        if constexpr (IDX16) {
+          // The passes run over the row, not over the lane's own entries, so that the LPR lanes of a row take the same
+          // number of passes and can shuffle; a lane's extra passes only add +0.0, which leaves its sum's bits alone.
+          // Entry jb + u*LPR + sl is the lane's u-th of the pass, as in the 32-bit form.  Its column is col (the column of
+          // the entry before the pass, the row's anchor at first) plus the deltas of the pass up to it: the totals of slices
+          // 0..u-1 plus the inclusive prefix of slice u over the row's lanes.  One butterfly per slice gives both the prefix
+          // and the total in log2(LPR) shuffles; the UNR slices are independent, so their shuffles overlap.
+          const unsigned gmask = LPR == 32 ? 0xffffffffu : ((1u << LPR) - 1u) << (sub * LPR);
+          for (int jb = rs - s_al; jb < jend; jb += UNR * LPR) {
+            int c[UNR], tot[UNR];
+            S av[UNR], xv[UNR];
 #pragma unroll
-          for (int u = 0; u < UNR; ++u) {
-            const int j = j0 + u * LPR;
-            const bool ok = j < jend;
-            c[u] = ok ? sc[j] : 0;
-            av[u] = ok ? sv[j] : S(0);
+            for (int u = 0; u < UNR; ++u) {
+              const int j = jb + u * LPR + sl;
+              c[u] = tot[u] = j < jend ? (int)sd[j] : 0;  // entries past the row contribute 0
+            }
+#pragma unroll
+            for (int o = 1; o < LPR; o <<= 1) {
+#pragma unroll
+              for (int u = 0; u < UNR; ++u) {
+                const int t = __shfl_xor_sync(gmask, tot[u], o);
+                if (sl & o) c[u] += t;
+                tot[u] += t;
+              }
+            }
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) {
+              c[u] += col;
+              col += tot[u];
+            }
+            // the values are read after the gathers are issued: fewer registers live across the scan
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) xv[u] = (jb + u * LPR + sl < jend) ? ldg(x + c[u]) : S(0);
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) av[u] = (jb + u * LPR + sl < jend) ? sv[jb + u * LPR + sl] : S(0);
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) sum += av[u] * xv[u];
           }
+        } else {
+          // UNR predicated entries per lane per pass: all gathers of a row (<= UNR*LPR entries) are
+          // in flight together -- one memory latency per row instead of one per remainder step
+          for (int j0 = rs + sl - s_al; j0 < jend; j0 += UNR * LPR) {
+            int c[UNR];
+            S av[UNR], xv[UNR];
 #pragma unroll
-          for (int u = 0; u < UNR; ++u) xv[u] = (j0 + u * LPR < jend) ? ldg(x + c[u]) : S(0);
+            for (int u = 0; u < UNR; ++u) {
+              const int j = j0 + u * LPR;
+              const bool ok = j < jend;
+              c[u] = ok ? sc[j] : 0;
+              av[u] = ok ? sv[j] : S(0);
+            }
 #pragma unroll
-          for (int u = 0; u < UNR; ++u) sum += av[u] * xv[u];
+            for (int u = 0; u < UNR; ++u) xv[u] = (j0 + u * LPR < jend) ? ldg(x + c[u]) : S(0);
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) sum += av[u] * xv[u];
+          }
         }
         sum = subwarp_sum<LPR>(sum);
         if (valid && !is_long && sl == 0) store_y(y, r, sum, alpha, beta, ex);
@@ -709,6 +809,17 @@ struct b200sp_spmv_plan {
   cudaEvent_t n_long_event = nullptr;
   bool n_long_known = false;
   int long_cap = 0;
+  // 16-bit column form of the tiled kernel (build_idx16_kernel, DESIGN.md section 3.5), keyed on col_idx on top of the
+  // analysis key and released with the analysis.  Calls use it once the flag, fetched without a host synchronisation like
+  // n_long, says that the matrix qualifies (idx16_state 1); until then, and for a matrix that does not, the 32-bit columns.
+  uint16_t* idx16_d = nullptr;     // nnz deltas, padded to a multiple of 8 entries
+  int* idx16_anchor = nullptr;     // m anchors, padded to a multiple of 4 rows
+  int* idx16_bad = nullptr;        // device flag
+  int* idx16_bad_host = nullptr;   // pinned mirror, valid once idx16_event completed
+  cudaEvent_t idx16_event = nullptr;
+  const int* idx16_key_ci = nullptr;  // col_idx the state below belongs to
+  int idx16_state = 0;                // -1: verdict pending, 0: 32-bit columns, 1: 16-bit form
+  bool idx16_launch = false;          // the current call's tiled launch takes the 16-bit form
   // host-vector staging (b200sp_spmv_hostvec_*)
   void* dx = nullptr;
   void* dy = nullptr;
@@ -785,7 +896,19 @@ struct b200sp_spmv_plan {
 
 namespace b200sp {
 
+static void plan_release_idx16_arrays(b200sp_spmv_plan* p, cudaStream_t st) {
+  void* ptrs[] = {p->idx16_d, p->idx16_anchor, p->idx16_bad};
+  for (void* q : ptrs)
+    if (q) cudaFreeAsync(q, st);
+  p->idx16_d = nullptr;
+  p->idx16_anchor = nullptr;
+  p->idx16_bad = nullptr;
+}
+
 static void plan_release_analysis(b200sp_spmv_plan* p, cudaStream_t st) {
+  plan_release_idx16_arrays(p, st);
+  p->idx16_key_ci = nullptr;
+  p->idx16_state = 0;
   if (p->tiles) cudaFreeAsync(p->tiles, st);
   if (p->long_rows) cudaFreeAsync(p->long_rows, st);
   if (p->n_long) cudaFreeAsync(p->n_long, st);
@@ -859,6 +982,41 @@ static int plan_analyse(b200sp_spmv_plan* p, cudaStream_t st, int cfg, int m, in
   p->key_cfg = cfg;
   p->at_calls = 0;
   p->at_choice = -1;
+  return B200SP_OK;
+}
+
+// The 16-bit column form of the analysed matrix (after plan_analyse): built once per col_idx, stream-ordered; the verdict
+// (every in-row delta of the rows <= LMAX within [0, 65535]) reaches the host through a pinned mirror and an event.  A matrix
+// that does not qualify, or whose streams do not fit in device memory, keeps the 32-bit columns: the call does not fail.
+static int plan_idx16(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, const int* col_idx) {
+  if (p->idx16_key_ci != col_idx) {
+    plan_release_idx16_arrays(p, st);
+    p->idx16_key_ci = col_idx;
+    p->idx16_state = 0;
+    const size_t nd = ((size_t)nnz + 7) & ~(size_t)7, na = ((size_t)m + 3) & ~(size_t)3;
+    if (cudaMallocAsync((void**)&p->idx16_d, sizeof(uint16_t) * nd, st) != cudaSuccess ||
+        cudaMallocAsync((void**)&p->idx16_anchor, sizeof(int) * na, st) != cudaSuccess ||
+        cudaMallocAsync((void**)&p->idx16_bad, sizeof(int), st) != cudaSuccess) {
+      (void)cudaGetLastError();  // not an error of the call: it runs on the 32-bit columns
+      plan_release_idx16_arrays(p, st);
+      return B200SP_OK;
+    }
+    B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_d + nnz, 0, sizeof(uint16_t) * (nd - (size_t)nnz), st));
+    B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_anchor + m, 0, sizeof(int) * (na - (size_t)m), st));
+    B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_bad, 0, sizeof(int), st));
+    const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)m + 31) / 32, (int64_t)sm_count() * 16));
+    build_idx16_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, p->LMAX, p->idx16_d, p->idx16_anchor, p->idx16_bad);
+    B200SP_LAUNCH_CHECK();
+    if (!p->idx16_bad_host) B200SP_CUDA_TRY(cudaMallocHost((void**)&p->idx16_bad_host, sizeof(int)));
+    if (!p->idx16_event) B200SP_CUDA_TRY(cudaEventCreateWithFlags(&p->idx16_event, cudaEventDisableTiming));
+    B200SP_CUDA_TRY(cudaMemcpyAsync(p->idx16_bad_host, p->idx16_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    B200SP_CUDA_TRY(cudaEventRecord(p->idx16_event, st));
+    p->idx16_state = -1;
+  }
+  if (p->idx16_state < 0 && cudaEventQuery(p->idx16_event) == cudaSuccess) {
+    p->idx16_state = *p->idx16_bad_host == 0 ? 1 : 0;
+    if (p->idx16_state == 0) plan_release_idx16_arrays(p, st);  // the key stays: not built again for this matrix
+  }
   return B200SP_OK;
 }
 
@@ -979,11 +1137,13 @@ int spmv_lanes_per_row(int64_t m, int64_t nnz) {  // also used by spmv64.cu: one
   return 32;
 }
 
-template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR = 8>
-static int launch_tile(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr,
-                       const int* col_idx, const S* vals, const S* x, S* y, S alpha, S beta) {
+template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, bool IDX16>
+static int launch_tile_form(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr,
+                            const int* col_idx, const S* vals, const S* x, S* y, S alpha, S beta) {
   using Smem = TileSmem<S, CAP, STAGES>;
-  auto kern = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, false>;
+  auto kern = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, IDX16, false>;
+  const uint16_t* dcol = p->idx16_d;
+  const int* anchor = p->idx16_anchor;
   const size_t smem = sizeof(Smem) + 128;
   static KernelSetup ks;
   int occ_dev = 1;
@@ -998,22 +1158,30 @@ static int launch_tile(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz,
   if constexpr (sizeof(S) == 8 && NW == 16 && STAGES == 4 && CAP == 2048 && UNR == 8) {
     // the forwarding form exists for the default configuration; elsewhere the consumers store to the destination themselves
     if (p->extra.n < 0) {
-      auto kf = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, true>;
+      auto kf = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, IDX16, true>;
       static KernelSetup ksf;
       int occ_f = 1;
       if (int rc = kernel_setup(ksf, kf, (NW + 1) * 32, smem, &occ_f)) return rc;
-      kf<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, vals, x, y, alpha, beta,
-                                            p->extra);
+      kf<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, dcol, anchor, vals, x, y,
+                                            alpha, beta, p->extra);
       launched = true;
     }
   }
   if (!launched)
-    kern<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, vals, x, y,
+    kern<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, dcol, anchor, vals, x, y,
                                             alpha, beta, direct_extra(p->extra));
   B200SP_LAUNCH_CHECK();
-  snprintf(p->last_kernel, sizeof(p->last_kernel), "tile<%s,LPR=%d,NW=%d,STAGES=%d,CAP=%d,UNR=%d>grid=%d",
-           sizeof(S) == 8 ? "f64" : "f32", LPR, NW, STAGES, CAP, UNR, grid);
+  snprintf(p->last_kernel, sizeof(p->last_kernel), "tile<%s,LPR=%d,NW=%d,STAGES=%d,CAP=%d,UNR=%d,IDX=%s>grid=%d",
+           sizeof(S) == 8 ? "f64" : "f32", LPR, NW, STAGES, CAP, UNR, IDX16 ? "u16" : "i32", grid);
   return B200SP_OK;
+}
+
+template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR = 8>
+static int launch_tile(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr,
+                       const int* col_idx, const S* vals, const S* x, S* y, S alpha, S beta) {
+  if (p->idx16_launch)
+    return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, true>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
+  return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, false>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
 }
 
 template <typename S, int LPR>
@@ -1181,6 +1349,14 @@ static int spmv_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   const int cfg = p->cfg >= 0 ? p->cfg : 8;  // CAP=2048, 4 stages, 16 consumer warps, 2 CTAs/SM
   int rc = plan_analyse<S>(p, st, cfg, m, n, nnz, row_ptr);
   if (rc) return rc;
+  // B200SP_SPMV_IDX16=0: the 32-bit columns (A/B comparisons; the 16-bit stream is not built for this call)
+  const char* i16 = getenv("B200SP_SPMV_IDX16");
+  p->idx16_launch = false;
+  if (!(i16 && i16[0] == '0')) {
+    rc = plan_idx16(p, st, m, nnz, row_ptr, col_idx);
+    if (rc) return rc;
+    p->idx16_launch = p->idx16_state == 1;
+  }
   const int lpr = p->lpr > 0 ? p->lpr : lpr_auto;
   // ---- self-tuning (only for untuned plans on whole-matrix launches)
   const bool autotune = p->cfg < 0 && p->range_hi < 0 && p->extra.n == 0 && getenv("B200SP_NO_AUTOTUNE") == nullptr;
@@ -1317,6 +1493,11 @@ int b200sp_spmv_plan_destroy(b200sp_spmv_plan* p, void* stream) {
     cudaEventDestroy(p->n_long_event);
   }
   if (p->n_long_host) cudaFreeHost(p->n_long_host);
+  if (p->idx16_event) {
+    cudaEventSynchronize(p->idx16_event);
+    cudaEventDestroy(p->idx16_event);
+  }
+  if (p->idx16_bad_host) cudaFreeHost(p->idx16_bad_host);
   delete p;
   return B200SP_OK;
 }
@@ -1340,8 +1521,8 @@ int b200sp_spmv_plan_set_option(b200sp_spmv_plan* p, int option, int value) {
 int b200sp_spmv_plan_invalidate(b200sp_spmv_plan* p, void* stream) {
   B200SP_REQUIRE(p != nullptr, "spmv_plan_invalidate: null plan");
   cudaStream_t st = (cudaStream_t)stream;
-  // everything derived from the STRUCTURE of the matrix the plan last saw: tiles, long rows, rank-2 tiles / segments / items,
-  // chunk table, cached transpose, host-vector piece bounds, self-tuning state.  Buffers that only depend on sizes stay.
+  // everything derived from the STRUCTURE of the matrix the plan last saw: tiles, long rows, 16-bit column stream, rank-2
+  // tiles / segments / items, chunk table, cached transpose, host-vector piece bounds, self-tuning state.  Buffers that only depend on sizes stay.
   plan_release_analysis(p, st);
   plan_release_mm(p, st);
   if (p->chunk_row) cudaFreeAsync(p->chunk_row, st);
