@@ -15,6 +15,8 @@
 //                       warp-shuffle reduction, fused alpha/beta epilogue.
 //                       IDX16 form: col_idx is replaced by the plan's 16-bit in-row
 //                       column deltas + one 32-bit anchor column per row (section 3.5).
+//                       Pattern form: one 16-bit pattern start per row into a dictionary
+//                       of in-row column offsets, + the anchors (section 3.6).
 //   spmv_longrow_kernel rows longer than the tile's row limit: one CTA per row (default), or -- opt-in,
 //                       B200SP_SPMV_LONGROWS=seg -- segments of <= 4096 entries + ordered combine.
 //   spmv_vector_kernel  no-analysis fallback (FAST_SETUP, tiny or misaligned
@@ -384,6 +386,139 @@ __global__ void build_idx16_kernel(int m, const int* __restrict__ row_ptr, const
   if (wide) *bad = 1;
 }
 
+// Pattern form of the tiled kernel (DESIGN.md section 3.6): the offsets col_idx[j] - anchor[r] of a row, taken over the row,
+// form its pattern.  Matrices from structured grids have a handful of patterns (lap27: 8), so a row's columns are its anchor
+// plus one uint16 pid[r], the start of its pattern in a dictionary of at most DCAP offsets that the tiled kernel keeps in
+// shared memory.  dict[DCAP] holds the dictionary's used length.  Three passes, stream-ordered: hash every row of 1..LMAX
+// entries into a small open-addressing table; lay the table's patterns out in the dictionary; then set pid[r] and check every
+// entry of every such row against the dictionary, so that a hash collision only makes the matrix fall back.  *bad is set
+// when the table or the dictionary overflows or an entry does not match.
+constexpr int DCAP = 1024;         // dictionary offsets (4 KB of shared memory)
+constexpr int PAT_SLOTS = 2048;    // hash table slots: a qualifying matrix has at most DCAP patterns
+constexpr int PAT_PROBES = 64;     // linear probes before the table counts as full
+
+__device__ __forceinline__ unsigned long long pat_mix(unsigned long long z) {  // splitmix64 finaliser
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+
+// 8 lanes per row: the hash of (length, offsets) is a sum of per-entry hashes, so the lanes add theirs with three shuffles
+__global__ void pattern_hash_kernel(int m, const int* __restrict__ row_ptr, const int* __restrict__ col_idx, int LMAX,
+                                    unsigned long long* __restrict__ table, int* __restrict__ rep, int* __restrict__ row_slot,
+                                    int* __restrict__ bad) {
+  constexpr int G = 8;
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int sl = (int)(t % G);
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x / G;
+  const int64_t r_end = ((int64_t)m + G - 1) / G * G;  // whole warps (4 rows each) run every pass: the shuffles
+  for (int64_t r = t / G; r < r_end; r += stride) {
+    int rs = 0, re = 0;
+    if (r < m) {
+      rs = row_ptr[r];
+      re = row_ptr[r + 1];
+    }
+    const int len = re - rs;
+    const bool mine = len >= 1 && len <= LMAX;
+    unsigned long long h = 0;
+    if (mine) {
+      const unsigned c0 = (unsigned)col_idx[rs];
+      for (int k = sl; k < len; k += G) h += pat_mix(((unsigned long long)k << 32) | ((unsigned)col_idx[rs + k] - c0));
+    }
+#pragma unroll
+    for (int o = 1; o < G; o <<= 1) h += __shfl_xor_sync(0xffffffffu, h, o);
+    if (!mine || sl != 0) continue;
+    h += pat_mix(0x9e3779b97f4a7c15ull ^ (unsigned long long)len);
+    if (h == 0) h = 1;  // 0 marks an empty slot
+    int slot = -1;
+    if (__ldcg(bad) == 0) {
+      // load first: the few distinct keys are inserted once, then every row finds its key without an atomic
+      for (int q = 0, s = (int)(h % PAT_SLOTS); q < PAT_PROBES; ++q, s = (s + 1) % PAT_SLOTS) {
+        unsigned long long k = __ldcg(table + s);
+        if (k == 0) {
+          k = atomicCAS(table + s, 0ull, h);
+          if (k == 0) rep[s] = (int)r;  // the inserting row represents the slot
+        }
+        if (k == 0 || k == h) {
+          slot = s;
+          break;
+        }
+      }
+      if (slot < 0) *bad = 1;
+    }
+    row_slot[r] = slot;
+  }
+}
+
+// one CTA of 256 threads, PAT_SLOTS / 256 consecutive slots each: pattern starts in slot order
+__global__ void __launch_bounds__(256) pattern_dict_kernel(const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
+                                                           const unsigned long long* __restrict__ table, const int* __restrict__ rep,
+                                                           int* __restrict__ slot_start, int* __restrict__ slot_len,
+                                                           int* __restrict__ dict, int* __restrict__ bad) {
+  constexpr int PER = PAT_SLOTS / 256;
+  __shared__ int part[257];
+  if (*bad) return;  // the same value for every thread
+  const int s0 = threadIdx.x * PER;
+  int len[PER], sum = 0;
+#pragma unroll
+  for (int i = 0; i < PER; ++i) {
+    len[i] = 0;
+    if (table[s0 + i]) len[i] = row_ptr[rep[s0 + i] + 1] - row_ptr[rep[s0 + i]];
+    sum += len[i];
+  }
+  part[threadIdx.x + 1] = sum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    part[0] = 0;
+    for (int i = 1; i <= 256; ++i) part[i] += part[i - 1];
+    dict[DCAP] = part[256];
+    if (part[256] > DCAP) *bad = 1;
+  }
+  __syncthreads();
+  if (part[256] > DCAP) return;
+  int base = part[threadIdx.x];
+#pragma unroll
+  for (int i = 0; i < PER; ++i) {
+    slot_start[s0 + i] = base;
+    slot_len[s0 + i] = len[i];
+    if (len[i]) {
+      const int rs = row_ptr[rep[s0 + i]];
+      const unsigned c0 = (unsigned)col_idx[rs];
+      for (int k = 0; k < len[i]; ++k) dict[base + k] = (int)((unsigned)col_idx[rs + k] - c0);
+    }
+    base += len[i];
+  }
+}
+
+// pid[r] for every row (0 for empty and long rows), and the check of every entry the tiled kernel will rebuild
+__global__ void pattern_assign_kernel(int m, const int* __restrict__ row_ptr, const int* __restrict__ col_idx, int LMAX,
+                                      const int* __restrict__ row_slot, const int* __restrict__ slot_start,
+                                      const int* __restrict__ slot_len, const int* __restrict__ dict,
+                                      uint16_t* __restrict__ pid, int* __restrict__ bad) {
+  constexpr int G = 8;
+  if (*bad) return;
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int sl = (int)(t % G);
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x / G;
+  bool wrong = false;
+  for (int64_t r = t / G; r < m; r += stride) {
+    const int rs = row_ptr[r], len = row_ptr[r + 1] - rs;
+    int start = 0;
+    if (len >= 1 && len <= LMAX) {
+      const int s = row_slot[r];
+      start = slot_start[s];
+      if (slot_len[s] != len) {
+        wrong = true;
+      } else {
+        const unsigned c0 = (unsigned)col_idx[rs];
+        for (int k = sl; k < len; k += G) wrong |= (int)((unsigned)col_idx[rs + k] - c0) != dict[start + k];
+      }
+    }
+    if (sl == 0) pid[r] = (uint16_t)start;
+  }
+  if (wrong) *bad = 1;
+}
+
 // ---------------------------------------------------------------------------
 // the TMA-tiled kernel
 // ---------------------------------------------------------------------------
@@ -402,6 +537,20 @@ struct TileSmem {
   alignas(8) uint64_t empty[STAGES];
 };
 
+// column area of the ring (TileSmem::cols) in the pattern form: per stage RCAP anchors and RCAP pattern starts, 3*CAP of its
+// 4*CAP bytes, and one dictionary in the STAGES*CAP bytes that frees (>= 5 KB in every configuration).  The ring is no larger
+// than in the 32-bit form, so occupancy is the same.
+template <int CAP, int STAGES>
+struct TilePatCols {
+  int anchor[STAGES][CAP / 2];
+  uint16_t pid[STAGES][CAP / 2];
+  int dict[DCAP];
+};
+
+// which columns the tiled kernel reads: col_idx, the plan's 16-bit deltas + anchors (section 3.5), or its pattern starts +
+// anchors + dictionary (section 3.6)
+enum TileCols { COLS_I32 = 0, COLS_DELTA = 1, COLS_PAT = 2 };
+
 // CTAs per SM with 56 registers per thread and the kernel's ring.  Both column forms are held to it: left alone, the compiler
 // gives the 16-bit form's decode up to 91 registers, and the 32-bit form 80 once both share this kernel -- one CTA per SM
 // instead of two in the default configuration.
@@ -416,25 +565,36 @@ constexpr int tile_ctas_per_sm() {
 // FWD: the fused all-gather form (b200sp_spmv_forward_f64_i32): the producer warp forwards finished tiles of y to ex.p[0].
 // A template parameter, so that the plain kernel -- the one every roofline number of this repository is measured on -- carries
 // no trace of it.
-// IDX16: columns come from dcol / anchor (build_idx16_kernel) instead of col_idx: 2 bytes per entry plus 4 per row instead of
-// 4 per entry.  Same lanes, same entries per lane, same order: the same bits as the 32-bit form.
-template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, bool IDX16 = false, bool FWD = false>
+// COLS_DELTA: columns come from c16 (deltas) / anchor (build_idx16_kernel) instead of col_idx: 2 bytes per entry plus 4 per
+// row instead of 4 per entry.  COLS_PAT: from c16 (pattern starts) / anchor / dict (pattern_*_kernel): 6 bytes per row.
+// Same lanes, same entries per lane, same order: the same bits as the 32-bit form.
+template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, int COLS = COLS_I32, bool FWD = false>
 __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES, CAP>())
     spmv_tile_kernel(int m, int64_t nnz, int n_tiles, int LMAX, const int4* __restrict__ tiles,
                      const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
-                     const uint16_t* __restrict__ dcol, const int* __restrict__ anchor,
+                     const uint16_t* __restrict__ c16, const int* __restrict__ anchor, const int* __restrict__ dict,
                      const S* __restrict__ vals, const S* __restrict__ x, S* __restrict__ y, S alpha,
                      S beta, YExtra ex) {
   using Smem = TileSmem<S, CAP, STAGES>;
+  using PatCols = TilePatCols<CAP, STAGES>;
+  static_assert(sizeof(PatCols) <= sizeof(int) * STAGES * CAP, "the pattern form's columns must fit the 32-bit ring");
   constexpr int RCAP = Smem::RCAP;
+  constexpr bool IDX16 = COLS == COLS_DELTA, PAT = COLS == COLS_PAT;
   // a stage starts at an entry that is a multiple of EAL: 16 bytes of the narrowest entry stream (bulk-copy alignment)
   constexpr int EAL = IDX16 ? 8 : 4;
+  // ... and at a row that is a multiple of RAL: 16 bytes of the narrowest row stream
+  constexpr int RAL = PAT ? 8 : 4;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+  PatCols& pc = *reinterpret_cast<PatCols*>(&sm.cols[0][0]);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
+  if constexpr (PAT) {
+    const int dl = dict[DCAP];  // used length
+    for (int i = threadIdx.x; i < dl; i += blockDim.x) pc.dict[i] = dict[i];
+  }
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) {
@@ -483,7 +643,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
       int* sc = sm.cols[stage];
       int* sr = sm.rows[stage];
       uint16_t* sd = reinterpret_cast<uint16_t*>(sc);  // IDX16: deltas, then anchors
-      int* sa = reinterpret_cast<int*>(sd + CAP);
+      int* sa = PAT ? pc.anchor[stage] : reinterpret_cast<int*>(sd + CAP);
       // entries [s_al, e) -> smem[0 ..); bulk part [s_al, bulk_end), tail by plain loads.  nnz_al is a multiple of 4 and
       // s_al of EAL, so every bulk length is a multiple of 16 bytes.  The delta stream is padded to a multiple of 8 entries
       // by the plan: its copy [s_al, e_up) is always whole.
@@ -496,12 +656,12 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
         const int t0 = (int)dmax64(s_al, nnz_al);
         for (int i = t0 + lane; i < e; i += 32) {
           sv[i - s_al] = vals[i];
-          if (!IDX16) sc[i - s_al] = col_idx[i];
+          if (COLS == COLS_I32) sc[i - s_al] = col_idx[i];
         }
       }
       // row_ptr[r0_al .. r1] -> rows[0 ..], at most RCAP entries
-      const int r0_al = r0 & ~3;
-      int nrp = 0, na = 0;
+      const int r0_al = r0 & ~(RAL - 1);
+      int nrp = 0, na = 0, np = 0;
       if (r1 > r0) {
         const int want_end = min(r1 + 1, r0_al + RCAP);  // exclusive
         const int want_up = (want_end + 3) & ~3;
@@ -512,18 +672,21 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
           for (int i = t0 + lane; i < want_end; i += 32) sr[i - r0_al] = row_ptr[i];
         }
         // anchors of rows [r0_al, r1), at most RCAP; the plan pads the anchor stream to a multiple of 4 rows
-        if (IDX16) na = min((r1 + 3) & ~3, r0_al + RCAP) - r0_al;
+        if (COLS != COLS_I32) na = min((r1 + 3) & ~3, r0_al + RCAP) - r0_al;
+        // PAT: pattern starts of the same rows; the plan pads that stream to a multiple of 8 rows
+        if (PAT) np = min((r1 + 7) & ~7, r0_al + RCAP) - r0_al;
       }
       __syncwarp();
       if (lane == 0) {
         sm.desc[stage] = d;
-        const uint32_t col_bytes = IDX16 ? (uint32_t)(nd * 2 + na * 4) : (uint32_t)(nb * 4);
+        const uint32_t col_bytes = COLS == COLS_I32 ? (uint32_t)(nb * 4) : (uint32_t)(nd * 2 + na * 4 + np * 2);
         mbar_arrive_expect_tx(&sm.full[stage], (uint32_t)(nb * sizeof(S)) + col_bytes + (uint32_t)(nrp * 4));
         if (nb > 0) {
           bulk_g2s(sv, vals + s_al, (uint32_t)(nb * sizeof(S)), &sm.full[stage], pol);
-          if (!IDX16) bulk_g2s(sc, col_idx + s_al, (uint32_t)(nb * 4), &sm.full[stage], pol);
+          if (COLS == COLS_I32) bulk_g2s(sc, col_idx + s_al, (uint32_t)(nb * 4), &sm.full[stage], pol);
         }
-        if (nd > 0) bulk_g2s(sd, dcol + s_al, (uint32_t)(nd * 2), &sm.full[stage], pol);
+        if (nd > 0) bulk_g2s(sd, c16 + s_al, (uint32_t)(nd * 2), &sm.full[stage], pol);
+        if (np > 0) bulk_g2s(pc.pid[stage], c16 + r0_al, (uint32_t)(np * 2), &sm.full[stage], pol);
         if (na > 0) bulk_g2s(sa, anchor + r0_al, (uint32_t)(na * 4), &sm.full[stage], pol);
         if (nrp > 0) bulk_g2s(sr, row_ptr + r0_al, (uint32_t)(nrp * 4), &sm.full[stage], pol);
       }
@@ -576,11 +739,11 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
       const int4 d = sm.desc[stage];
       const int r0 = d.x, r1 = d.y;
       const int s_al = d.z & ~(EAL - 1);
-      const int r0_al = r0 & ~3;
+      const int r0_al = r0 & ~(RAL - 1);
       const S* sv = sm.vals[stage];
       const int* sc = sm.cols[stage];
       const uint16_t* sd = reinterpret_cast<const uint16_t*>(sc);
-      const int* sa = reinterpret_cast<const int*>(sd + CAP);
+      const int* sa = PAT ? pc.anchor[stage] : reinterpret_cast<const int*>(sd + CAP);
       const int* sr = sm.rows[stage];
       // absolute row groups of RPW rows are dealt round-robin to the warps
       const int g_first = r0 / RPW;
@@ -588,17 +751,19 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
       for (; g * RPW < r1; g += NW) {
         const int r = g * RPW + sub;
         const bool valid = (r >= r0) && (r < r1);
-        int rs = 0, re = 0, col = 0;
+        int rs = 0, re = 0, col = 0, pb = 0;
         if (valid) {
           const int o = r - r0_al;
           if (o + 1 < RCAP) {
             rs = sr[o];
             re = sr[o + 1];
-            if (IDX16) col = sa[o];
+            if (COLS != COLS_I32) col = sa[o];
+            if (PAT) pb = pc.pid[stage][o];
           } else {
             rs = row_ptr[r];
             re = row_ptr[r + 1];
-            if (IDX16) col = anchor[r];
+            if (COLS != COLS_I32) col = anchor[r];
+            if (PAT) pb = c16[r];
           }
         }
         const bool is_long = (re - rs) > LMAX;
@@ -640,6 +805,25 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
             for (int u = 0; u < UNR; ++u) xv[u] = (jb + u * LPR + sl < jend) ? ldg(x + c[u]) : S(0);
 #pragma unroll
             for (int u = 0; u < UNR; ++u) av[u] = (jb + u * LPR + sl < jend) ? sv[jb + u * LPR + sl] : S(0);
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) sum += av[u] * xv[u];
+          }
+        } else if constexpr (PAT) {
+          // the 32-bit form's loop with col + dict[pb + k] for the column of the row's entry k: the rows of a warp mostly
+          // share a pattern, so the dictionary reads are mostly broadcasts
+          const int db = pb - (rs - s_al);
+          for (int j0 = rs + sl - s_al; j0 < jend; j0 += UNR * LPR) {
+            int c[UNR];
+            S av[UNR], xv[UNR];
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) {
+              const int j = j0 + u * LPR;
+              const bool ok = j < jend;
+              c[u] = ok ? col + pc.dict[db + j] : 0;
+              av[u] = ok ? sv[j] : S(0);
+            }
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) xv[u] = (j0 + u * LPR < jend) ? ldg(x + c[u]) : S(0);
 #pragma unroll
             for (int u = 0; u < UNR; ++u) sum += av[u] * xv[u];
           }
@@ -812,14 +996,18 @@ struct b200sp_spmv_plan {
   // 16-bit column form of the tiled kernel (build_idx16_kernel, DESIGN.md section 3.5), keyed on col_idx on top of the
   // analysis key and released with the analysis.  Calls use it once the flag, fetched without a host synchronisation like
   // n_long, says that the matrix qualifies (idx16_state 1); until then, and for a matrix that does not, the 32-bit columns.
+  // The pattern form (pattern_*_kernel, section 3.6) is built in the same call and its verdict comes with the same event;
+  // once it is chosen the deltas are released.
   uint16_t* idx16_d = nullptr;     // nnz deltas, padded to a multiple of 8 entries
   int* idx16_anchor = nullptr;     // m anchors, padded to a multiple of 4 rows
-  int* idx16_bad = nullptr;        // device flag
+  uint16_t* pat_pid = nullptr;     // m pattern starts, padded to a multiple of 8 rows
+  int* pat_dict = nullptr;         // DCAP offsets + the used length
+  int* idx16_bad = nullptr;        // device flags: [0] deltas, [1] patterns
   int* idx16_bad_host = nullptr;   // pinned mirror, valid once idx16_event completed
   cudaEvent_t idx16_event = nullptr;
   const int* idx16_key_ci = nullptr;  // col_idx the state below belongs to
-  int idx16_state = 0;                // -1: verdict pending, 0: 32-bit columns, 1: 16-bit form
-  bool idx16_launch = false;          // the current call's tiled launch takes the 16-bit form
+  int idx16_state = 0;                // -1: verdict pending, else the TileCols of the matrix
+  int cols_launch = COLS_I32;         // the current call's tiled launch takes this form
   // host-vector staging (b200sp_spmv_hostvec_*)
   void* dx = nullptr;
   void* dy = nullptr;
@@ -897,11 +1085,13 @@ struct b200sp_spmv_plan {
 namespace b200sp {
 
 static void plan_release_idx16_arrays(b200sp_spmv_plan* p, cudaStream_t st) {
-  void* ptrs[] = {p->idx16_d, p->idx16_anchor, p->idx16_bad};
+  void* ptrs[] = {p->idx16_d, p->idx16_anchor, p->pat_pid, p->pat_dict, p->idx16_bad};
   for (void* q : ptrs)
     if (q) cudaFreeAsync(q, st);
   p->idx16_d = nullptr;
   p->idx16_anchor = nullptr;
+  p->pat_pid = nullptr;
+  p->pat_dict = nullptr;
   p->idx16_bad = nullptr;
 }
 
@@ -985,37 +1175,77 @@ static int plan_analyse(b200sp_spmv_plan* p, cudaStream_t st, int cfg, int m, in
   return B200SP_OK;
 }
 
-// The 16-bit column form of the analysed matrix (after plan_analyse): built once per col_idx, stream-ordered; the verdict
-// (every in-row delta of the rows <= LMAX within [0, 65535]) reaches the host through a pinned mirror and an event.  A matrix
-// that does not qualify, or whose streams do not fit in device memory, keeps the 32-bit columns: the call does not fail.
+// The 16-bit column forms of the analysed matrix (after plan_analyse): built once per col_idx, stream-ordered.  The verdicts
+// (deltas: every in-row delta of the rows <= LMAX within [0, 65535]; patterns: every such row matches the dictionary, which
+// holds at most DCAP offsets) reach the host together through a pinned mirror and an event.  The pattern form wins when the
+// matrix qualifies for both.  A matrix that qualifies for neither, or whose streams do not fit in device memory, keeps the
+// 32-bit columns: the call does not fail.  B200SP_SPMV_PATTERN=0 at the build leaves out the pattern analysis.
 static int plan_idx16(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, const int* col_idx) {
+  // the deltas of a pattern-form matrix go on the call after the one that learnt the verdict: a call never frees the streams
+  // it has built, so what a handle holds after its first call does not depend on how soon the verdict arrived
+  if (p->idx16_state == COLS_PAT && p->idx16_d) {
+    cudaFreeAsync(p->idx16_d, st);
+    p->idx16_d = nullptr;
+  }
   if (p->idx16_key_ci != col_idx) {
     plan_release_idx16_arrays(p, st);
     p->idx16_key_ci = col_idx;
-    p->idx16_state = 0;
-    const size_t nd = ((size_t)nnz + 7) & ~(size_t)7, na = ((size_t)m + 3) & ~(size_t)3;
+    p->idx16_state = COLS_I32;
+    const char* pe = getenv("B200SP_SPMV_PATTERN");
+    const bool pat = !(pe && pe[0] == '0');
+    const size_t nd = ((size_t)nnz + 7) & ~(size_t)7, na = ((size_t)m + 3) & ~(size_t)3, np = ((size_t)m + 7) & ~(size_t)7;
+    // hash table, slot representatives, slot starts, slot lengths, row slots: freed once the pattern passes are issued
+    const size_t scratch = sizeof(unsigned long long) * PAT_SLOTS + sizeof(int) * (3 * (size_t)PAT_SLOTS + (size_t)m);
+    unsigned long long* table = nullptr;
     if (cudaMallocAsync((void**)&p->idx16_d, sizeof(uint16_t) * nd, st) != cudaSuccess ||
         cudaMallocAsync((void**)&p->idx16_anchor, sizeof(int) * na, st) != cudaSuccess ||
-        cudaMallocAsync((void**)&p->idx16_bad, sizeof(int), st) != cudaSuccess) {
+        cudaMallocAsync((void**)&p->idx16_bad, 2 * sizeof(int), st) != cudaSuccess ||
+        (pat && (cudaMallocAsync((void**)&p->pat_pid, sizeof(uint16_t) * np, st) != cudaSuccess ||
+                 cudaMallocAsync((void**)&p->pat_dict, sizeof(int) * (DCAP + 1), st) != cudaSuccess ||
+                 cudaMallocAsync((void**)&table, scratch, st) != cudaSuccess))) {
       (void)cudaGetLastError();  // not an error of the call: it runs on the 32-bit columns
+      if (table) cudaFreeAsync(table, st);
       plan_release_idx16_arrays(p, st);
       return B200SP_OK;
     }
     B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_d + nnz, 0, sizeof(uint16_t) * (nd - (size_t)nnz), st));
     B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_anchor + m, 0, sizeof(int) * (na - (size_t)m), st));
-    B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_bad, 0, sizeof(int), st));
+    B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_bad, 0, 2 * sizeof(int), st));
     const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)m + 31) / 32, (int64_t)sm_count() * 16));
     build_idx16_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, p->LMAX, p->idx16_d, p->idx16_anchor, p->idx16_bad);
     B200SP_LAUNCH_CHECK();
-    if (!p->idx16_bad_host) B200SP_CUDA_TRY(cudaMallocHost((void**)&p->idx16_bad_host, sizeof(int)));
+    if (pat) {
+      int* rep = reinterpret_cast<int*>(table + PAT_SLOTS);
+      int* slot_start = rep + PAT_SLOTS;
+      int* slot_len = slot_start + PAT_SLOTS;
+      int* row_slot = slot_len + PAT_SLOTS;
+      B200SP_CUDA_TRY(cudaMemsetAsync(table, 0, sizeof(unsigned long long) * PAT_SLOTS, st));
+      B200SP_CUDA_TRY(cudaMemsetAsync(p->pat_pid + m, 0, sizeof(uint16_t) * (np - (size_t)m), st));
+      pattern_hash_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, p->LMAX, table, rep, row_slot, p->idx16_bad + 1);
+      B200SP_LAUNCH_CHECK();
+      pattern_dict_kernel<<<1, 256, 0, st>>>(row_ptr, col_idx, table, rep, slot_start, slot_len, p->pat_dict, p->idx16_bad + 1);
+      B200SP_LAUNCH_CHECK();
+      pattern_assign_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, p->LMAX, row_slot, slot_start, slot_len, p->pat_dict,
+                                                    p->pat_pid, p->idx16_bad + 1);
+      B200SP_LAUNCH_CHECK();
+      cudaFreeAsync(table, st);
+    }
+    if (!p->idx16_bad_host) B200SP_CUDA_TRY(cudaMallocHost((void**)&p->idx16_bad_host, 2 * sizeof(int)));
     if (!p->idx16_event) B200SP_CUDA_TRY(cudaEventCreateWithFlags(&p->idx16_event, cudaEventDisableTiming));
-    B200SP_CUDA_TRY(cudaMemcpyAsync(p->idx16_bad_host, p->idx16_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    B200SP_CUDA_TRY(cudaMemcpyAsync(p->idx16_bad_host, p->idx16_bad, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
     B200SP_CUDA_TRY(cudaEventRecord(p->idx16_event, st));
     p->idx16_state = -1;
   }
   if (p->idx16_state < 0 && cudaEventQuery(p->idx16_event) == cudaSuccess) {
-    p->idx16_state = *p->idx16_bad_host == 0 ? 1 : 0;
-    if (p->idx16_state == 0) plan_release_idx16_arrays(p, st);  // the key stays: not built again for this matrix
+    const int* bad = p->idx16_bad_host;
+    p->idx16_state = (p->pat_pid && bad[1] == 0) ? COLS_PAT : bad[0] == 0 ? COLS_DELTA : COLS_I32;
+    if (p->idx16_state == COLS_I32) plan_release_idx16_arrays(p, st);  // the key stays: not built again for this matrix
+    if (p->idx16_state == COLS_DELTA) {
+      if (p->pat_pid) cudaFreeAsync(p->pat_pid, st);
+      if (p->pat_dict) cudaFreeAsync(p->pat_dict, st);
+      p->pat_pid = nullptr;
+      p->pat_dict = nullptr;
+    }
   }
   return B200SP_OK;
 }
@@ -1137,13 +1367,14 @@ int spmv_lanes_per_row(int64_t m, int64_t nnz) {  // also used by spmv64.cu: one
   return 32;
 }
 
-template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, bool IDX16>
+template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, int COLS>
 static int launch_tile_form(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr,
                             const int* col_idx, const S* vals, const S* x, S* y, S alpha, S beta) {
   using Smem = TileSmem<S, CAP, STAGES>;
-  auto kern = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, IDX16, false>;
-  const uint16_t* dcol = p->idx16_d;
+  auto kern = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, COLS, false>;
+  const uint16_t* c16 = COLS == COLS_PAT ? p->pat_pid : p->idx16_d;
   const int* anchor = p->idx16_anchor;
+  const int* dict = p->pat_dict;
   const size_t smem = sizeof(Smem) + 128;
   static KernelSetup ks;
   int occ_dev = 1;
@@ -1158,30 +1389,34 @@ static int launch_tile_form(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t
   if constexpr (sizeof(S) == 8 && NW == 16 && STAGES == 4 && CAP == 2048 && UNR == 8) {
     // the forwarding form exists for the default configuration; elsewhere the consumers store to the destination themselves
     if (p->extra.n < 0) {
-      auto kf = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, IDX16, true>;
+      auto kf = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, COLS, true>;
       static KernelSetup ksf;
       int occ_f = 1;
       if (int rc = kernel_setup(ksf, kf, (NW + 1) * 32, smem, &occ_f)) return rc;
-      kf<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, dcol, anchor, vals, x, y,
-                                            alpha, beta, p->extra);
+      kf<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals,
+                                            x, y, alpha, beta, p->extra);
       launched = true;
     }
   }
   if (!launched)
-    kern<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, dcol, anchor, vals, x, y,
-                                            alpha, beta, direct_extra(p->extra));
+    kern<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals,
+                                            x, y, alpha, beta, direct_extra(p->extra));
   B200SP_LAUNCH_CHECK();
-  snprintf(p->last_kernel, sizeof(p->last_kernel), "tile<%s,LPR=%d,NW=%d,STAGES=%d,CAP=%d,UNR=%d,IDX=%s>grid=%d",
-           sizeof(S) == 8 ? "f64" : "f32", LPR, NW, STAGES, CAP, UNR, IDX16 ? "u16" : "i32", grid);
+  // the pattern form is a sub-form of the 16-bit column data (pattern starts + anchors): IDX=u16, and COLS names the source
+  static const char* const kColsLabel[] = {"IDX=i32", "IDX=u16,COLS=delta", "IDX=u16,COLS=pat"};
+  snprintf(p->last_kernel, sizeof(p->last_kernel), "tile<%s,LPR=%d,NW=%d,STAGES=%d,CAP=%d,UNR=%d,%s>grid=%d",
+           sizeof(S) == 8 ? "f64" : "f32", LPR, NW, STAGES, CAP, UNR, kColsLabel[COLS], grid);
   return B200SP_OK;
 }
 
 template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR = 8>
 static int launch_tile(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr,
                        const int* col_idx, const S* vals, const S* x, S* y, S alpha, S beta) {
-  if (p->idx16_launch)
-    return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, true>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
-  return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, false>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
+  if (p->cols_launch == COLS_PAT)
+    return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, COLS_PAT>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
+  if (p->cols_launch == COLS_DELTA)
+    return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, COLS_DELTA>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
+  return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, COLS_I32>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
 }
 
 template <typename S, int LPR>
@@ -1349,13 +1584,13 @@ static int spmv_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   const int cfg = p->cfg >= 0 ? p->cfg : 8;  // CAP=2048, 4 stages, 16 consumer warps, 2 CTAs/SM
   int rc = plan_analyse<S>(p, st, cfg, m, n, nnz, row_ptr);
   if (rc) return rc;
-  // B200SP_SPMV_IDX16=0: the 32-bit columns (A/B comparisons; the 16-bit stream is not built for this call)
+  // B200SP_SPMV_IDX16=0: the 32-bit columns (A/B comparisons; the 16-bit streams are not built for this call)
   const char* i16 = getenv("B200SP_SPMV_IDX16");
-  p->idx16_launch = false;
+  p->cols_launch = COLS_I32;
   if (!(i16 && i16[0] == '0')) {
     rc = plan_idx16(p, st, m, nnz, row_ptr, col_idx);
     if (rc) return rc;
-    p->idx16_launch = p->idx16_state == 1;
+    if (p->idx16_state > 0) p->cols_launch = p->idx16_state;
   }
   const int lpr = p->lpr > 0 ? p->lpr : lpr_auto;
   // ---- self-tuning (only for untuned plans on whole-matrix launches)

@@ -254,4 +254,7 @@ static inline int __ffs(int v) { return __builtin_ffs(v); }
 static inline int atomicMax(int* p, int v) { int o = *p; if (v > o) *p = v; b200emu::note_progress(); return o; }
 static inline unsigned atomicOr(unsigned* p, unsigned v) { unsigned o = *p; *p = o | v; b200emu::note_progress(); return o; }
 static inline int atomicCAS(int* p, int cmp, int v) { int o = *p; if (o == cmp) *p = v; b200emu::note_progress(); return o; }
+static inline unsigned long long atomicCAS(unsigned long long* p, unsigned long long cmp, unsigned long long v) {
+  unsigned long long o = *p; if (o == cmp) *p = v; b200emu::note_progress(); return o;
+}
 static inline int atomicExch(int* p, int v) { int o = *p; *p = v; b200emu::note_progress(); return o; }
