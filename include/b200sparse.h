@@ -207,6 +207,24 @@ int b200sp_spmm_f32_i32(b200sp_spmv_plan* plan, void* stream, char mode, int m, 
                         int k, float alpha, const int* row_ptr, const int* col_idx,
                         const float* vals, const float* X, int64_t ldx, int x_row_major,
                         float beta, float* Y, int64_t ldy, int y_row_major);
+/* Half precision (Kokkos::Experimental::half_t, the reference's cusparseSpMM slot with an fp32 compute type,
+ * sparse/tpls/KokkosSparse_spmv_mv_tpl_spec_decl.hpp:47-61): vals, X and Y hold IEEE binary16 bit patterns.
+ *  - Every product a*x is formed in fp32, where it is exact (two 11-bit significands; even 2^-24 * 2^-24 is an fp32
+ *    normal).  Products are accumulated in fp32; rows cut into several pieces keep their partial sums in fp32.
+ *  - The epilogue beta*y + alpha*acc is evaluated in fp32 and rounded ONCE to binary16, to nearest even; a result
+ *    beyond +-65504 becomes +-inf.  Intermediate sums may exceed the fp16 range without harm.
+ *  - alpha and beta are used as given (the Kokkos shim converts half_t to float exactly).
+ *  - Modes N == C, T == H.  beta == 0 never reads Y (NaN in Y is overwritten); alpha == 0 or an empty A gives
+ *    Y = beta*Y.  Any mix of layouts is accepted.
+ * Mode N with a plan and row-major X and Y runs the item kernels (16-byte loads of 8 halves when k, ldx and ldy are
+ * multiples of 8 and X and Y are 16-byte aligned); LayoutLeft operands with a plan and k >= 4 go through row-major
+ * copies; without a plan, or LayoutLeft with k < 4, one thread per (row, column) computes the entry.  On those item paths
+ * the result has the same bits as b200sp_spmm_f32_i32 on the widened inputs, rounded to binary16.  T / H add the exact
+ * products into a zeroed fp32 scratch (the plan's, or a stream-ordered temporary without a plan) with atomics and round
+ * each entry once.  B200SP_SPMM_KERNEL (row / split / tile) does not apply to this entry point. */
+int b200sp_spmm_f16_i32(b200sp_spmv_plan* plan, void* stream, char mode, int m, int n, int64_t nnz, int k, float alpha,
+                        const int* row_ptr, const int* col_idx, const uint16_t* vals, const uint16_t* X, int64_t ldx,
+                        int x_row_major, float beta, uint16_t* Y, int64_t ldy, int y_row_major);
 
 /* ---- SpGEMM: C = A*B, A is m x n, B is n x k ---------------------------- */
 int b200sp_spgemm_plan_create(b200sp_spgemm_plan** plan);

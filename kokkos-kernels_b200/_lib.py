@@ -58,6 +58,7 @@ SPARSE_API = {
     "b200sp_spmv_hostvec_f64_i32": (i32, [vp, vp, cp, i32, i32, i64, f64, vp, vp, vp, vp, f64, vp]),
     "b200sp_spmm_f64_i32": (i32, [vp, vp, cp, i32, i32, i64, i32, f64, vp, vp, vp, vp, i64, i32, f64, vp, i64, i32]),
     "b200sp_spmm_f32_i32": (i32, [vp, vp, cp, i32, i32, i64, i32, f32, vp, vp, vp, vp, i64, i32, f32, vp, i64, i32]),
+    "b200sp_spmm_f16_i32": (i32, [vp, vp, cp, i32, i32, i64, i32, f32, vp, vp, vp, vp, i64, i32, f32, vp, i64, i32]),
     "b200sp_spgemm_plan_create": (i32, [C.POINTER(vp)]),
     "b200sp_spgemm_plan_destroy": (i32, [vp, vp]),
     "b200sp_spgemm_symbolic_i32": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), C.POINTER(i32)]),

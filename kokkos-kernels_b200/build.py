@@ -86,6 +86,17 @@ def _build_locked(force, verbose):
         if verbose:
             print("[build]", " ".join(cmd), flush=True)
         subprocess.check_call(cmd)
+    # the same for the half_t SPMV_MV specialisations (half_t stand-in: Kokkos_Mock_Half.hpp, under KOKKOS_HALF_T_IS_FLOAT == 0)
+    hdrv = os.path.join(LIB, "shim_half_driver")
+    hsrc = os.path.join(root, "tests", "shim_mock", "shim_half_driver.cpp")
+    hdeps = [os.path.join(root, "tests", "shim_mock", f) for f in ("Kokkos_Mock.hpp", "Kokkos_Mock_Half.hpp")]
+    if os.path.exists(hsrc) and (force or not _newer(hdrv, [hsrc, out] + hdeps + shim)):
+        cmd = [_nvcc(), "-std=c++17", "-O1", "-Wno-deprecated-gpu-targets", "-I", os.path.join(root, "tests", "shim_mock"),
+               "-I", os.path.join(HERE, "kokkos_shim"), "-I", os.path.join(root, "include"), hsrc, "-o", hdrv,
+               "-L", LIB, "-lb200sparse", "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN"]
+        if verbose:
+            print("[build]", " ".join(cmd), flush=True)
+        subprocess.check_call(cmd)
     # torch-free GPU validation harness (tools/gpu_check.cpp; links the oracle as the CHECKER -- test infrastructure)
     chk = os.path.join(LIB, "gpu_check")
     csrc = os.path.join(root, "tools", "gpu_check.cpp")

@@ -4,6 +4,7 @@
 #include "cuda_emu.h"  // tools/emu: CUDA-on-CPU emulation of the kernels (test infrastructure)
 #else
 #include <cuda_runtime.h>
+#include <cuda_fp16.h>
 #endif
 #include <stdint.h>
 #include <stdio.h>
@@ -134,6 +135,9 @@ __device__ __forceinline__ void st_once(float* p, float v, uint64_t) { *p = v; }
 __device__ __forceinline__ void st_once(double* p, double v, uint64_t) { *p = v; }
 __device__ __forceinline__ void st_once(float4* p, const float4& v, uint64_t) { *p = v; }
 __device__ __forceinline__ void st_once(double2* p, const double2& v, uint64_t) { *p = v; }
+__device__ __forceinline__ __half ld_once(const __half* p, uint64_t) { return *p; }
+__device__ __forceinline__ void st_once(__half* p, __half v, uint64_t) { *p = v; }
+__device__ __forceinline__ void st_once(uint4* p, const uint4& v, uint64_t) { *p = v; }
 #else
 // ---- PTX wrappers: mbarrier + 1-D bulk (TMA) copies ------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -259,6 +263,19 @@ __device__ __forceinline__ void st_once(float4* p, const float4& v, uint64_t pol
 }
 __device__ __forceinline__ void st_once(double2* p, const double2& v, uint64_t pol) {
   asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1, %2}, %3;" ::"l"(p), "d"(v.x), "d"(v.y), "l"(pol) : "memory");
+}
+// binary16: one value, or 8 packed in a uint4 (the 16-byte form of the half-precision rank-2 kernels)
+__device__ __forceinline__ __half ld_once(const __half* p, uint64_t pol) {
+  unsigned short v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.b16 %0, [%1], %2;" : "=h"(v) : "l"(p), "l"(pol));
+  return __ushort_as_half(v);
+}
+__device__ __forceinline__ void st_once(__half* p, __half v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.b16 [%0], %1, %2;" ::"l"(p), "h"(__half_as_ushort(v)), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_once(uint4* p, const uint4& v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.v4.b32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol)
+               : "memory");
 }
 
 #endif  // B200SP_EMU

@@ -15,11 +15,14 @@
 //   spmm_transpose_kernel T/H modes: Y pre-scaled, atomicAdd scatter.
 // Column-major (LayoutLeft) X with k >= 4 goes through a transposed copy so the
 // gather touches one segment per nonzero instead of k sectors (DESIGN.md 3.4).
+// binary16 (b200sp_spmm_f16_i32, spmm_impl_f16): the item, general and relayout kernels with fp32 accumulators, and an fp32
+// scratch for T/H (DESIGN.md 4.3).
 #include <limits.h>
 #include "common.cuh"
 #include "tile_ring.cuh"
 #include "spmm_items.h"
 #include <algorithm>
+#include <type_traits>
 #include <atomic>
 #include <stdlib.h>
 
@@ -32,8 +35,21 @@ int plan_mv_scratch(b200sp_spmv_plan* p, cudaStream_t st, size_t xt_bytes, size_
 void plan_set_last_kernel(b200sp_spmv_plan* p, const char* s);
 MMItems* plan_mm_items(b200sp_spmv_plan* p);
 
+// Storage type S -> accumulator type: fp32 and fp64 accumulate in their own type, binary16 (__half) in fp32.  wide() is exact;
+// narrow() rounds once, to nearest even (a result beyond the fp16 range becomes +-inf).  Kernels that serve fp16 compute in
+// AccT<S> and touch S only to load and store.
+template <typename S> struct AccOf { using type = S; };
+template <> struct AccOf<__half> { using type = float; };
+template <typename S> using AccT = typename AccOf<S>::type;
+__device__ __forceinline__ float wide(float v) { return v; }
+__device__ __forceinline__ double wide(double v) { return v; }
+__device__ __forceinline__ float wide(__half v) { return __half2float(v); }
+template <typename S> __device__ __forceinline__ S narrow(AccT<S> v) { return v; }
+template <> __device__ __forceinline__ __half narrow<__half>(float v) { return __float2half_rn(v); }
+
 template <typename S>
-__global__ void scale2d_kernel(int64_t rows, int k, S beta, S* __restrict__ Y, int64_t yr, int64_t yc) {
+__global__ void scale2d_kernel(int64_t rows, int k, AccT<S> beta, S* __restrict__ Y, int64_t yr, int64_t yc) {
+  using A = AccT<S>;
   const int64_t total = rows * k;
   const bool by_rows = (yc == 1 || yr != 1);  // walk memory-contiguously for either layout
   if (total <= (int64_t)INT32_MAX) {  // 32-bit index arithmetic: a 64-bit division per element costs more than the element's traffic
@@ -42,7 +58,7 @@ __global__ void scale2d_kernel(int64_t rows, int k, S beta, S* __restrict__ Y, i
       unsigned r, j;
       if (by_rows) { r = i / k32; j = i - r * k32; } else { j = i / r32; r = i - j * r32; }
       S* p = &Y[(int64_t)r * yr + (int64_t)j * yc];
-      *p = (beta == S(0)) ? S(0) : beta * *p;
+      *p = narrow<S>((beta == A(0)) ? A(0) : beta * wide(*p));
     }
     return;
   }
@@ -50,7 +66,7 @@ __global__ void scale2d_kernel(int64_t rows, int k, S beta, S* __restrict__ Y, i
     int64_t r, j;
     if (by_rows) { r = i / k; j = i % k; } else { j = i / rows; r = i % rows; }
     S* p = &Y[r * yr + j * yc];
-    *p = (beta == S(0)) ? S(0) : beta * *p;
+    *p = narrow<S>((beta == A(0)) ? A(0) : beta * wide(*p));
   }
 }
 
@@ -151,15 +167,16 @@ template <typename S>
 __global__ void __launch_bounds__(256)
     spmm_general_kernel(int m, int k, const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
                         const S* __restrict__ vals, const S* __restrict__ X, int64_t xr, int64_t xc,
-                        S* __restrict__ Y, int64_t yr, int64_t yc, S alpha, S beta) {
+                        S* __restrict__ Y, int64_t yr, int64_t yc, AccT<S> alpha, AccT<S> beta) {
+  using A = AccT<S>;
   const int64_t total = (int64_t)m * k;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int r = (int)(i / k), j = (int)(i % k);
-    S acc = S(0);
-    for (int e = row_ptr[r]; e < row_ptr[r + 1]; ++e) acc += vals[e] * ldg(X + (int64_t)col_idx[e] * xr + (int64_t)j * xc);
+    A acc = A(0);
+    for (int e = row_ptr[r]; e < row_ptr[r + 1]; ++e) acc += wide(vals[e]) * wide(ldg(X + (int64_t)col_idx[e] * xr + (int64_t)j * xc));
     acc *= alpha;
     S* yp = Y + (int64_t)r * yr + (int64_t)j * yc;
-    *yp = (beta == S(0)) ? acc : beta * *yp + acc;
+    *yp = narrow<S>((beta == A(0)) ? acc : beta * wide(*yp) + acc);
   }
 }
 
@@ -174,6 +191,20 @@ __global__ void __launch_bounds__(256)
     const S xv = X[(int64_t)r * xr + (int64_t)j * xc];
     for (int e = row_ptr[r]; e < row_ptr[r + 1]; ++e)
       atomicAdd(Y + (int64_t)col_idx[e] * yr + (int64_t)j * yc, alpha * vals[e] * xv);
+  }
+}
+
+// T/H for fp16: exact fp32 products a*x added into a zeroed fp32 row-major [yrows x k] scratch, then ONE rounding per entry of Y
+// in spmm_acc_epilogue_kernel (a half atomicAdd into Y would round at every addition)
+__global__ void __launch_bounds__(256)
+    spmm_transpose_acc_kernel(int m, int k, const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
+                              const __half* __restrict__ vals, const __half* __restrict__ X, int64_t xr, int64_t xc,
+                              float* __restrict__ acc) {
+  const int64_t total = (int64_t)m * k;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int r = (int)(i / k), j = (int)(i % k);
+    const float xv = wide(X[(int64_t)r * xr + (int64_t)j * xc]);
+    for (int e = row_ptr[r]; e < row_ptr[r + 1]; ++e) atomicAdd(acc + (int64_t)col_idx[e] * k + j, wide(vals[e]) * xv);
   }
 }
 
@@ -299,6 +330,22 @@ __device__ __forceinline__ void vec_unpack(const float4& v, float* a) { a[0] = v
 __device__ __forceinline__ void vec_unpack(const double2& v, double* a) { a[0] = v.x; a[1] = v.y; }
 __device__ __forceinline__ float4 vec_pack(const float* a) { return make_float4(a[0], a[1], a[2], a[3]); }
 __device__ __forceinline__ double2 vec_pack(const double* a) { return make_double2(a[0], a[1]); }
+// binary16: 8 halves per 16-byte load, unpacked straight to fp32 (item kernels only)
+template <> struct VecOf<__half> { using type = uint4; static constexpr int W = 8; };
+__device__ __forceinline__ void vec_unpack(const uint4& v, float* a) {
+  const unsigned w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    a[2 * i] = __half2float(__ushort_as_half((unsigned short)(w[i] & 0xffffu)));
+    a[2 * i + 1] = __half2float(__ushort_as_half((unsigned short)(w[i] >> 16)));
+  }
+}
+__device__ __forceinline__ uint4 vec_pack(const __half* a) {
+  unsigned w[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) w[i] = (unsigned)__half_as_ushort(a[2 * i]) | ((unsigned)__half_as_ushort(a[2 * i + 1]) << 16);
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
 
 // ---------------------------------------------------------------------------
 // Tile kernel (B200SP_SPMM_KERNEL=tile|tilev; row-major X and Y): the matrix is streamed ONCE, whatever k,
@@ -320,18 +367,63 @@ struct Acc {
 __device__ __forceinline__ float axpby_rn(float alpha, float acc, float beta, float y) { return fmaf(beta, y, __fmul_rn(alpha, acc)); }
 __device__ __forceinline__ double axpby_rn(double alpha, double acc, double beta, double y) { return fma(beta, y, __dmul_rn(alpha, acc)); }
 
+// the fp16 transpose's epilogue: Y = beta*Y + alpha*acc in fp32, rounded once to fp16; beta == 0 never reads Y
+__global__ void __launch_bounds__(256)
+    spmm_acc_epilogue_kernel(int64_t rows, int k, const float* __restrict__ acc, float alpha, float beta, __half* __restrict__ Y,
+                             int64_t yr, int64_t yc) {
+  const int64_t total = rows * k;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / k, j = i % k;
+    __half* yp = Y + r * yr + j * yc;
+    *yp = narrow<__half>(beta == 0.0f ? __fmul_rn(alpha, acc[i]) : axpby_rn(alpha, acc[i], beta, wide(*yp)));
+  }
+}
+
+// X rows (and Y for beta != 0) in the accumulator type: VW == 1 one element, else one 16-byte load of VW elements
 template <typename S, int VW>
-__device__ __forceinline__ Acc<S, VW> load_x(const S* __restrict__ p) {
+__device__ __forceinline__ Acc<AccT<S>, VW> load_x(const S* __restrict__ p) {
   static_assert(VW == 1 || VW == VecOf<S>::W, "VW is 1 or the 16-byte vector width");
-  Acc<S, VW> r;
+  Acc<AccT<S>, VW> r;
   if constexpr (VW == 1) {
-    r.a[0] = ldg(p);
+    r.a[0] = wide(ldg(p));
   } else {
     using V = typename VecOf<S>::type;
     const V v = __ldg(reinterpret_cast<const V*>(p));
     vec_unpack(v, r.a);
   }
   return r;
+}
+
+// VW accumulator values rounded to T and stored evict-first: VW == 1 one element, else 16-byte stores (two for 8 fp32 partial
+// sums of the fp16 kernels)
+template <int VW, typename T>
+__device__ __forceinline__ void st_vec_once(T* dst, const AccT<T>* o, uint64_t once) {
+  if constexpr (VW == 1) {
+    st_once(dst, narrow<T>(o[0]), once);
+  } else {
+    constexpr int PER = VecOf<T>::W;
+    static_assert(VW % PER == 0, "whole 16-byte stores");
+#pragma unroll
+    for (int h = 0; h < VW; h += PER) {
+      T t[PER];
+#pragma unroll
+      for (int i = 0; i < PER; ++i) t[i] = narrow<T>(o[h + i]);
+      st_once(reinterpret_cast<typename VecOf<T>::type*>(dst + h), vec_pack(t), once);
+    }
+  }
+}
+
+// an item that is a whole row: o = alpha*acc (beta == 0: Y is not read) or beta*y + alpha*acc, in the accumulator type
+template <typename S, int VW>
+__device__ __forceinline__ void item_epilogue(AccT<S>* o, const Acc<AccT<S>, VW>& acc, AccT<S> alpha, AccT<S> beta, const S* y) {
+  if (beta == AccT<S>(0)) {
+#pragma unroll
+    for (int cc = 0; cc < VW; ++cc) o[cc] = alpha * acc.a[cc];
+  } else {
+    const Acc<AccT<S>, VW> old = load_x<S, VW>(y);
+#pragma unroll
+    for (int cc = 0; cc < VW; ++cc) o[cc] = axpby_rn(alpha, acc.a[cc], beta, old.a[cc]);
+  }
 }
 
 template <typename S, int VW, int KTL, int NW, int STAGES, int CAP, int UNR>
@@ -1034,7 +1126,8 @@ template <typename S, int VW, int KTL>
 __global__ void __launch_bounds__(256)
     spmm_item_kernel(int n_items, const int4* __restrict__ items, int k, const int* __restrict__ col_idx,
                      const S* __restrict__ vals, const S* __restrict__ X, int64_t ldx, S* __restrict__ Y, int64_t ldy,
-                     S* __restrict__ partial, S alpha, S beta) {
+                     AccT<S>* __restrict__ partial, AccT<S> alpha, AccT<S> beta) {
+  using A = AccT<S>;
   const int64_t gt = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t q = gt / KTL;
   const int t = (int)(gt % KTL);
@@ -1047,20 +1140,20 @@ __global__ void __launch_bounds__(256)
   for (int strip = 0; strip < nstrips; ++strip) {
     const int j = (strip * KTL + t) * VW;
     if (j >= k) break;  // k % VW == 0: a lane's VW columns are all in or all out
-    Acc<S, VW> acc;
+    Acc<A, VW> acc;
 #pragma unroll
-    for (int c = 0; c < VW; ++c) acc.a[c] = S(0);
+    for (int c = 0; c < VW; ++c) acc.a[c] = A(0);
     const S* xb = X + j;
     int e = e0;
     const int e4 = e0 + (len & ~3);
     for (; e < e4; e += 4) {
       int c[4];
-      S av[4];
-      Acc<S, VW> xv[4];
+      A av[4];
+      Acc<A, VW> xv[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         c[u] = ld_once(col_idx + e + u, once);
-        av[u] = ld_once(vals + e + u, once);
+        av[u] = wide(ld_once(vals + e + u, once));
       }
 #pragma unroll
       for (int u = 0; u < 4; ++u) xv[u] = load_x<S, VW>(xb + (int64_t)c[u] * ldx);
@@ -1071,33 +1164,29 @@ __global__ void __launch_bounds__(256)
     }
     for (; e < e0 + len; ++e) {
       const int c = ld_once(col_idx + e, once);
-      const S av = ld_once(vals + e, once);
-      const Acc<S, VW> xv = load_x<S, VW>(xb + (int64_t)c * ldx);
+      const A av = wide(ld_once(vals + e, once));
+      const Acc<A, VW> xv = load_x<S, VW>(xb + (int64_t)c * ldx);
 #pragma unroll
       for (int cc = 0; cc < VW; ++cc) acc.a[cc] += av * xv.a[cc];
     }
-    S o[VW];
-    S* dst;
-    if (slot < 0) {
-      dst = Y + (int64_t)row * ldy + j;
-      if (beta == S(0)) {
-#pragma unroll
-        for (int cc = 0; cc < VW; ++cc) o[cc] = alpha * acc.a[cc];
+    A o[VW];
+    if constexpr (std::is_same<S, A>::value) {  // fp32 / fp64: Y and the partial sums share a type, one store
+      S* dst;
+      if (slot < 0) {
+        dst = Y + (int64_t)row * ldy + j;
+        item_epilogue<S, VW>(o, acc, alpha, beta, dst);
       } else {
-        const Acc<S, VW> old = load_x<S, VW>(dst);
+        dst = partial + (int64_t)slot * k + j;  // raw sums; alpha and beta are applied by the reduce kernel
 #pragma unroll
-        for (int cc = 0; cc < VW; ++cc) o[cc] = axpby_rn(alpha, acc.a[cc], beta, old.a[cc]);
+        for (int cc = 0; cc < VW; ++cc) o[cc] = acc.a[cc];
       }
+      st_vec_once<VW>(dst, o, once);
+    } else if (slot < 0) {  // fp16: Y in S, the partial sums in A
+      S* dst = Y + (int64_t)row * ldy + j;
+      item_epilogue<S, VW>(o, acc, alpha, beta, dst);
+      st_vec_once<VW>(dst, o, once);
     } else {
-      dst = partial + (int64_t)slot * k + j;  // raw sums; alpha and beta are applied by the reduce kernel
-#pragma unroll
-      for (int cc = 0; cc < VW; ++cc) o[cc] = acc.a[cc];
-    }
-    if constexpr (VW == 1) {
-      st_once(dst, o[0], once);
-    } else {
-      using V = typename VecOf<S>::type;
-      st_once(reinterpret_cast<V*>(dst), vec_pack(o), once);
+      st_vec_once<VW>(partial + (int64_t)slot * k + j, acc.a, once);
     }
   }
 }
@@ -1114,7 +1203,8 @@ template <typename S, int VW, int KTL, int EB /* entries per batch: 4 or 8 */>
 __global__ void __launch_bounds__(256)
     spmm_item_coop_kernel(int n_items, const int4* __restrict__ items, int k, const int* __restrict__ col_idx,
                           const S* __restrict__ vals, const S* __restrict__ X, int64_t ldx, S* __restrict__ Y, int64_t ldy,
-                          S* __restrict__ partial, S alpha, S beta) {
+                          AccT<S>* __restrict__ partial, AccT<S> alpha, AccT<S> beta) {
+  using A = AccT<S>;
   constexpr int PL = (EB + KTL - 1) / KTL;    // entries a lane loads per batch (KTL > EB: lanes >= EB load nothing)
   const int64_t gt = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t q = gt / KTL;
@@ -1129,9 +1219,9 @@ __global__ void __launch_bounds__(256)
   for (int strip = 0; strip < nstrips; ++strip) {
     const int j = (strip * KTL + t) * VW;
     const bool live = j < k;  // k % VW == 0: a lane's VW columns are all in or all out; dead lanes still load and shuffle
-    Acc<S, VW> acc;
+    Acc<A, VW> acc;
 #pragma unroll
-    for (int c = 0; c < VW; ++c) acc.a[c] = S(0);
+    for (int c = 0; c < VW; ++c) acc.a[c] = A(0);
     const S* xb = X + (live ? j : 0);
     int e = e0;
     for (; e + EB <= eend; e += EB) {
@@ -1141,26 +1231,26 @@ __global__ void __launch_bounds__(256)
       for (int i = 0; i < PL; ++i) {
         const int idx = i * KTL + t;
         cl[i] = 0;
-        vl[i] = S(0);
+        vl[i] = S();
         if (KTL <= EB || idx < EB) {
           cl[i] = ld_once(col_idx + e + idx, once);
           vl[i] = ld_once(vals + e + idx, once);
         }
       }
       int c[EB];
-      S av[EB];
+      A av[EB];
 #pragma unroll
       for (int u = 0; u < EB; ++u) {
         if constexpr (KTL == 1) {
           c[u] = cl[u];
-          av[u] = vl[u];
+          av[u] = wide(vl[u]);
         } else {
           c[u] = __shfl_sync(gmask, cl[u / KTL], u % KTL, KTL);
-          av[u] = __shfl_sync(gmask, vl[u / KTL], u % KTL, KTL);
+          av[u] = wide(__shfl_sync(gmask, vl[u / KTL], u % KTL, KTL));
         }
       }
       if (live) {
-        Acc<S, VW> xv[EB];
+        Acc<A, VW> xv[EB];
 #pragma unroll
         for (int u = 0; u < EB; ++u) xv[u] = load_x<S, VW>(xb + (int64_t)c[u] * ldx);
 #pragma unroll
@@ -1177,26 +1267,26 @@ __global__ void __launch_bounds__(256)
       for (int i = 0; i < PL; ++i) {
         const int idx = i * KTL + t;
         cl[i] = 0;
-        vl[i] = S(0);
+        vl[i] = S();
         if (idx < rem) {
           cl[i] = ld_once(col_idx + e + idx, once);
           vl[i] = ld_once(vals + e + idx, once);
         }
       }
       int c[EB];
-      S av[EB];
+      A av[EB];
 #pragma unroll
       for (int u = 0; u < EB; ++u) {
         if constexpr (KTL == 1) {
           c[u] = cl[u];
-          av[u] = vl[u];
+          av[u] = wide(vl[u]);
         } else {
           c[u] = __shfl_sync(gmask, cl[u / KTL], u % KTL, KTL);
-          av[u] = __shfl_sync(gmask, vl[u / KTL], u % KTL, KTL);
+          av[u] = wide(__shfl_sync(gmask, vl[u / KTL], u % KTL, KTL));
         }
       }
       if (live) {
-        Acc<S, VW> xv[EB];
+        Acc<A, VW> xv[EB];
 #pragma unroll
         for (int u = 0; u < EB - 1; ++u)
           if (u < rem) xv[u] = load_x<S, VW>(xb + (int64_t)c[u] * ldx);
@@ -1209,28 +1299,24 @@ __global__ void __launch_bounds__(256)
       }
     }
     if (!live) continue;
-    S o[VW];
-    S* dst;
-    if (slot < 0) {
-      dst = Y + (int64_t)row * ldy + j;
-      if (beta == S(0)) {
-#pragma unroll
-        for (int cc = 0; cc < VW; ++cc) o[cc] = alpha * acc.a[cc];
+    A o[VW];
+    if constexpr (std::is_same<S, A>::value) {  // fp32 / fp64: Y and the partial sums share a type, one store
+      S* dst;
+      if (slot < 0) {
+        dst = Y + (int64_t)row * ldy + j;
+        item_epilogue<S, VW>(o, acc, alpha, beta, dst);
       } else {
-        const Acc<S, VW> old = load_x<S, VW>(dst);
+        dst = partial + (int64_t)slot * k + j;  // raw sums; alpha and beta are applied by the reduce kernel
 #pragma unroll
-        for (int cc = 0; cc < VW; ++cc) o[cc] = axpby_rn(alpha, acc.a[cc], beta, old.a[cc]);
+        for (int cc = 0; cc < VW; ++cc) o[cc] = acc.a[cc];
       }
+      st_vec_once<VW>(dst, o, once);
+    } else if (slot < 0) {  // fp16: Y in S, the partial sums in A
+      S* dst = Y + (int64_t)row * ldy + j;
+      item_epilogue<S, VW>(o, acc, alpha, beta, dst);
+      st_vec_once<VW>(dst, o, once);
     } else {
-      dst = partial + (int64_t)slot * k + j;  // raw sums; alpha and beta are applied by the reduce kernel
-#pragma unroll
-      for (int cc = 0; cc < VW; ++cc) o[cc] = acc.a[cc];
-    }
-    if constexpr (VW == 1) {
-      st_once(dst, o[0], once);
-    } else {
-      using V = typename VecOf<S>::type;
-      st_once(reinterpret_cast<V*>(dst), vec_pack(o), once);
+      st_vec_once<VW>(partial + (int64_t)slot * k + j, acc.a, once);
     }
   }
 }
@@ -1242,8 +1328,9 @@ __global__ void __launch_bounds__(256)
 // took a fifth of the whole product.)
 template <typename S>
 __global__ void __launch_bounds__(256)
-    spmm_item_reduce_kernel(int n_multi, const int4* __restrict__ multi, int k, const S* __restrict__ partial, S* __restrict__ Y,
-                            int64_t ldy, S alpha, S beta) {
+    spmm_item_reduce_kernel(int n_multi, const int4* __restrict__ multi, int k, const AccT<S>* __restrict__ partial,
+                            S* __restrict__ Y, int64_t ldy, AccT<S> alpha, AccT<S> beta) {
+  using A = AccT<S>;
   const int lane = threadIdx.x & 31;
   int KC = 1;
   while (KC < k && KC < 32) KC <<= 1;
@@ -1254,15 +1341,15 @@ __global__ void __launch_bounds__(256)
     const int4 d = multi[w];  // (row, first partial slot, pieces, 0)
     for (int jb = 0; jb < k; jb += KC) {
       const int j = jb + j0;
-      S sum = S(0);
+      A sum = A(0);
       if (j < k) {
-        const S* src = partial + (int64_t)d.y * k + j;
+        const A* src = partial + (int64_t)d.y * k + j;
         for (int s = sub; s < d.z; s += SUB) sum += src[(int64_t)s * k];
       }
       for (int o = 16; o >= KC; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
       if (sub == 0 && j < k) {
         S* yp = Y + (int64_t)d.x * ldy + j;
-        *yp = (beta == S(0)) ? alpha * sum : beta * *yp + alpha * sum;
+        *yp = narrow<S>((beta == A(0)) ? alpha * sum : beta * wide(*yp) + alpha * sum);
       }
     }
   }
@@ -1273,9 +1360,10 @@ __global__ void __launch_bounds__(256)
 // joined in subsequence order through shared memory by the threads of subsequence 0.  Fixed order: reproducible.
 template <typename S>
 __global__ void __launch_bounds__(256)
-    spmm_item_reduce_long_kernel(int n_long, const int4* __restrict__ multi_long, int k, const S* __restrict__ partial,
-                                 S* __restrict__ Y, int64_t ldy, S alpha, S beta) {
-  __shared__ S part[256];
+    spmm_item_reduce_long_kernel(int n_long, const int4* __restrict__ multi_long, int k, const AccT<S>* __restrict__ partial,
+                                 S* __restrict__ Y, int64_t ldy, AccT<S> alpha, AccT<S> beta) {
+  using A = AccT<S>;
+  __shared__ A part[256];
   int KC = 1;
   while (KC < k && KC < 32) KC <<= 1;
   const int SUB = 256 / KC;
@@ -1284,18 +1372,18 @@ __global__ void __launch_bounds__(256)
     const int4 d = multi_long[w];
     for (int jb = 0; jb < k; jb += KC) {
       const int j = jb + j0;
-      S sum = S(0);
+      A sum = A(0);
       if (j < k) {
-        const S* src = partial + (int64_t)d.y * k + j;
+        const A* src = partial + (int64_t)d.y * k + j;
         for (int s = sub; s < d.z; s += SUB) sum += src[(int64_t)s * k];
       }
       part[threadIdx.x] = sum;
       __syncthreads();
       if (sub == 0 && j < k) {
-        S t = part[j0];
+        A t = part[j0];
         for (int q = 1; q < SUB; ++q) t += part[q * KC + j0];
         S* yp = Y + (int64_t)d.x * ldy + j;
-        *yp = (beta == S(0)) ? alpha * t : beta * *yp + alpha * t;
+        *yp = narrow<S>((beta == A(0)) ? alpha * t : beta * wide(*yp) + alpha * t);
       }
       __syncthreads();
     }
@@ -1304,7 +1392,8 @@ __global__ void __launch_bounds__(256)
 
 template <typename S>
 static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m, int k, int64_t nnz, const int* row_ptr,
-                           const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
+                           const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, AccT<S> alpha, AccT<S> beta) {
+  using A = AccT<S>;
   int LMAX = 64;  // entries per item (B200SP_SPMM_ITEM_LMAX: 16..256); 64 was the best of 32..256 on R-MAT scale 23 when tuned
   if (const char* e = getenv("B200SP_SPMM_ITEM_LMAX")) {
     const int v = atoi(e);
@@ -1313,7 +1402,7 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   MMItems* mi;
   int rc = plan_analyse_items(p, st, LMAX, m, nnz, row_ptr, &mi);
   if (rc) return rc;
-  const size_t need = sizeof(S) * (size_t)mi->n_partial * (size_t)k;
+  const size_t need = sizeof(A) * (size_t)mi->n_partial * (size_t)k;
   if (need > mi->partial_bytes) {
     if (mi->partial) cudaFreeAsync(mi->partial, st);
     mi->partial = nullptr;
@@ -1336,13 +1425,13 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   case L:                                                                                                                  \
     if (coop == 8)                                                                                                         \
       spmm_item_coop_kernel<S, V, L, 8><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,    \
-                                                              (S*)mi->partial, alpha, beta);                               \
+                                                              (A*)mi->partial, alpha, beta);                               \
     else if (coop == 4)                                                                                                    \
       spmm_item_coop_kernel<S, V, L, 4><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,    \
-                                                              (S*)mi->partial, alpha, beta);                               \
+                                                              (A*)mi->partial, alpha, beta);                               \
     else                                                                                                                   \
       spmm_item_kernel<S, V, L><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,            \
-                                                      (S*)mi->partial, alpha, beta);                                       \
+                                                      (A*)mi->partial, alpha, beta);                                       \
     break;
     if (vec) {
       switch (KTL) { B200SP_MMI(W, 1) B200SP_MMI(W, 2) B200SP_MMI(W, 4) B200SP_MMI(W, 8) B200SP_MMI(W, 16) B200SP_MMI(W, 32) }
@@ -1355,12 +1444,12 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   const int n_short = mi->n_multi - mi->n_multi_long;
   if (n_short > 0) {
     const int g = (int)std::min<int64_t>(((int64_t)n_short + 7) / 8, (int64_t)sm_count() * 16);  // a warp per row
-    spmm_item_reduce_kernel<S><<<std::max(g, 1), 256, 0, st>>>(n_short, mi->multi, k, (const S*)mi->partial, Y, ldy, alpha, beta);
+    spmm_item_reduce_kernel<S><<<std::max(g, 1), 256, 0, st>>>(n_short, mi->multi, k, (const A*)mi->partial, Y, ldy, alpha, beta);
     B200SP_LAUNCH_CHECK();
   }
   if (mi->n_multi_long > 0) {
     const int g = std::min(mi->n_multi_long, sm_count() * 8);  // a CTA per row
-    spmm_item_reduce_long_kernel<S><<<g, 256, 0, st>>>(mi->n_multi_long, mi->multi + n_short, k, (const S*)mi->partial, Y, ldy, alpha, beta);
+    spmm_item_reduce_long_kernel<S><<<g, 256, 0, st>>>(mi->n_multi_long, mi->multi + n_short, k, (const A*)mi->partial, Y, ldy, alpha, beta);
     B200SP_LAUNCH_CHECK();
   }
   return B200SP_OK;
@@ -1508,6 +1597,101 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   return B200SP_OK;
 }
 
+// binary16 A, X and Y with fp32 products, sums and epilogue (include/b200sparse.h, DESIGN.md 4.3).  The item path and its
+// relayout serve mode N with a plan; B200SP_SPMM_KERNEL does not apply.  Without a plan, or for LayoutLeft with k < 4:
+// spmm_general_kernel.  T/H: fp32 scratch + one epilogue.
+static int spmm_impl_f16(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int n, int64_t nnz, int k, float alpha,
+                         const int* row_ptr, const int* col_idx, const __half* vals, const __half* X, int64_t ldx, int xrm,
+                         float beta, __half* Y, int64_t ldy, int yrm) {
+  using S = __half;
+  B200SP_REQUIRE(m >= 0 && n >= 0 && nnz >= 0 && k >= 0, "spmm: negative dimension");
+  bool trans;
+  switch (mode) {
+    case 'N': case 'n': case 'C': case 'c': trans = false; break;
+    case 'T': case 't': case 'H': case 'h': trans = true; break;
+    default: set_error("Invalid transpose mode %c for KokkosSparse::spmv()", mode); return B200SP_ERR_INVALID_ARGUMENT;
+  }
+  const int64_t xrows = trans ? m : n, yrows = trans ? n : m;
+  const int64_t xr = xrm ? ldx : 1, xc = xrm ? 1 : ldx;
+  const int64_t yr = yrm ? ldy : 1, yc = yrm ? 1 : ldy;
+  if (k == 0 || yrows == 0) return B200SP_OK;
+  B200SP_REQUIRE(Y != nullptr, "spmm: Y is null");
+  B200SP_REQUIRE((xrm ? ldx >= k : ldx >= xrows) && (yrm ? ldy >= k : ldy >= yrows), "spmm: leading dimension too small");
+  const int grid_elem = (int)std::min<int64_t>((yrows * k + 255) / 256, (int64_t)sm_count() * 16);
+  if (alpha == 0.0f || m == 0 || n == 0 || nnz == 0) {
+    if (beta != 1.0f) {
+      scale2d_kernel<S><<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, beta, Y, yr, yc);
+      B200SP_LAUNCH_CHECK();
+    }
+    return B200SP_OK;
+  }
+  B200SP_REQUIRE(row_ptr && col_idx && vals && X, "spmm: null pointer argument");
+  if (trans) {
+    DevTmp tmp(st);
+    float* acc = nullptr;
+    const size_t acc_bytes = sizeof(float) * (size_t)yrows * (size_t)k;
+    if (p) {
+      void *unused = nullptr, *yt = nullptr;
+      if (int rc = plan_mv_scratch(p, st, 0, acc_bytes, &unused, &yt)) return rc;
+      acc = (float*)yt;
+    } else {
+      B200SP_CUDA_TRY(tmp.alloc(&acc, (size_t)yrows * (size_t)k));
+    }
+    B200SP_CUDA_TRY(cudaMemsetAsync(acc, 0, acc_bytes, st));
+    const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
+    spmm_transpose_acc_kernel<<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, acc);
+    B200SP_LAUNCH_CHECK();
+    spmm_acc_epilogue_kernel<<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, acc, alpha, beta, Y, yr, yc);
+    B200SP_LAUNCH_CHECK();
+    plan_set_last_kernel(p, "spmm_transpose");
+    return B200SP_OK;
+  }
+  constexpr int W = VecOf<S>::W;
+  if (p && xrm && yrm) {
+    const bool vec = (k % W == 0) && (ldx % W == 0) && (ldy % W == 0) && ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0;
+    plan_set_last_kernel(p, vec ? "spmm_items_vec" : "spmm_items");
+    return launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
+  }
+  if (p && k >= 4) {  // LayoutLeft operands: row-major copies in the plan's scratch, as for fp32
+    void *xt = nullptr, *yt = nullptr;
+    const size_t xtb = xrm ? 0 : sizeof(S) * (size_t)xrows * k;
+    const size_t ytb = yrm ? 0 : sizeof(S) * (size_t)yrows * k;
+    if (int rc = plan_mv_scratch(p, st, xtb, ytb, &xt, &yt)) return rc;
+    auto rl_grid = [](int64_t rows) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>((rows + 127) / 128, (int64_t)sm_count() * 16)); };
+    const S* Xr = X;
+    int64_t ldxr = ldx;
+    if (!xrm) {
+      relayout_kernel<S, true><<<rl_grid(xrows), 256, 0, st>>>(xrows, k, (S*)xt, X, nullptr, xr, xc);
+      B200SP_LAUNCH_CHECK();
+      Xr = (const S*)xt;
+      ldxr = k;
+    }
+    S* Yr = Y;
+    int64_t ldyr = ldy;
+    if (!yrm) {
+      Yr = (S*)yt;
+      ldyr = k;
+      if (beta != 0.0f) {
+        relayout_kernel<S, true><<<rl_grid(yrows), 256, 0, st>>>(yrows, k, Yr, Y, nullptr, yr, yc);
+        B200SP_LAUNCH_CHECK();
+      }
+    }
+    const bool vec = (k % W == 0) && (ldxr % W == 0) && (ldyr % W == 0) && ((((uintptr_t)Xr) | ((uintptr_t)Yr)) & 15u) == 0;
+    if (int rc = launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta)) return rc;
+    if (!yrm) {
+      relayout_kernel<S, false><<<rl_grid(yrows), 256, 0, st>>>(yrows, k, Yr, nullptr, Y, yr, yc);
+      B200SP_LAUNCH_CHECK();
+    }
+    plan_set_last_kernel(p, "spmm_relayout+items");
+    return B200SP_OK;
+  }
+  const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
+  spmm_general_kernel<S><<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, Y, yr, yc, alpha, beta);
+  B200SP_LAUNCH_CHECK();
+  plan_set_last_kernel(p, "spmm_general");
+  return B200SP_OK;
+}
+
 }  // namespace b200sp
 
 using namespace b200sp;
@@ -1524,5 +1708,12 @@ int b200sp_spmm_f32_i32(b200sp_spmv_plan* plan, void* stream, char mode, int m, 
                         int64_t ldx, int x_row_major, float beta, float* Y, int64_t ldy, int y_row_major) {
   return spmm_impl<float>(plan, (cudaStream_t)stream, mode, m, n, nnz, k, alpha, row_ptr, col_idx, vals, X, ldx,
                           x_row_major, beta, Y, ldy, y_row_major);
+}
+int b200sp_spmm_f16_i32(b200sp_spmv_plan* plan, void* stream, char mode, int m, int n, int64_t nnz, int k, float alpha,
+                        const int* row_ptr, const int* col_idx, const uint16_t* vals, const uint16_t* X, int64_t ldx,
+                        int x_row_major, float beta, uint16_t* Y, int64_t ldy, int y_row_major) {
+  static_assert(sizeof(__half) == sizeof(uint16_t), "binary16 bit patterns");
+  return spmm_impl_f16(plan, (cudaStream_t)stream, mode, m, n, nnz, k, alpha, row_ptr, col_idx, reinterpret_cast<const __half*>(vals),
+                       reinterpret_cast<const __half*>(X), ldx, x_row_major, beta, reinterpret_cast<__half*>(Y), ldy, y_row_major);
 }
 }

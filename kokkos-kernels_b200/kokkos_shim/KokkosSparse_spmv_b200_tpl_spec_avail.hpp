@@ -49,6 +49,19 @@ KOKKOSSPARSE_B200_SPMV_AVAIL_ALL(float, Kokkos::CudaUVMSpace)
 
 #undef KOKKOSSPARSE_B200_SPMV_AVAIL_ALL
 
+// half_t, rank 2 only, where half_t is a real 16-bit type (the guard of the reference's cuSPARSE slot,
+// sparse/tpls/KokkosSparse_spmv_mv_tpl_spec_avail.hpp:93-104); fp32 products and sums, every layout pair
+#if defined(KOKKOS_HALF_T_IS_FLOAT) && !KOKKOS_HALF_T_IS_FLOAT
+#define KOKKOSSPARSE_B200_SPMV_MV_HALF_AVAIL_ALL(MEMSPACE)                                                                          \
+  KOKKOSSPARSE_B200_SPMV_MV_AVAIL(Kokkos::Experimental::half_t, Kokkos::LayoutLeft, Kokkos::LayoutLeft, MEMSPACE)                   \
+  KOKKOSSPARSE_B200_SPMV_MV_AVAIL(Kokkos::Experimental::half_t, Kokkos::LayoutRight, Kokkos::LayoutLeft, MEMSPACE)                  \
+  KOKKOSSPARSE_B200_SPMV_MV_AVAIL(Kokkos::Experimental::half_t, Kokkos::LayoutLeft, Kokkos::LayoutRight, MEMSPACE)                  \
+  KOKKOSSPARSE_B200_SPMV_MV_AVAIL(Kokkos::Experimental::half_t, Kokkos::LayoutRight, Kokkos::LayoutRight, MEMSPACE)
+KOKKOSSPARSE_B200_SPMV_MV_HALF_AVAIL_ALL(Kokkos::CudaSpace)
+KOKKOSSPARSE_B200_SPMV_MV_HALF_AVAIL_ALL(Kokkos::CudaUVMSpace)
+#undef KOKKOSSPARSE_B200_SPMV_MV_HALF_AVAIL_ALL
+#endif
+
 // 64-bit offsets: (int64_t, size_t) -- the instantiation of the cuSPARSE slot (..._tpl_spec_avail.hpp:85-102) -- and
 // (int, size_t), which cuSPARSE does not take (:86); rank 1 and rank 2
 #define KOKKOSSPARSE_B200_SPMV64_AVAIL(SCALAR, ORDINAL, OFFSET, LAYOUT, MEMSPACE)                                   \

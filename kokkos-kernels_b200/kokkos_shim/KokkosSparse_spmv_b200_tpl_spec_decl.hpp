@@ -120,6 +120,27 @@ KOKKOSSPARSE_B200_SPMV_DECL_ALL(float, Kokkos::CudaUVMSpace)
 
 #undef KOKKOSSPARSE_B200_SPMV_DECL_ALL
 
+// ---- half_t, rank 2 (guard as in the avail header): binary16 data, alpha and beta converted to float exactly ----------
+#if defined(KOKKOS_HALF_T_IS_FLOAT) && !KOKKOS_HALF_T_IS_FLOAT
+static_assert(sizeof(Kokkos::Experimental::half_t) == sizeof(uint16_t), "half_t is passed as binary16 bit patterns");
+inline int b200_call_spmm(b200sp_spmv_plan* p, void* s, char mode, int m, int n, int64_t nnz, int k,
+                          Kokkos::Experimental::half_t alpha, const int* rp, const int* ci, const Kokkos::Experimental::half_t* v,
+                          const Kokkos::Experimental::half_t* X, int64_t ldx, int xrm, Kokkos::Experimental::half_t beta,
+                          Kokkos::Experimental::half_t* Y, int64_t ldy, int yrm) {
+  return b200sp_spmm_f16_i32(p, s, mode, m, n, nnz, k, static_cast<float>(alpha), rp, ci, reinterpret_cast<const uint16_t*>(v),
+                             reinterpret_cast<const uint16_t*>(X), ldx, xrm, static_cast<float>(beta),
+                             reinterpret_cast<uint16_t*>(Y), ldy, yrm);
+}
+#define KOKKOSSPARSE_B200_SPMV_MV_HALF_DECL_ALL(MEMSPACE)                                                                          \
+  KOKKOSSPARSE_B200_SPMV_MV_DECL(Kokkos::Experimental::half_t, Kokkos::LayoutLeft, Kokkos::LayoutLeft, MEMSPACE)                   \
+  KOKKOSSPARSE_B200_SPMV_MV_DECL(Kokkos::Experimental::half_t, Kokkos::LayoutRight, Kokkos::LayoutLeft, MEMSPACE)                  \
+  KOKKOSSPARSE_B200_SPMV_MV_DECL(Kokkos::Experimental::half_t, Kokkos::LayoutLeft, Kokkos::LayoutRight, MEMSPACE)                  \
+  KOKKOSSPARSE_B200_SPMV_MV_DECL(Kokkos::Experimental::half_t, Kokkos::LayoutRight, Kokkos::LayoutRight, MEMSPACE)
+KOKKOSSPARSE_B200_SPMV_MV_HALF_DECL_ALL(Kokkos::CudaSpace)
+KOKKOSSPARSE_B200_SPMV_MV_HALF_DECL_ALL(Kokkos::CudaUVMSpace)
+#undef KOKKOSSPARSE_B200_SPMV_MV_HALF_DECL_ALL
+#endif
+
 // ---- 64-bit offsets -----------------------------------------------------------------------------------------------
 inline b200sp_spmv64_plan* b200_plan64_of(TPL_SpMV_Data<Kokkos::Cuda>*& slot, const Kokkos::Cuda& exec, int algo) {
   B200_SpMV64_Data* sub;

@@ -225,6 +225,8 @@ def spmv(handle, mode, alpha, A, x, beta, y):
             f"KokkosSparse::spmv: Dimensions do not match: , A: {m} x {n}, x: {x.shape[0]} x {xcols}, "
             f"y: {y.shape[0]} x {ycols}"
         )
+    if torch.float16 in (A.values.dtype, x.dtype, y.dtype):
+        return _spmm_f16(handle, m0, alpha, A, x, beta, y, m, n, xcols)
     if A.values.dtype != x.dtype or x.dtype != y.dtype:
         raise B200SparseError("b200sparse: A.values, x and y must share one scalar type (f64 or f32)")
     lib = _lib.sparse()
@@ -272,6 +274,36 @@ def spmv(handle, mode, alpha, A, x, beta, y):
     fn = lib.b200sp_spmm_f64_i32 if f64 else lib.b200sp_spmm_f32_i32
     check(fn(plan, _stream(), mc, m, n, A.nnz(), xcols, alpha, _idx(A.row_map), _idx(A.entries), _ptr(A.values),
              _ptr(x), ldx, xrm, beta, _ptr(y), ldy, yrm))
+    return y
+
+
+def _half_coefficient(c):
+    """A coefficient as the half_t it is in Kokkos (coefficient_type of a half_t multivector): rounded to binary16, to
+    nearest even; beyond +-65504 it is +-inf."""
+    import numpy as np
+
+    with np.errstate(over="ignore"):
+        return float(np.float16(c))
+
+
+def _spmm_f16(handle, m0, alpha, A, x, beta, y, m, n, xcols):
+    """Rank-2 SpMV on float16 A, X and Y with fp32 products, sums and epilogue (b200sp_spmm_f16_i32; the reference's half_t
+    SPMV_MV slot, sparse/tpls/KokkosSparse_spmv_mv_tpl_spec_avail.hpp:93-104)."""
+    if not (A.values.dtype == x.dtype == y.dtype == torch.float16):
+        raise B200SparseError(f"b200sparse: half precision needs A.values, x and y all float16, got {A.values.dtype}, {x.dtype}, "
+                              f"{y.dtype} (mixed precision is not provided)")
+    if isinstance(A, BsrMatrix):
+        raise B200SparseError("b200sparse: half precision is provided for CrsMatrix only, not BsrMatrix")
+    if x.dim() != 2:
+        raise B200SparseError("b200sparse: half precision is provided for rank-2 x and y only, not rank 1")
+    if A.row_map.dtype != torch.int32 or A.entries.dtype != torch.int32:
+        raise B200SparseError("b200sparse: half precision takes int32 row maps and entries, not 64-bit offsets")
+    ldx, xrm = _mv_layout(x)
+    ldy, yrm = _mv_layout(y)
+    plan = handle._plan if handle is not None else C.c_void_p(0)
+    check(_lib.sparse().b200sp_spmm_f16_i32(plan, _stream(), m0.encode(), m, n, A.nnz(), xcols, _half_coefficient(alpha),
+                                            _idx(A.row_map), _idx(A.entries), _ptr(A.values), _ptr(x), ldx, xrm,
+                                            _half_coefficient(beta), _ptr(y), ldy, yrm))
     return y
 
 

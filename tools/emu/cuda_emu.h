@@ -39,6 +39,17 @@ struct int2 { int x, y; };
 struct alignas(16) int4 { int x, y, z, w; };
 struct alignas(16) float4 { float x, y, z, w; };
 struct alignas(16) double2 { double x, y; };
+struct alignas(16) uint4 { unsigned x, y, z, w; };
+static inline uint4 make_uint4(unsigned x, unsigned y, unsigned z, unsigned w) { return uint4{x, y, z, w}; }
+// IEEE binary16 on g++'s _Float16: float -> half rounds to nearest even, subnormals included, as __float2half_rn does.  Only
+// the conversions exist (no arithmetic operators), so emulated kernels cannot compute in half by accident.
+struct __half {
+  _Float16 v;
+};
+static inline __half __float2half_rn(float f) { return __half{(_Float16)f}; }
+static inline float __half2float(__half h) { return (float)h.v; }
+static inline unsigned short __half_as_ushort(__half h) { unsigned short b; memcpy(&b, &h, 2); return b; }
+static inline __half __ushort_as_half(unsigned short b) { __half h; memcpy(&h, &b, 2); return h; }
 static inline int2 make_int2(int x, int y) { return int2{x, y}; }
 static inline int4 make_int4(int x, int y, int z, int w) { return int4{x, y, z, w}; }
 static inline float4 make_float4(float x, float y, float z, float w) { return float4{x, y, z, w}; }
