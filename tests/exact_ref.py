@@ -1,9 +1,11 @@
-"""Exact reference and per-entry rounding-error bound of rank-2 SpMV, Y = beta*Y0 + alpha*op(A)*X.
+"""Exact reference and per-entry rounding-error bound of SpMV, y = beta*y0 + alpha*op(A)*x, rank 1 and rank 2, on
+CrsMatrix and (through bsr_to_point_crs) BsrMatrix.
 
 The oracle (oracle_lib.Oracle.spmv_mv) computes in the kernel's own precision, so its rounding error is about as large as
 the error it is meant to detect.  spmm_exact computes the same product in a wider format (float64 for fp32 data,
 np.longdouble for fp64 data), and spmm_bound gives, for every entry of Y, how far a correctly implemented kernel may be
-from it.  assert_within checks a kernel's output entry by entry against that bound."""
+from it.  assert_within checks a kernel's output entry by entry against that bound.  All three take 1-D x and y (rank 1)
+as well as 2-D X and Y."""
 import numpy as np
 
 assert np.finfo(np.longdouble).nmant >= 63, "the fp64 reference needs an x87-extended or quad np.longdouble"
@@ -155,6 +157,36 @@ def spmm_scale(rp, ci, v, X, Y0, alpha, beta, trans=False):
         with np.errstate(invalid="ignore"):  # 0 * Inf where X holds an Inf: that entry's exact value is not finite either
             scale += a * _segment_sums(starts, xrow, w, np.abs(X.astype(np.float64)), np.float64)
     return scale
+
+
+def bsr_to_point_crs(bs, rp, ci, v):
+    """A BsrMatrix (block row map rp, block columns ci, values of nnzb blocks of bs x bs, each row-major as the library
+    stores them) as point CSR (rp, ci, v).  Point row br*bs + i holds, block by block in storage order, the bs entries of
+    row i of each block of block row br at columns ci[k]*bs + j.  Its length is bs * (block degree), the len_i the bound
+    of a block kernel's row needs: every point entry of a block is one term, explicit zeros included."""
+    bs = int(bs)
+    rp = np.asarray(rp, dtype=np.int64)
+    ci = np.asarray(ci, dtype=np.int64)
+    v = np.asarray(v)
+    mb = len(rp) - 1
+    nnzb = int(rp[-1])
+    assert len(ci) == nnzb and v.size == nnzb * bs * bs
+    deg = np.diff(rp)
+    prp = np.zeros(mb * bs + 1, dtype=np.int64)
+    np.cumsum(np.repeat(deg * bs, bs), out=prp[1:])
+    assert prp[-1] < 2**31
+    # entry (i, j) of block k (the q-th of its block row br) goes to bs*bs*rp[br] + bs*(i*deg[br] + q) + j: block row, then
+    # point row inside the block, then block of the row, then column inside the block
+    br = np.repeat(np.arange(mb, dtype=np.int64), deg)
+    q = np.arange(nnzb, dtype=np.int64) - rp[br]
+    i = np.arange(bs, dtype=np.int64)[None, :, None]
+    j = np.arange(bs, dtype=np.int64)[None, None, :]
+    pos = bs * bs * rp[br][:, None, None] + bs * (i * deg[br][:, None, None] + q[:, None, None]) + j
+    pci = np.empty(nnzb * bs * bs, dtype=np.int32)
+    pv = np.empty(nnzb * bs * bs, dtype=v.dtype)
+    pci[pos.reshape(-1)] = np.broadcast_to(ci[:, None, None] * bs + j, pos.shape).reshape(-1)
+    pv[pos.reshape(-1)] = v.reshape(-1)
+    return prp.astype(np.int32), pci, pv
 
 
 def assert_within(got, exact, bound, what):

@@ -7,6 +7,8 @@ import numpy as np
 import pytest
 
 import emu_lib as E
+import exact_ref as R
+import spmm_cases
 from bsr_cases import BLOCK_SIZES, COEFS_ALPHA, COEFS_BETA, PRIME_CASE, SHAPES, bsr_random, op_max_nnz_per_row, tolerance
 
 
@@ -24,15 +26,26 @@ def expected(oracle, mode, bs, nb, rp, ci, v, X, Y0, alpha, beta):
     return oracle.bsr_spmv_v41(mode, bs, nb, rp, ci, v, X, Yc, alpha, beta)
 
 
-def run_rank1(oracle, plan, mode, bs, mb, nb, rp, ci, v, rng, alpha, beta, dtype):
+def run_rank1(oracle, plan, mode, bs, mb, nb, rp, ci, v, rng, alpha, beta, dtype, signed=False):
+    """signed: mixed-sign values (spmm_cases._values), x and y0, checked against the exact product only (the reference's
+    law assumes entries in [0, 10)); every call is checked against it."""
     trans = mode in "TH"
     nx, ny = (mb * bs, nb * bs) if trans else (nb * bs, mb * bs)
     x = rng.uniform(0, 10, nx).astype(dtype)
     y0 = rng.uniform(0, 10, ny).astype(dtype)
+    if signed:
+        v = spmm_cases._values(rng, len(v), dtype)
+        x = spmm_cases.dense_operands(rng, nx, 1, dtype)[:, 0]
+        y0 = spmm_cases.dense_operands(rng, ny, 1, dtype)[:, 0]
     if beta == 0.0:
         y0[::7] = np.nan
     y = y0.copy()
     E.bsr_spmv(plan, mode, mb, nb, bs, rp, ci, v, x, y, alpha, beta)
+    prp, pci, pv = R.bsr_to_point_crs(bs, rp, ci, v)
+    R.assert_within(y, R.spmm_exact(prp, pci, pv, x, y0, alpha, beta, trans), R.spmm_bound(prp, pci, pv, x, y0, alpha, beta, trans),
+                    f"{plan.kernel()} mode {mode} bs {bs} alpha {alpha} beta {beta} signed {signed}")
+    if signed:
+        return
     exp = expected(oracle, mode, bs, nb, rp, ci, v, x, y0, alpha, beta)
     assert not np.isnan(y).any(), "NaN survived beta == 0"
     tol = tolerance(dtype, alpha, beta, op_max_nnz_per_row(bs, rp, ci, nb, trans))
@@ -48,12 +61,13 @@ CASES = [(bs, mb, nb) for (mb, nb) in SHAPES for bs in BLOCK_SIZES] + [PRIME_CAS
 def test_reference_sweep_rank1(emu, oracle, bs, mb, nb, dtype):
     rp, ci, v = bsr_random(bs, mb, nb, seed=3 + bs + mb, dtype=dtype, sort=False)
     rng = np.random.default_rng(17)
-    plan = E.BsrPlan()
-    for mode in "NTCH":
-        for alpha in COEFS_ALPHA:
-            for beta in COEFS_BETA:
-                run_rank1(oracle, plan, mode, bs, mb, nb, rp, ci, v, rng, alpha, beta, dtype)
-    plan.close()
+    for signed in (False, True):
+        plan = E.BsrPlan()
+        for mode in "NTCH":
+            for alpha in COEFS_ALPHA:
+                for beta in COEFS_BETA:
+                    run_rank1(oracle, plan, mode, bs, mb, nb, rp, ci, v, rng, alpha, beta, dtype, signed)
+        plan.close()
 
 
 @pytest.mark.parametrize("bs,mb,nb", CASES)
@@ -100,6 +114,7 @@ def test_tile_kernel_every_block_size(emu, oracle, bs):
                 for dtype in (np.float64, np.float32):
                     vv = v.astype(dtype)
                     run_rank1(oracle, plan, "N", bs, mb, nb, rp, ci, vv, rng, alpha, beta, dtype)
+                    run_rank1(oracle, plan, "N", bs, mb, nb, rp, ci, vv, rng, alpha, beta, dtype, signed=True)
                     # default: element-per-lane tile kernel for bs 2..5, row-vector kernel above (the measured choice)
                     if bs > 5 and not knob:  # default: tensor-core kernel for double up to bs = 16, row-vector kernel otherwise
                         want = "bsr_mm_tc<f64" if (dtype == np.float64 and bs <= 16) else "bsr_vector"
@@ -127,8 +142,9 @@ def test_long_block_rows_and_tail(emu, oracle, dtype):
     v = rng.uniform(0, 10, len(ci) * bs * bs).astype(dtype)
     plan = E.BsrPlan()
     for alpha, beta in ((1.0, 0.0), (-1.0, 1.0), (3.7, -1.5)):
-        run_rank1(oracle, plan, "N", bs, mb, nb, rp, ci, v, rng, alpha, beta, dtype)
-        assert plan.kernel().startswith("bsr_tile"), plan.kernel()
+        for signed in (False, True):
+            run_rank1(oracle, plan, "N", bs, mb, nb, rp, ci, v, rng, alpha, beta, dtype, signed)
+            assert plan.kernel().startswith("bsr_tile"), plan.kernel()
     plan.close()
 
 

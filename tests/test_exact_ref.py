@@ -163,6 +163,64 @@ def test_bound_catches_swapped_columns(oracle, dtype):
         R.assert_within(got, R.spmm_exact(rp, ci, v, X, Y0, 1.0, 0.0), R.spmm_bound(rp, ci, v, X, Y0, 1.0, 0.0), "swapped")
 
 
+def _bsr_dense(bs, mb, nb, rp, ci, v):
+    D = np.zeros((mb * bs, nb * bs), dtype=np.float64)
+    blocks = v.reshape(-1, bs, bs)
+    for br in range(mb):
+        for k in range(rp[br], rp[br + 1]):
+            D[br * bs:(br + 1) * bs, ci[k] * bs:(ci[k] + 1) * bs] += blocks[k]
+    return D
+
+
+@pytest.mark.parametrize("bs", [1, 2, 3, 7])
+def test_bsr_to_point_crs_matches_a_dense_product(bs):
+    """The expansion against a dense matrix assembled block by block (row-major blocks), rank 1 and 2, N and T; point rows
+    hold bs * (block degree) entries; an empty block row gives empty point rows."""
+    from bsr_cases import bsr_random
+
+    rng = np.random.default_rng(bs)
+    mb, nb = 9, 11
+    rp, ci, v = bsr_random(bs, mb, nb, seed=bs, min_blocks=0, max_blocks=5, sort=False)
+    v = spmm_cases._values(rng, len(v), np.float64)
+    prp, pci, pv = R.bsr_to_point_crs(bs, rp, ci, v)
+    assert np.array_equal(np.diff(prp), np.repeat(np.diff(rp) * bs, bs))
+    D = _bsr_dense(bs, mb, nb, rp, ci, v)
+    P = np.zeros_like(D)
+    np.add.at(P, (np.repeat(np.arange(mb * bs), np.diff(prp)), pci), pv)
+    assert np.array_equal(P, D)
+    for trans in (False, True):
+        rows_out, rows_in = (nb * bs, mb * bs) if trans else (mb * bs, nb * bs)
+        for X in (spmm_cases.dense_operands(rng, rows_in, 3, np.float64), spmm_cases.dense_operands(rng, rows_in, 1, np.float64)[:, 0]):
+            Y0 = np.ones((rows_out,) + X.shape[1:])
+            got = R.spmm_exact(prp, pci, pv, X, Y0, 1.5, -0.5, trans)
+            ref = 1.5 * ((D.T if trans else D) @ X) - 0.5 * Y0
+            R.assert_within(ref, got.reshape(ref.shape), R.spmm_bound(prp, pci, pv, X, Y0, 1.5, -0.5, trans), f"bs={bs} trans={trans}")
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_bound_rejects_a_transposed_block(dtype):
+    """A kernel that reads a block column-major instead of row-major: caught in the point rows of that block."""
+    from bsr_cases import bsr_random
+
+    bs, mb, nb = 4, 12, 10
+    rng = np.random.default_rng(5)
+    rp, ci, v = bsr_random(bs, mb, nb, seed=5, min_blocks=1, max_blocks=4, sort=False)
+    v = spmm_cases._values(rng, len(v), dtype)
+    x = spmm_cases.dense_operands(rng, nb * bs, 1, dtype)[:, 0]
+    y0 = spmm_cases.dense_operands(rng, mb * bs, 1, dtype)[:, 0]
+    prp, pci, pv = R.bsr_to_point_crs(bs, rp, ci, v)
+    exact = R.spmm_exact(prp, pci, pv, x, y0, 1.0, 1.0)
+    bound = R.spmm_bound(prp, pci, pv, x, y0, 1.0, 1.0)
+    good = (_bsr_dense(bs, mb, nb, rp, ci, v.astype(np.float64)) @ x.astype(np.float64) + y0).astype(dtype)
+    R.assert_within(good, exact, bound, "row-major blocks")
+    vt = v.reshape(-1, bs, bs).copy()
+    k = int(rp[3])  # the first block of block row 3
+    vt[k] = vt[k].T
+    bad = (_bsr_dense(bs, mb, nb, rp, ci, vt.reshape(-1).astype(np.float64)) @ x.astype(np.float64) + y0).astype(dtype)
+    with pytest.raises(AssertionError, match=r"first at row 1[2-5], column 0"):
+        R.assert_within(bad, exact, bound, "one block transposed")
+
+
 def test_assert_within_special_values():
     exact = np.array([[1.0, np.inf, np.nan]], dtype=np.longdouble)
     bound = np.zeros((1, 3))

@@ -6,11 +6,14 @@ import numpy as np
 import pytest
 import torch
 
+import exact_ref as R
+import spmm_cases
 from bsr_cases import BLOCK_SIZES, COEFS_ALPHA, COEFS_BETA, PRIME_CASE, SHAPES, bsr_random, op_max_nnz_per_row, tolerance
 
 pytestmark = pytest.mark.gpu
 
 CASES = [(bs, mb, nb) for (mb, nb) in SHAPES for bs in BLOCK_SIZES] + [PRIME_CASE]
+EXACT_MAX = 1 << 22  # point entries up to which the all-positive runs are also checked against the exact product
 
 
 def to_dev(sp, dev, bs, nb, rp, ci, v):
@@ -24,23 +27,45 @@ def expected(oracle, mode, bs, nb, rp, ci, v, X, Y0, alpha, beta):
     return oracle.bsr_spmv_v41(mode, bs, nb, rp, ci, v, X, Yc, alpha, beta)
 
 
-def run_rank1(sp, oracle, dev, handle, A, host, mode, rng, alpha, beta, dtype):
+def mixed(sp, dev, bs, nb, rp, ci, v, seed):
+    """The same structure with mixed-sign values over several binades: (device matrix, host tuple's values)"""
+    vm = spmm_cases._values(np.random.default_rng(seed), len(v), v.dtype)
+    return to_dev(sp, dev, bs, nb, rp, ci, vm), vm
+
+
+def check_exact(got, bs, rp, ci, v, x, y0, alpha, beta, trans, what):
+    """entry by entry within the rounding bound of the exact product of the point CSR form (tests/exact_ref.py)"""
+    prp, pci, pv = R.bsr_to_point_crs(bs, rp, ci, v)
+    R.assert_within(got, R.spmm_exact(prp, pci, pv, x, y0, alpha, beta, trans), R.spmm_bound(prp, pci, pv, x, y0, alpha, beta, trans), what)
+
+
+def run_rank1(sp, oracle, dev, handle, A, host, mode, rng, alpha, beta, dtype, signed=False):
+    """signed: the values are mixed-sign (mixed()), x and y0 too, and only the exact bound applies (the reference's law
+    assumes entries in [0, 10))"""
     bs, mb, nb, rp, ci, v = host
     trans = mode in "TH"
     nx, ny = (mb * bs, nb * bs) if trans else (nb * bs, mb * bs)
     x = rng.uniform(0, 10, nx).astype(dtype)
     y0 = rng.uniform(0, 10, ny).astype(dtype)
+    if signed:
+        x = spmm_cases.dense_operands(rng, nx, 1, dtype)[:, 0]
+        y0 = spmm_cases.dense_operands(rng, ny, 1, dtype)[:, 0]
     if beta == 0.0:
         y0[::7] = np.nan
     yd = torch.from_numpy(y0).to(dev)
     sp.spmv(handle, mode, alpha, A, torch.from_numpy(x).to(dev), beta, yd)
     torch.cuda.synchronize()
     got = yd.cpu().numpy()
+    what = f"{handle.last_kernel()} mode {mode} bs {bs} alpha {alpha} beta {beta}"
+    if signed or len(v) <= EXACT_MAX:
+        check_exact(got, bs, rp, ci, v, x, y0, alpha, beta, trans, what)
+    if signed:
+        return
     exp = expected(oracle, mode, bs, nb, rp, ci, v, x, y0, alpha, beta)
     assert not np.isnan(got).any(), "NaN survived beta == 0"
     tol = tolerance(dtype, alpha, beta, op_max_nnz_per_row(bs, rp, ci, nb, trans))
     err = np.max(np.abs(got - exp), initial=0.0)
-    assert err <= tol, f"{handle.last_kernel()} mode {mode} bs {bs} alpha {alpha} beta {beta}: err {err:.3e} > {tol:.3e}"
+    assert err <= tol, f"{what}: err {err:.3e} > {tol:.3e}"
 
 
 @pytest.mark.parametrize("bs,mb,nb", CASES)
@@ -51,12 +76,14 @@ def test_reference_sweep_rank1(cuda, oracle, bs, mb, nb, dtype):
     rp, ci, v = bsr_random(bs, mb, nb, seed=3 + bs + mb, dtype=dtype, sort=False)
     A = to_dev(sp, cuda, bs, nb, rp, ci, v)
     rng = np.random.default_rng(17)
+    Am, vm = mixed(sp, cuda, bs, nb, rp, ci, v, seed=bs + mb)
     for algo in (sp.SPMV_DEFAULT, sp.SPMV_NATIVE, sp.SPMV_BSR_V41):  # test_spmv_combos (:364)
-        h = sp.SPMVHandle(algo)
-        for mode in "NTCH":
-            for alpha in COEFS_ALPHA:
-                for beta in COEFS_BETA:
-                    run_rank1(sp, oracle, cuda, h, A, (bs, mb, nb, rp, ci, v), mode, rng, alpha, beta, dtype)
+        for signed, AA, vv in ((False, A, v), (True, Am, vm)):
+            h = sp.SPMVHandle(algo)
+            for mode in "NTCH":
+                for alpha in COEFS_ALPHA:
+                    for beta in COEFS_BETA:
+                        run_rank1(sp, oracle, cuda, h, AA, (bs, mb, nb, rp, ci, vv), mode, rng, alpha, beta, dtype, signed)
 
 
 @pytest.mark.parametrize("bs,mb,nb", CASES)
@@ -74,25 +101,32 @@ def test_reference_sweep_multivector(cuda, oracle, bs, mb, nb, layout):
         t = torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
         return t if layout == "right" else t.t().contiguous().t()
 
-    for mode in "NTCH":
-        trans = mode in "TH"
-        nx, ny = (mb * bs, nb * bs) if trans else (nb * bs, mb * bs)
-        max_row = op_max_nnz_per_row(bs, rp, ci, nb, trans)
-        for k in (1, 7):
-            X = rng.uniform(0, 10, (nx, k))
-            Y0 = rng.uniform(0, 10, (ny, k))
-            for alpha in COEFS_ALPHA:
-                for beta in COEFS_BETA:
-                    Yin = Y0.copy()
-                    if beta == 0.0 and ny:
-                        Yin[::5] = np.nan
-                    Yd = dev2d(Yin)
-                    sp.spmv(h, mode, alpha, A, dev2d(X), beta, Yd)
-                    torch.cuda.synchronize()
-                    got = Yd.cpu().numpy()
-                    exp = expected(oracle, mode, bs, nb, rp, ci, v, X, Yin, alpha, beta)
-                    assert not np.isnan(got).any()
-                    assert np.max(np.abs(got - exp), initial=0.0) <= tolerance(dtype, alpha, beta, max_row), (h.last_kernel(), mode, k, alpha, beta)
+    Am, vm = mixed(sp, cuda, bs, nb, rp, ci, v, seed=bs + nb)
+    for signed in (False, True):
+        for mode in "NTCH":
+            trans = mode in "TH"
+            nx, ny = (mb * bs, nb * bs) if trans else (nb * bs, mb * bs)
+            max_row = op_max_nnz_per_row(bs, rp, ci, nb, trans)
+            for k in (1, 7):
+                X = rng.uniform(0, 10, (nx, k))
+                Y0 = rng.uniform(0, 10, (ny, k))
+                if signed:
+                    X, Y0 = spmm_cases.dense_operands(rng, nx, k, dtype), spmm_cases.dense_operands(rng, ny, k, dtype)
+                for alpha in COEFS_ALPHA:
+                    for beta in COEFS_BETA:
+                        Yin = Y0.copy()
+                        if beta == 0.0 and ny:
+                            Yin[::5] = np.nan
+                        Yd = dev2d(Yin)
+                        sp.spmv(h, mode, alpha, Am if signed else A, dev2d(X), beta, Yd)
+                        torch.cuda.synchronize()
+                        got = Yd.cpu().numpy()
+                        check_exact(got, bs, rp, ci, vm if signed else v, X, Yin, alpha, beta, trans, f"{h.last_kernel()} mode {mode} k {k}")
+                        if signed:
+                            continue
+                        exp = expected(oracle, mode, bs, nb, rp, ci, v, X, Yin, alpha, beta)
+                        assert not np.isnan(got).any()
+                        assert np.max(np.abs(got - exp), initial=0.0) <= tolerance(dtype, alpha, beta, max_row), (h.last_kernel(), mode, k, alpha, beta)
 
 
 @pytest.mark.parametrize("bs", [1, 2, 3, 4, 5, 7, 8, 11, 16, 17])
@@ -108,6 +142,7 @@ def test_tensor_core_multivector(cuda, oracle, bs, layout):
     A = to_dev(sp, cuda, bs, nb, rp, ci, v)
     rng = np.random.default_rng(29)
     h = sp.SPMVHandle(sp.SPMV_BSR_TC)
+    Am, vm = mixed(sp, cuda, bs, nb, rp, ci, v, seed=40 + bs)
 
     def dev2d(a):
         t = torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
@@ -131,6 +166,16 @@ def test_tensor_core_multivector(cuda, oracle, bs, layout):
                 exp = expected(oracle, mode, bs, nb, rp, ci, v, X, Yin, alpha, beta)
                 assert not np.isnan(got).any()
                 assert np.max(np.abs(got - exp), initial=0.0) <= tolerance(dtype, alpha, beta, max_row), (h.last_kernel(), mode, k, alpha, beta)
+                check_exact(got, bs, rp, ci, v, X, Yin, alpha, beta, trans, f"{h.last_kernel()} mode {mode} k {k}")
+                # once more with mixed signs: the same kernel, checked against the exact product only
+                k0 = h.last_kernel()
+                Xm, Ym = spmm_cases.dense_operands(rng, nx, k, dtype), spmm_cases.dense_operands(rng, ny, k, dtype)
+                Ymd = dev2d(Ym)
+                sp.spmv(h, mode, alpha, Am, dev2d(Xm), beta, Ymd)
+                torch.cuda.synchronize()
+                km = h.last_kernel()
+                assert km.split("<")[0] == k0.split("<")[0], (km, k0)
+                check_exact(Ymd.cpu().numpy(), bs, rp, ci, vm, Xm, Ym, alpha, beta, trans, f"{km} mixed signs mode {mode} k {k}")
                 if mode == "N" and 2 <= bs <= 16:
                     assert h.last_kernel().startswith("bsr_mm_tc<f64"), h.last_kernel()
                 else:
@@ -174,6 +219,18 @@ def test_tile_kernel_every_block_size(cuda, oracle, bs, force, monkeypatch):
             want = "bsr_tile_e" if bs <= 5 else ("bsr_mm_tc<f64" if bs <= 16 else "bsr_vector")  # double: tensor cores for bs 6..16
             assert h.last_kernel().startswith(want), h.last_kernel()
     run_rank1(sp, oracle, cuda, h, A, (bs, mb, nb, rp, ci, v), "T", rng, -1.0, 1.0, np.float64)
+    # once more with mixed signs on the first 3000 block rows (the exact reference of the whole matrix is too slow)
+    ms = 3000
+    rps, cis = rp[:ms + 1], ci[:rp[ms]]
+    Am, vm = mixed(sp, cuda, bs, nb, rps, cis, v[:rp[ms] * bs * bs], seed=bs)
+    hm = sp.SPMVHandle()
+    for mode, alpha, beta in (("N", 1.0, 0.0), ("N", 3.7, -1.5), ("T", -1.0, 1.0)):
+        run_rank1(sp, oracle, cuda, hm, Am, (bs, ms, nb, rps, cis, vm), mode, rng, alpha, beta, np.float64, signed=True)
+        if mode == "N" and force:
+            assert hm.last_kernel().startswith("bsr_tile<" if bs <= 16 else "bsr_vector"), hm.last_kernel()
+        elif mode == "N":
+            want = "bsr_tile_e" if bs <= 5 else ("bsr_mm_tc<f64" if bs <= 16 else "bsr_vector")
+            assert hm.last_kernel().startswith(want), hm.last_kernel()
 
 
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
@@ -191,8 +248,11 @@ def test_long_block_rows_and_tail(cuda, oracle, dtype):
     v = rng.uniform(0, 10, len(ci) * bs * bs).astype(dtype)
     A = to_dev(sp, cuda, bs, nb, rp, ci, v)
     h = sp.SPMVHandle()
+    Am, vm = mixed(sp, cuda, bs, nb, rp, ci, v, seed=23)
     for alpha, beta in ((1.0, 0.0), (-1.0, 1.0), (3.7, -1.5)):
         run_rank1(sp, oracle, cuda, h, A, (bs, mb, nb, rp, ci, v), "N", rng, alpha, beta, dtype)
+        assert h.last_kernel().startswith("bsr_tile"), h.last_kernel()
+        run_rank1(sp, oracle, cuda, h, Am, (bs, mb, nb, rp, ci, vm), "N", rng, alpha, beta, dtype, signed=True)
         assert h.last_kernel().startswith("bsr_tile"), h.last_kernel()
 
 

@@ -292,6 +292,10 @@ def test_spmv_cached_transpose(cuda, oracle, dtype, tol):
     assert h.last_kernel().startswith("cached_transpose")
     err = np.max(np.abs(outs[0].astype(np.float64) - yref.astype(np.float64)) / np.maximum(scale, 1e-300))
     assert err <= tol, err
+    import exact_ref as R
+
+    R.assert_within(outs[0], R.spmm_exact(rp, ci, v, x, y0, alpha, beta, True), R.spmm_bound(rp, ci, v, x, y0, alpha, beta, True),
+                    h.last_kernel())
     assert np.array_equal(outs[0], outs[1]) and np.array_equal(outs[0], outs[2]), "deterministic: no atomics"
     # the values may change in place between calls: they are re-gathered
     A.values.mul_(2.0)

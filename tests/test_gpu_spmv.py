@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+import exact_ref as R
 from helpers import kk_matrix, rowwise_scale, spmv_tolerance
 
 pytestmark = pytest.mark.gpu
@@ -38,6 +39,9 @@ def run_case(sp, oracle, dev, handle, A, host, mode, alpha, beta, x, y0, ref_tol
     assert not bad.any(), f"mode {mode} a={alpha} b={beta}: {bad.sum()} rows beyond {tol} (max {np.max(err / np.maximum(scale, 1e-300)):.3e})"
     # the reference's own acceptance law against its own test oracle
     assert np.max(np.abs(got - exp3)) <= ref_tol + 1e-300
+    # entry by entry within the rounding bound of the exact product (tests/exact_ref.py)
+    R.assert_within(got, R.spmm_exact(rp, ci, v, x, y0, alpha, beta, trans), R.spmm_bound(rp, ci, v, x, y0, alpha, beta, trans),
+                    f"{handle.last_kernel() if handle is not None else 'no plan'} mode {mode} a={alpha} b={beta}")
     return got
 
 

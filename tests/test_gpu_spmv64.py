@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+import exact_ref as R
 from test_emulated_spmv64 import random_crs
 
 pytestmark = pytest.mark.gpu
@@ -41,6 +42,8 @@ def test_rank1_equals_the_32_bit_path(cuda, oracle, dtype, col_bits, window):
         if window is not None:
             h64.set_window(window)
         xd = torch.from_numpy(x).to(cuda)
+        exact = R.spmm_exact(rp64, ci32, v, x, y0, alpha, beta, trans)
+        bound = R.spmm_bound(rp64, ci32, v, x, y0, alpha, beta, trans)
         for _ in range(5):  # through the self-tuning phases of every window's plan
             y32, y64 = torch.from_numpy(y0).to(cuda), torch.from_numpy(y0).to(cuda)
             sp.spmv(h32, mode, alpha, A32, xd, beta, y32)
@@ -48,6 +51,10 @@ def test_rank1_equals_the_32_bit_path(cuda, oracle, dtype, col_bits, window):
             torch.cuda.synchronize()
             g32, g64 = y32.cpu().numpy(), y64.cpu().numpy()
             assert not np.isnan(g64).any()
+            k64 = h64.last_kernel()
+            assert k64.startswith(f"{h64.windows()} window{'' if h64.windows() == 1 else 's'} x "), k64
+            R.assert_within(g64, exact, bound, f"{k64} mode {mode} a={alpha} b={beta}")
+            R.assert_within(g32, exact, bound, f"{h32.last_kernel()} mode {mode} a={alpha} b={beta}")
             if trans:
                 assert np.allclose(g32, g64, rtol=0, atol=tol * 50)
             else:

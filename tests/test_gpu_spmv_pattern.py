@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+import exact_ref as R
 import pattern_cases as K
 from helpers import rowwise_scale
 
@@ -77,6 +78,7 @@ def check_oracle(oracle, A, x, y0, alpha, beta, y):
     tol = 1e-10 if x.dtype == np.float64 else 1e-4
     assert not np.isnan(y).any()
     assert np.all(np.abs(y - exp) <= tol * scale + 1e-300)
+    R.assert_within(y, R.spmm_exact(rp, ci, v, x, y0, alpha, beta), R.spmm_bound(rp, ci, v, x, y0, alpha, beta), f"a={alpha} b={beta}")
 
 
 def three_forms(cfg, lpr, Ad, xd, y0d, alpha, beta):
