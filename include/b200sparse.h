@@ -279,6 +279,27 @@ int b200sp_spgemm_jacobi_f32_i32(b200sp_spgemm_plan* plan, void* stream, int m, 
                                  const int* row_ptr_C, int* col_idx_C, float* vals_C, float omega,
                                  const float* dinv);
 
+/* Block SpGEMM numeric: replaces Impl::BSPGEMM_NUMERIC (native KokkosBSPGEMM + sort_bsr_matrix,
+ * sparse/impl/KokkosSparse_bspgemm_numeric_spec.hpp:113-191).  A is mb x nb blocks, B is nb x kb blocks, all
+ * bs x bs and row-major within the block; row_ptr_C is what b200sp_spgemm_symbolic_i32 wrote on the same plan for
+ * the BLOCK graphs (block symbolic is point symbolic, sparse/src/KokkosSparse_spgemm.hpp:77-103).  col_idx_C comes
+ * out sorted in every block row; vals_C holds nnz(C) * bs * bs values.  Entry (r, c) of block C(i, j) is one chain
+ * from +0.0 over the products of block row i in ordinal order (A's row in storage order, each B row in storage
+ * order) and, within a product, over p = 0..bs-1: acc = acc + a(r,p) * b(p,c), every multiply and add rounded on
+ * its own -- bit-identical to bspgemm_debug_numeric (sparse/impl/KokkosSparse_bspgemm_impl_seq.hpp:39-130) built
+ * without FMA contraction.  Rows need not be sorted; explicit zero blocks are kept.  bs == 1 forwards to
+ * b200sp_spgemm_numeric_*.  B200SP_ERR_INVALID_ARGUMENT for bs < 1, negative sizes or null arrays;
+ * B200SP_ERR_STATE without a prior symbolic.  The first call on a plan groups the block rows by product count
+ * (synchronises once); later calls with new value pointers on the same structure are asynchronous on `stream`. */
+int b200sp_bspgemm_numeric_f64_i32(b200sp_spgemm_plan* plan, void* stream, int mb, int nb, int kb, int bs,
+                                   const int* row_ptr_A, const int* col_idx_A, const double* vals_A,
+                                   const int* row_ptr_B, const int* col_idx_B, const double* vals_B,
+                                   const int* row_ptr_C, int* col_idx_C, double* vals_C);
+int b200sp_bspgemm_numeric_f32_i32(b200sp_spgemm_plan* plan, void* stream, int mb, int nb, int kb, int bs,
+                                   const int* row_ptr_A, const int* col_idx_A, const float* vals_A,
+                                   const int* row_ptr_B, const int* col_idx_B, const float* vals_B,
+                                   const int* row_ptr_C, int* col_idx_C, float* vals_C);
+
 /* ---- CrsMatrix utilities either side of the hot path (SURVEY.md section 8f) ----------------- */
 /* sort_crs_matrix / sort_crs_graph (sparse/src/KokkosSparse_SortCrs.hpp:43-120,209-270): every row
  * sorted ascending by column, values permuted along, IN PLACE.  The sort is stable (entries with the

@@ -66,6 +66,8 @@ SPARSE_API = {
     "b200sp_spgemm_numeric_f32_i32": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "b200sp_spgemm_jacobi_f64_i32": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, f64, vp]),
     "b200sp_spgemm_jacobi_f32_i32": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, f32, vp]),
+    "b200sp_bspgemm_numeric_f64_i32": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "b200sp_bspgemm_numeric_f32_i32": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "b200sp_sort_crs_f64_i32": (i32, [vp, i32, vp, vp, vp]),
     "b200sp_sort_crs_f32_i32": (i32, [vp, i32, vp, vp, vp]),
     "b200sp_sort_crs_graph_i32": (i32, [vp, i32, vp, vp]),

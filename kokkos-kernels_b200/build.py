@@ -16,7 +16,7 @@ NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
-CU_SOURCES = ["spmv.cu", "spmv64.cu", "spmm.cu", "spgemm.cu", "crs_utils.cu", "bsr.cu", "cg.cu", "gmres.cu", "gs.cu", "gs2.cu", "sptrsv.cu", "crs_io.cpp"]
+CU_SOURCES = ["spmv.cu", "spmv64.cu", "spmm.cu", "spgemm.cu", "bspgemm.cu", "crs_utils.cu", "bsr.cu", "cg.cu", "gmres.cu", "gs.cu", "gs2.cu", "sptrsv.cu", "crs_io.cpp"]
 
 
 def _newer(target, sources):
@@ -49,7 +49,7 @@ def build(force=False, verbose=True):
 def _build_locked(force, verbose):
     out = os.path.join(LIB, "libb200sparse.so")
     srcs = [os.path.join(CSRC, s) for s in CU_SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scan.cuh"), os.path.join(CSRC, "tile_ring.cuh"), os.path.join(CSRC, "spgemm_esc.cuh"), os.path.join(CSRC, "spmm_items.h"), os.path.join(HERE, "..", "include", "b200sparse.h")]
+    deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scan.cuh"), os.path.join(CSRC, "tile_ring.cuh"), os.path.join(CSRC, "spgemm_esc.cuh"), os.path.join(CSRC, "bspgemm.cuh"), os.path.join(CSRC, "spmm_items.h"), os.path.join(HERE, "..", "include", "b200sparse.h")]
     if force or not _newer(out, deps):
         objs = []
         procs = []
@@ -93,6 +93,17 @@ def _build_locked(force, verbose):
     if os.path.exists(hsrc) and (force or not _newer(hdrv, [hsrc, out] + hdeps + shim)):
         cmd = [_nvcc(), "-std=c++17", "-O1", "-Wno-deprecated-gpu-targets", "-I", os.path.join(root, "tests", "shim_mock"),
                "-I", os.path.join(HERE, "kokkos_shim"), "-I", os.path.join(root, "include"), hsrc, "-o", hdrv,
+               "-L", LIB, "-lb200sparse", "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN"]
+        if verbose:
+            print("[build]", " ".join(cmd), flush=True)
+        subprocess.check_call(cmd)
+    # the same for the block SpGEMM path: SPGEMM_SYMBOLIC on the block graphs + BSPGEMM_NUMERIC (Kokkos_Mock_Bspgemm.hpp)
+    bdrv = os.path.join(LIB, "shim_bspgemm_driver")
+    bsrc = os.path.join(root, "tests", "shim_mock", "shim_bspgemm_driver.cpp")
+    bdeps = [os.path.join(root, "tests", "shim_mock", f) for f in ("Kokkos_Mock.hpp", "Kokkos_Mock_Bspgemm.hpp")]
+    if os.path.exists(bsrc) and (force or not _newer(bdrv, [bsrc, out] + bdeps + shim)):
+        cmd = [_nvcc(), "-std=c++17", "-O1", "-Wno-deprecated-gpu-targets", "-I", os.path.join(root, "tests", "shim_mock"),
+               "-I", os.path.join(HERE, "kokkos_shim"), "-I", os.path.join(root, "include"), bsrc, "-o", bdrv,
                "-L", LIB, "-lb200sparse", "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN"]
         if verbose:
             print("[build]", " ".join(cmd), flush=True)

@@ -29,6 +29,7 @@
 #include "common.cuh"
 #include "scan.cuh"
 #include "spgemm_esc.cuh"
+#include "bspgemm.cuh"
 #include <algorithm>
 #include <limits.h>
 #include <stdlib.h>
@@ -1028,6 +1029,7 @@ struct b200sp_spgemm_plan {
   int* fb_keys = nullptr;
   void* fb_vals = nullptr;
   size_t fb_vals_bytes = 0;
+  b200sp::BspState* bsp = nullptr;  // block-row grouping of the block numeric phase (bspgemm.cu), built on first use
 };
 
 namespace b200sp {
@@ -1044,7 +1046,13 @@ static void spgemm_release(b200sp_spgemm_plan* p, cudaStream_t st) {
   p->cur_off = nullptr;
   p->fb_vals = nullptr;
   p->fb_vals_bytes = 0;
+  bsp_state_free(p->bsp, st);
+  p->bsp = nullptr;
   p->symbolic_done = false;
+}
+
+SpgemmPlanView spgemm_plan_view(b200sp_spgemm_plan* p) {
+  return SpgemmPlanView{p->symbolic_done, p->m, p->n, p->k, p->c_nnz, p->c_max, p->flops, &p->bsp};
 }
 
 static int bin_rows(cudaStream_t st, int m, const int* key, const BinSpec& spec, int* d_counts /*MAXBINS*/,

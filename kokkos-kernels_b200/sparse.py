@@ -861,12 +861,20 @@ def spgemm_symbolic_views(kh, m, n, k, row_mapA, entriesA, transposeA, row_mapB,
 
 
 def spgemm_numeric_views(kh, m, n, k, row_mapA, entriesA, valuesA, transposeA, row_mapB, entriesB, valuesB,
-                         transposeB, row_mapC, entriesC, valuesC):
+                         transposeB, row_mapC, entriesC, valuesC, block_dim=1):
+    """View-level spgemm_numeric (sparse/src/KokkosSparse_spgemm_numeric.hpp:35-256).  block_dim > 1: m, n, k count
+    blocks, the values hold bs*bs entries per block (row-major) and the product is the block SpGEMM
+    (b200sp_bspgemm_numeric_*, bit-identical to the reference's bspgemm_debug_numeric); block_dim == 1 is the point
+    product, as in the reference (:191)."""
     if transposeA or transposeB:
         raise B200SparseError("KokkosSparse::spgemm_numeric: transposing A or B is not supported")
     sh = kh.get_spgemm_handle()
     if sh is None or not sh.is_symbolic_called():  # numeric_spec.hpp:116-118
         raise B200SparseError("Call spgemm symbolic before spgemm numeric")
+    if int(block_dim) > 1:
+        _bspgemm_numeric(sh, m, n, k, int(block_dim), row_mapA, entriesA, valuesA, row_mapB, entriesB, valuesB, row_mapC,
+                         entriesC, valuesC)
+        return
     f64 = valuesA.dtype == torch.float64
     fn = _lib.sparse().b200sp_spgemm_numeric_f64_i32 if f64 else _lib.sparse().b200sp_spgemm_numeric_f32_i32
     check(fn(sh._plan, _stream(), m, n, k, _idx(row_mapA), _idx(entriesA), _ptr(valuesA), _idx(row_mapB),
@@ -912,6 +920,64 @@ def spgemm_jacobi(kh, A, Amode, B, Bmode, Cm, omega, dinv):
              _ptr(dv.contiguous())))
     sh._numeric = True
     sh._entries = True
+    return Cm
+
+
+def _bspgemm_numeric(sh, mb, nb, kb, bs, row_mapA, entriesA, valuesA, row_mapB, entriesB, valuesB, row_mapC, entriesC, valuesC):
+    if bs < 1:
+        raise B200SparseError(f"KokkosSparse::block_spgemm_numeric: inappropriate block size {bs}")
+    vals = (valuesA, valuesB, valuesC)
+    if any(v.dtype != valuesA.dtype for v in vals):
+        raise B200SparseError("KokkosSparse::block_spgemm_numeric: A, B and C must have the same scalar type "
+                              f"(got {valuesA.dtype}, {valuesB.dtype}, {valuesC.dtype})")
+    if any(t.dtype != torch.int32 for t in (row_mapA, entriesA, row_mapB, entriesB, row_mapC, entriesC)):
+        raise B200SparseError("KokkosSparse::block_spgemm_numeric: 64-bit offsets or ordinals are not provided for block "
+                              "SpGEMM (int32 row maps and entries only)")
+    for v, nz, what in ((valuesA, entriesA.numel(), "A"), (valuesB, entriesB.numel(), "B"), (valuesC, entriesC.numel(), "C")):
+        if v.numel() != nz * bs * bs:
+            raise B200SparseError(f"KokkosSparse::block_spgemm_numeric: values of {what} must hold nnz*blockDim*blockDim entries")
+    _sfx(valuesA)
+    L = _lib.sparse()
+    fn = L.b200sp_bspgemm_numeric_f64_i32 if valuesA.dtype == torch.float64 else L.b200sp_bspgemm_numeric_f32_i32
+    check(fn(sh._plan, _stream(), mb, nb, kb, bs, _idx(row_mapA), _idx(entriesA), _ptr(valuesA), _idx(row_mapB), _idx(entriesB),
+             _ptr(valuesB), _idx(row_mapC), _idx(entriesC), _ptr(valuesC)))
+    sh._numeric = True
+    sh._entries = True
+
+
+def block_spgemm_symbolic(kh, A, transposeA, B, transposeB):
+    """KokkosSparse::block_spgemm_symbolic (sparse/src/KokkosSparse_spgemm.hpp:77-103): the point symbolic on the block
+    graphs.  Returns a BsrMatrix C whose entries hold nnz(C) blocks and whose values hold nnz(C)*bs*bs entries
+    (uninitialised until block_spgemm_numeric)."""
+    if not isinstance(A, BsrMatrix) or not isinstance(B, BsrMatrix):
+        raise B200SparseError("KokkosSparse::block_spgemm_symbolic: A and B must be BsrMatrix")
+    bs = A.blockDim()
+    if bs != B.blockDim():
+        raise B200SparseInvalidArgument("Block SpGEMM must be called for matrices with the same block size")
+    if A.values.dtype != B.values.dtype:
+        raise B200SparseError(f"KokkosSparse::block_spgemm_symbolic: A and B must have the same scalar type "
+                              f"(got {A.values.dtype} and {B.values.dtype})")
+    _sfx(A.values)
+    m, n, k = A.numRows(), B.numRows(), B.numCols()
+    dev = A.row_map.device
+    row_mapC = torch.empty(m + 1, dtype=torch.int32, device=dev)
+    spgemm_symbolic_views(kh, m, n, k, A.row_map, A.entries, transposeA, B.row_map, B.entries, transposeB, row_mapC)
+    c_nnz = kh.get_spgemm_handle().get_c_nnz()
+    entriesC = torch.empty(c_nnz, dtype=torch.int32, device=dev)
+    valuesC = torch.empty(c_nnz * bs * bs, dtype=A.values.dtype, device=dev)
+    return BsrMatrix(row_mapC, entriesC, valuesC, k, bs)
+
+
+def block_spgemm_numeric(kh, A, transposeA, B, transposeB, Cm):
+    """KokkosSparse::block_spgemm_numeric (sparse/src/KokkosSparse_spgemm.hpp:145-156): fills C's sorted block columns and
+    values on the structure block_spgemm_symbolic produced with the same handle.  Re-runnable with new values."""
+    if transposeA or transposeB:
+        raise B200SparseError("KokkosSparse::spgemm_numeric: transposing A or B is not supported")
+    bs = A.blockDim()
+    if bs != B.blockDim() or bs != Cm.blockDim():
+        raise B200SparseInvalidArgument("Block SpGEMM must be called for matrices with the same block size")
+    spgemm_numeric_views(kh, A.numRows(), B.numRows(), B.numCols(), A.row_map, A.entries, A.values, transposeA, B.row_map,
+                         B.entries, B.values, transposeB, Cm.row_map, Cm.entries, Cm.values, block_dim=bs)
     return Cm
 
 

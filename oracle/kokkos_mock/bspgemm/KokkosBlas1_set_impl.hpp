@@ -1,0 +1,3 @@
+// Stand-in: SerialSetInternal lives in KokkosKernels_helpers.hpp of this directory.  TEST INFRASTRUCTURE ONLY.
+#pragma once
+#include "KokkosKernels_helpers.hpp"

@@ -19,8 +19,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, "kokkos-kernels_b200", "csrc")
 OUT = os.path.join(HERE, "_build")
-SOURCES = ["spmv.cu", "spmv64.cu", "spmm.cu", "spgemm.cu", "crs_utils.cu", "bsr.cu", "cg.cu", "gmres.cu", "gs.cu", "gs2.cu", "sptrsv.cu", "crs_io.cpp"]
-HEADERS = ["common.cuh", "scan.cuh", "tile_ring.cuh", "spgemm_esc.cuh", "spmm_items.h"]
+SOURCES = ["spmv.cu", "spmv64.cu", "spmm.cu", "spgemm.cu", "bspgemm.cu", "crs_utils.cu", "bsr.cu", "cg.cu", "gmres.cu", "gs.cu", "gs2.cu", "sptrsv.cu", "crs_io.cpp"]
+HEADERS = ["common.cuh", "scan.cuh", "tile_ring.cuh", "spgemm_esc.cuh", "bspgemm.cuh", "spmm_items.h"]
 
 
 def _match_back_angle(text, end):
