@@ -30,6 +30,7 @@
 
 #include <limits.h>
 #include "common.cuh"
+#include "tile_ring.cuh"
 
 namespace b200sp {
 
@@ -69,41 +70,6 @@ template <typename S>
 __device__ __forceinline__ void bsr_store(S* __restrict__ p, S sum, S alpha, S beta) {
   sum *= alpha;
   *p = (beta == S(0)) ? sum : beta * *p + sum;
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// tile analysis (the CSR one of spmv.cu with blocks for entries): tile b owns the block rows whose first block lies in
-// [b*T, (b+1)*T); descriptor {r0, r1, s, e}, e capped so that [s & ~3, e) fits the stage.
-// ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ int bsr_lower_bound(const int* __restrict__ row_ptr, int m, int64_t v) {
-  int lo = 0, hi = m;
-  while (lo < hi) {
-    const int mid = lo + ((hi - lo) >> 1);
-    if ((int64_t)row_ptr[mid] < v) lo = mid + 1;
-    else hi = mid;
-  }
-  return lo;
-}
-
-__global__ void bsr_build_tiles_kernel(int mb, const int* __restrict__ row_ptr, int n_tiles, int T, int capb, int4* __restrict__ tiles) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= n_tiles) return;
-  const int r0 = bsr_lower_bound(row_ptr, mb, (int64_t)b * T);
-  const int r1 = bsr_lower_bound(row_ptr, mb, (int64_t)(b + 1) * T);
-  int s = 0, e = 0;
-  if (r1 > r0) {
-    s = row_ptr[r0];
-    e = row_ptr[r1];
-    const int cap_end = (s & ~3) + capb - 4;
-    if (e > cap_end) e = cap_end;  // only a long last block row can exceed the stage; the tile kernel skips it
-  }
-  tiles[b] = make_int4(r0, r1, s, e);
-}
-
-__global__ void bsr_find_long_rows_kernel(int mb, const int* __restrict__ row_ptr, int lmaxb, int* __restrict__ long_rows,
-                                          int* __restrict__ n_long) {
-  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < mb; r += gridDim.x * blockDim.x)
-    if (row_ptr[r + 1] - row_ptr[r] > lmaxb) long_rows[atomicAdd(n_long, 1)] = r;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -193,93 +159,16 @@ __global__ void __launch_bounds__(256) bsr_vector_kernel(int mb, int bs, int lpr
 // ---------------------------------------------------------------------------------------------------------------
 // the TMA-tiled kernel
 // ---------------------------------------------------------------------------------------------------------------
+// the ring of the BSR kernels: VCAP values per stage, columns and row-map entries for VCAP / 4 blocks (bs >= 2)
 template <typename S, int VCAP, int STAGES>
-struct BsrSmem {
-  static constexpr int CCAP = VCAP / 4;  // block slots of a stage (bs >= 2)
-  static constexpr int RCAP = CCAP;      // staged row-map entries of a stage
-  alignas(128) S vals[STAGES][VCAP];
-  alignas(128) int cols[STAGES][CCAP];
-  alignas(128) int rows[STAGES][RCAP];
-  int4 desc[STAGES];
-  alignas(8) uint64_t full[STAGES];
-  alignas(8) uint64_t empty[STAGES];
-};
-
-// The producer warp of both tile kernels: streams tile after tile into the ring (values, block columns, row-map slice).
-template <typename S, typename Smem, int STAGES>
-__device__ __forceinline__ void bsr_produce(Smem& sm, int lane, int mb, int64_t nnzb, int vpe, int n_tiles, const int4* __restrict__ tiles,
-                                            const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
-                                            const S* __restrict__ vals) {
-  constexpr int RCAP = Smem::RCAP;
-  const uint64_t pol = l2_policy_evict_first();
-  const int64_t nnzb_al = nnzb & ~(int64_t)3;  // bulk copies stay below this block
-  const int rp_al_end = (mb + 1) & ~3;         // ... and below this row-map entry
-  int4 mine = make_int4(0, 0, 0, 0);
-  for (int it = 0;; ++it) {
-    const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-    if (tile >= n_tiles) break;
-    if ((it & 31) == 0) {
-      const int64_t t = blockIdx.x + (int64_t)(it + lane) * gridDim.x;
-      if (t < n_tiles) mine = tiles[t];
-    }
-    int4 d;
-    d.x = __shfl_sync(0xffffffffu, mine.x, it & 31);
-    d.y = __shfl_sync(0xffffffffu, mine.y, it & 31);
-    d.z = __shfl_sync(0xffffffffu, mine.z, it & 31);
-    d.w = __shfl_sync(0xffffffffu, mine.w, it & 31);
-    const int stage = it % STAGES;
-    const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-    mbar_wait(&sm.empty[stage], ph ^ 1u);
-
-    const int r0 = d.x, r1 = d.y, s = d.z, e = d.w;
-    S* sv = sm.vals[stage];
-    int* sc = sm.cols[stage];
-    int* sr = sm.rows[stage];
-    // blocks [s_al, e) -> stage slot 0..; bulk part [s_al, bulk_end), the last (< 4) blocks of the matrix by plain loads
-    const int s_al = s & ~3;
-    const int e_up = (e + 3) & ~3;
-    const int bulk_end = (int)((int64_t)e_up < nnzb_al ? (int64_t)e_up : nnzb_al);
-    const int nbk = (r1 > r0 && bulk_end > s_al) ? bulk_end - s_al : 0;
-    if (r1 > r0 && (int64_t)e > nnzb_al) {
-      const int t0 = (int)((int64_t)s_al > nnzb_al ? (int64_t)s_al : nnzb_al);
-      for (int b = t0 + lane; b < e; b += 32) sc[b - s_al] = col_idx[b];
-      const int64_t v0 = (int64_t)t0 * vpe, v1 = (int64_t)e * vpe, voff = (int64_t)s_al * vpe;
-      for (int64_t q = v0 + lane; q < v1; q += 32) sv[q - voff] = vals[q];
-    }
-    const int r0_al = r0 & ~3;
-    int nrp = 0;
-    if (r1 > r0) {
-      const int want_end = min(r1 + 1, r0_al + RCAP);  // exclusive
-      const int want_up = (want_end + 3) & ~3;
-      const int rbulk_end = min(min(want_up, r0_al + RCAP), rp_al_end);
-      nrp = rbulk_end > r0_al ? rbulk_end - r0_al : 0;
-      if (want_end > rp_al_end) {
-        const int t0 = max(r0_al, rp_al_end);
-        for (int i = t0 + lane; i < want_end; i += 32) sr[i - r0_al] = row_ptr[i];
-      }
-    }
-    __syncwarp();
-    if (lane == 0) {
-      sm.desc[stage] = d;
-      const uint32_t vbytes = (uint32_t)((size_t)nbk * vpe * sizeof(S));
-      mbar_arrive_expect_tx(&sm.full[stage], vbytes + (uint32_t)(nbk * 4) + (uint32_t)(nrp * 4));
-      if (nbk > 0) {
-        bulk_g2s(sv, vals + (int64_t)s_al * vpe, vbytes, &sm.full[stage], pol);
-        bulk_g2s(sc, col_idx + s_al, (uint32_t)(nbk * 4), &sm.full[stage], pol);
-      }
-      if (nrp > 0) bulk_g2s(sr, row_ptr + r0_al, (uint32_t)(nrp * 4), &sm.full[stage], pol);
-    }
-    __syncwarp();
-  }
-}
+using BsrTileRing = TileRing<S, VCAP, VCAP / 4, VCAP / 4, STAGES>;
 
 template <typename S, int NW, int STAGES, int VCAP, int UNR>
 __global__ void __launch_bounds__((NW + 1) * 32)
     bsr_tile_kernel(int mb, int64_t nnzb, int bs, int lpr, int lmaxb, int n_tiles, const int4* __restrict__ tiles,
                     const int* __restrict__ row_ptr, const int* __restrict__ col_idx, const S* __restrict__ vals,
                     const S* __restrict__ x, S* __restrict__ y, S alpha, S beta) {
-  using Smem = BsrSmem<S, VCAP, STAGES>;
-  constexpr int RCAP = Smem::RCAP;
+  using Smem = BsrTileRing<S, VCAP, STAGES>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
 
@@ -287,18 +176,10 @@ __global__ void __launch_bounds__((NW + 1) * 32)
   const int lane = threadIdx.x & 31;
   const int vpe = bs * bs;
 
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&sm.full[s], 1);    // the producer's arrive.expect_tx (+ the bytes of its bulk copies)
-      mbar_init(&sm.empty[s], NW);  // one arrive per consumer warp
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
+  tile_ring_init(sm, NW);
 
   if (warp == NW) {
-    bsr_produce<S, Smem, STAGES>(sm, lane, mb, nnzb, vpe, n_tiles, tiles, row_ptr, col_idx, vals);
+    tile_ring_produce(sm, lane, mb, nnzb, vpe, n_tiles, tiles, row_ptr, col_idx, vals);
   } else {
     // ------------------------------------------------ consumer warps
     const int G = bs * lpr;    // lanes of one block row
@@ -307,19 +188,11 @@ __global__ void __launch_bounds__((NW + 1) * 32)
     const int lr = (lane % G) / lpr, sl = lane % lpr;
     const bool lane_used = b_in < BRW;
     const int j0 = sl / bs, i0 = sl % bs, dj = lpr / bs, di = lpr % bs;
-    for (int it = 0;; ++it) {
-      const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-      if (tile >= n_tiles) break;
-      const int stage = it % STAGES;
-      const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-      mbar_wait(&sm.full[stage], ph);
-      const int4 d = sm.desc[stage];
-      const int r0 = d.x, r1 = d.y;
-      const int s_al = d.z & ~3;
-      const int r0_al = r0 & ~3;
+    for (int it = 0; tile_ring_more(it, n_tiles); ++it) {
+      const TileView tv = tile_ring_acquire<4, 4>(sm, it);
+      const int stage = tv.stage, r0 = tv.r0, r1 = tv.r1, s_al = tv.s_al;
       const S* sv = sm.vals[stage];
       const int* sc = sm.cols[stage];
-      const int* sr = sm.rows[stage];
       // absolute groups of BRW block rows are dealt round-robin to the warps
       const int g_first = r0 / BRW;
       int g = g_first + ((warp - g_first % NW) + NW) % NW;
@@ -327,16 +200,7 @@ __global__ void __launch_bounds__((NW + 1) * 32)
         const int brow = g * BRW + b_in;
         const bool valid = lane_used && (brow >= r0) && (brow < r1);
         int rs = 0, re = 0;
-        if (valid) {
-          const int o = brow - r0_al;
-          if (o + 1 < RCAP) {
-            rs = sr[o];
-            re = sr[o + 1];
-          } else {
-            rs = row_ptr[brow];
-            re = row_ptr[brow + 1];
-          }
-        }
+        if (valid) tile_row_bounds(sm, stage, row_ptr, brow, brow - tv.r0_al, rs, re);
         const bool is_long = (re - rs) > lmaxb;  // left to bsr_vector_kernel
         if (is_long) re = rs;
         S sum = bsr_row_dot<S, UNR, false>(sv + (rs - s_al) * vpe + lr * bs, sc + (rs - s_al), x, (re - rs) * bs, bs, vpe, lpr, sl, j0, i0,
@@ -344,8 +208,7 @@ __global__ void __launch_bounds__((NW + 1) * 32)
         sum = bsr_group_sum(sum, lpr);
         if (valid && !is_long && sl == 0) bsr_store(y + (int64_t)brow * bs + lr, sum, alpha, beta);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.empty[stage]);
+      tile_ring_release(sm, stage, lane);
     }
   }
 }
@@ -364,8 +227,7 @@ __global__ void __launch_bounds__((NW + 1) * 32)
     bsr_tile_e_kernel(int mb, int64_t nnzb, int lmaxb, int n_tiles, const int4* __restrict__ tiles, const int* __restrict__ row_ptr,
                       const int* __restrict__ col_idx, const S* __restrict__ vals, const S* __restrict__ x, S* __restrict__ y, S alpha,
                       S beta) {
-  using Smem = BsrSmem<S, VCAP, STAGES>;
-  constexpr int RCAP = Smem::RCAP;
+  using Smem = BsrTileRing<S, VCAP, STAGES>;
   constexpr int VPE = BS * BS;
   constexpr int P = 32 / VPE;
   static_assert(P >= 1, "element-per-lane kernel needs BS*BS <= 32");
@@ -375,46 +237,23 @@ __global__ void __launch_bounds__((NW + 1) * 32)
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&sm.full[s], 1);
-      mbar_init(&sm.empty[s], NW);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
+  tile_ring_init(sm, NW);
 
   if (warp == NW) {
-    bsr_produce<S, Smem, STAGES>(sm, lane, mb, nnzb, VPE, n_tiles, tiles, row_ptr, col_idx, vals);
+    tile_ring_produce(sm, lane, mb, nnzb, VPE, n_tiles, tiles, row_ptr, col_idx, vals);
   } else {
     const int p = lane / VPE, e = lane % VPE;
     const int lr = e / BS, i = e % BS;
     const bool lane_used = p < P;
-    for (int it = 0;; ++it) {
-      const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-      if (tile >= n_tiles) break;
-      const int stage = it % STAGES;
-      const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-      mbar_wait(&sm.full[stage], ph);
-      const int4 d = sm.desc[stage];
-      const int r0 = d.x, r1 = d.y;
-      const int s_al = d.z & ~3;
-      const int r0_al = r0 & ~3;
+    for (int it = 0; tile_ring_more(it, n_tiles); ++it) {
+      const TileView tv = tile_ring_acquire<4, 4>(sm, it);
+      const int stage = tv.stage, r0 = tv.r0, r1 = tv.r1, s_al = tv.s_al;
       const S* sv = sm.vals[stage];
       const int* sc = sm.cols[stage];
-      const int* sr = sm.rows[stage];
       // block rows dealt round-robin to the warps by absolute index
       for (int brow = r0 + ((warp - r0 % NW) + NW) % NW; brow < r1; brow += NW) {
         int rs, re;
-        const int o = brow - r0_al;
-        if (o + 1 < RCAP) {
-          rs = sr[o];
-          re = sr[o + 1];
-        } else {
-          rs = row_ptr[brow];
-          re = row_ptr[brow + 1];
-        }
+        tile_row_bounds(sm, stage, row_ptr, brow, brow - tv.r0_al, rs, re);
         if (re - rs > lmaxb) continue;  // left to bsr_vector_kernel (uniform across the warp)
         const int nblk = re - rs;
         const S* vb = sv + (rs - s_al) * VPE + e;
@@ -445,8 +284,7 @@ __global__ void __launch_bounds__((NW + 1) * 32)
         for (int q = 1; q < P; ++q) r += __shfl_down_sync(0xffffffffu, t, q * VPE);
         if (p == 0 && i == 0) bsr_store(y + (int64_t)brow * BS + lr, r, alpha, beta);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.empty[stage]);
+      tile_ring_release(sm, stage, lane);
     }
   }
 }
@@ -677,19 +515,15 @@ int bsr_analyse(b200sp_bsr_plan* p, cudaStream_t st, int mb, int64_t nnzb, int b
   if (p->tiles && p->key_row_ptr == row_ptr && p->key_mb == mb && p->key_nnzb == nnzb && p->key_bs == bs && p->key_capb == capb)
     return B200SP_OK;
   bsr_release(p, st);
-  p->lmaxb = capb / 4;
-  p->T = capb - p->lmaxb - 8;
-  p->n_tiles = (int)(nnzb / p->T) + 1;
-  const int long_cap = (int)(nnzb / (p->lmaxb + 1)) + 1;
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->tiles, sizeof(int4) * (size_t)p->n_tiles, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->long_rows, sizeof(int) * (size_t)long_cap, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->n_long, sizeof(int), st));
-  B200SP_CUDA_TRY(cudaMemsetAsync(p->n_long, 0, sizeof(int), st));
-  bsr_build_tiles_kernel<<<(p->n_tiles + 255) / 256, 256, 0, st>>>(mb, row_ptr, p->n_tiles, p->T, capb, p->tiles);
-  B200SP_LAUNCH_CHECK();
-  bsr_find_long_rows_kernel<<<std::max(1, std::min((mb + 255) / 256, sm_count() * 8)), 256, 0, st>>>(mb, row_ptr, p->lmaxb, p->long_rows,
-                                                                                                    p->n_long);
-  B200SP_LAUNCH_CHECK();
+  TileAnalysis a;
+  const int rc = tile_analyse(st, mb, nnzb, row_ptr, capb, capb / 4, &a);  // blocks for entries
+  p->tiles = a.tiles;
+  p->n_tiles = a.n_tiles;
+  p->T = a.T;
+  p->lmaxb = a.LMAX;
+  p->long_rows = a.long_rows;
+  p->n_long = a.n_long;
+  if (rc != B200SP_OK) return rc;
   p->key_row_ptr = row_ptr;
   p->key_mb = mb;
   p->key_nnzb = nnzb;
@@ -714,7 +548,7 @@ int launch_vector(b200sp_bsr_plan* p, cudaStream_t st, int mb, int64_t nnzb, int
 template <typename S, int NW, int STAGES, int VCAP>
 int launch_tile(b200sp_bsr_plan* p, cudaStream_t st, int mb, int64_t nnzb, int bs, const int* rp, const int* ci, const S* v, const S* x,
                 S* y, S alpha, S beta) {
-  using Smem = BsrSmem<S, VCAP, STAGES>;
+  using Smem = BsrTileRing<S, VCAP, STAGES>;
   constexpr int UNR = 4;
   auto kern = bsr_tile_kernel<S, NW, STAGES, VCAP, UNR>;
   const size_t smem = sizeof(Smem) + 128;
@@ -741,7 +575,7 @@ int launch_tile(b200sp_bsr_plan* p, cudaStream_t st, int mb, int64_t nnzb, int b
 template <typename S, int BS, int NW, int STAGES, int VCAP>
 int launch_tile_e(b200sp_bsr_plan* p, cudaStream_t st, int mb, int64_t nnzb, const int* rp, const int* ci, const S* v, const S* x, S* y,
                   S alpha, S beta) {
-  using Smem = BsrSmem<S, VCAP, STAGES>;
+  using Smem = BsrTileRing<S, VCAP, STAGES>;
   constexpr int UNR = 4;
   auto kern = bsr_tile_e_kernel<S, BS, NW, STAGES, VCAP, UNR>;
   const size_t smem = sizeof(Smem) + 128;

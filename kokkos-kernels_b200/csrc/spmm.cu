@@ -431,49 +431,31 @@ __global__ void __launch_bounds__((NW + 1) * 32)
     spmm_tile_kernel(int m, int k, int64_t nnz, int n_tiles, int LMAX, const int4* __restrict__ tiles,
                      const int* __restrict__ row_ptr, const int* __restrict__ col_idx, const S* __restrict__ vals,
                      const S* __restrict__ X, int64_t ldx, S* __restrict__ Y, int64_t ldy, S alpha, S beta) {
-  using Ring = TileRing<S, CAP, STAGES>;
-  constexpr int RCAP = Ring::RCAP;
+  using Ring = CsrTileRing<S, CAP, STAGES>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Ring& sm = *reinterpret_cast<Ring*>(smem_raw);
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   tile_ring_init(sm, NW);
   if (warp == NW) {
-    tile_ring_produce<S, CAP, STAGES>(sm, lane, m, nnz, n_tiles, tiles, row_ptr, col_idx, vals);
+    tile_ring_produce(sm, lane, m, nnz, 1, n_tiles, tiles, row_ptr, col_idx, vals);
     return;
   }
   constexpr int RPW = 32 / KTL;  // rows per warp
   const int sub = lane / KTL, t = lane % KTL;
   const int nstrips = (k + KTL * VW - 1) / (KTL * VW);
-  for (int it = 0;; ++it) {
-    const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-    if (tile >= n_tiles) break;
-    const int stage = it % STAGES;
-    const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-    mbar_wait(&sm.full[stage], ph);
-    const int4 d = sm.desc[stage];
-    const int r0 = d.x, r1 = d.y;
-    const int s_al = d.z & ~3;
-    const int r0_al = r0 & ~3;
+  for (int it = 0; tile_ring_more(it, n_tiles); ++it) {
+    const TileView tv = tile_ring_acquire<4, 4>(sm, it);
+    const int stage = tv.stage, r0 = tv.r0, r1 = tv.r1, s_al = tv.s_al;
     const S* sv = sm.vals[stage];
     const int* sc = sm.cols[stage];
-    const int* sr = sm.rows[stage];
     const int g_first = r0 / RPW;
     int g = g_first + ((warp - g_first % NW) + NW) % NW;
     for (; g * RPW < r1; g += NW) {
       const int r = g * RPW + sub;
       const bool valid = (r >= r0) && (r < r1);
       int rs = 0, re = 0;
-      if (valid) {
-        const int o = r - r0_al;
-        if (o + 1 < RCAP) {
-          rs = sr[o];
-          re = sr[o + 1];
-        } else {
-          rs = row_ptr[r];
-          re = row_ptr[r + 1];
-        }
-      }
+      if (valid) tile_row_bounds(sm, stage, row_ptr, r, r - tv.r0_al, rs, re);
       const bool is_long = (re - rs) > LMAX;
       if (is_long) re = rs;
       const int jbeg = rs - s_al, jend = re - s_al;
@@ -527,8 +509,7 @@ __global__ void __launch_bounds__((NW + 1) * 32)
         }
       }
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&sm.empty[stage]);
+    tile_ring_release(sm, stage, lane);
   }
 }
 
@@ -893,7 +874,7 @@ int plan_analyse_mm(b200sp_spmv_plan* p, cudaStream_t st, int cap, int lmax, int
 template <typename S, int VW, int KTL, int NW, int STAGES, int CAP, int UNR>
 static int launch_mm_tile_k(cudaStream_t st, const MMTileView& tv, int m, int k, int64_t nnz, const int* row_ptr,
                             const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
-  using Ring = TileRing<S, CAP, STAGES>;
+  using Ring = CsrTileRing<S, CAP, STAGES>;
   auto kern = spmm_tile_kernel<S, VW, KTL, NW, STAGES, CAP, UNR>;
   const size_t smem = sizeof(Ring) + 128;
   static KernelSetup ks;  // per instantiation and device: attribute set + occupancy queried once

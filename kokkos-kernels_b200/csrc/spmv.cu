@@ -361,6 +361,26 @@ __global__ void find_long_rows_kernel(int m, const int* __restrict__ row_ptr, in
     if (row_ptr[r + 1] - row_ptr[r] > LMAX) long_rows[atomicAdd(n_long, 1)] = r;
 }
 
+// The tiles and long rows of the tile kernels (spmv_tile_kernel, spmm_tile_kernel, the BSR ones of bsr.cu with blocks for
+// entries) for a stage of cap entries and a row limit of lmax.  *out owns what it allocated, also on an error.
+int tile_analyse(cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int cap, int lmax, TileAnalysis* out) {
+  *out = TileAnalysis();
+  out->LMAX = lmax;
+  out->T = cap - lmax - 8;
+  out->n_tiles = (int)(nnz / out->T) + 1;
+  out->long_cap = (int)(nnz / (lmax + 1)) + 1;  // every long row holds more than lmax entries
+  B200SP_CUDA_TRY(cudaMallocAsync((void**)&out->tiles, sizeof(int4) * (size_t)out->n_tiles, st));
+  B200SP_CUDA_TRY(cudaMallocAsync((void**)&out->long_rows, sizeof(int) * (size_t)out->long_cap, st));
+  B200SP_CUDA_TRY(cudaMallocAsync((void**)&out->n_long, sizeof(int), st));
+  B200SP_CUDA_TRY(cudaMemsetAsync(out->n_long, 0, sizeof(int), st));
+  build_tiles_kernel<<<(out->n_tiles + 255) / 256, 256, 0, st>>>(m, row_ptr, out->n_tiles, out->T, cap, out->tiles);
+  B200SP_LAUNCH_CHECK();
+  find_long_rows_kernel<<<std::max(1, std::min((m + 255) / 256, sm_count() * 8)), 256, 0, st>>>(m, row_ptr, lmax, out->long_rows,
+                                                                                                out->n_long);
+  B200SP_LAUNCH_CHECK();
+  return B200SP_OK;
+}
+
 // 16-bit column form of the tiled kernel (DESIGN.md section 3.5): d[j] = col_idx[j] - col_idx[j-1] inside a row, 0 for the
 // first entry of a row; anchor[r] = col_idx[row_ptr[r]], 0 for an empty row.  *bad is set when a row the tiled kernel reads
 // (<= LMAX entries) has an in-row delta outside [0, 65535] (unsorted, or a gap too wide); longer rows go to the long-row
@@ -525,19 +545,7 @@ __global__ void pattern_assign_kernel(int m, const int* __restrict__ row_ptr, co
 __device__ __forceinline__ int64_t dmin64(int64_t a, int64_t b) { return a < b ? a : b; }
 __device__ __forceinline__ int64_t dmax64(int64_t a, int64_t b) { return a > b ? a : b; }
 
-template <typename S, int CAP, int STAGES>
-struct TileSmem {
-  static constexpr int RCAP = CAP / 2;  // staged row_ptr entries per tile
-  alignas(128) S vals[STAGES][CAP];
-  // 32-bit columns; in the 16-bit form the same 4*CAP bytes hold CAP column deltas (uint16) followed by RCAP anchors (int)
-  alignas(128) int cols[STAGES][CAP];
-  alignas(128) int rows[STAGES][RCAP];
-  int4 desc[STAGES];
-  alignas(8) uint64_t full[STAGES];
-  alignas(8) uint64_t empty[STAGES];
-};
-
-// column area of the ring (TileSmem::cols) in the pattern form: per stage RCAP anchors and RCAP pattern starts, 3*CAP of its
+// column area of the ring (TileRing::cols) in the pattern form: per stage RCAP anchors and RCAP pattern starts, 3*CAP of its
 // 4*CAP bytes, and one dictionary in the STAGES*CAP bytes that frees (>= 5 KB in every configuration).  The ring is no larger
 // than in the 32-bit form, so occupancy is the same.
 template <int CAP, int STAGES>
@@ -557,7 +565,7 @@ enum TileCols { COLS_I32 = 0, COLS_DELTA = 1, COLS_PAT = 2 };
 template <typename S, int NW, int STAGES, int CAP>
 constexpr int tile_ctas_per_sm() {
   const int by_regs = 65536 / ((NW + 1) * 32 * 56);
-  const int by_smem = (227 * 1024) / (int)(sizeof(TileSmem<S, CAP, STAGES>) + 128 + 1024);
+  const int by_smem = (227 * 1024) / (int)(sizeof(CsrTileRing<S, CAP, STAGES>) + 128 + 1024);
   const int c = by_regs < by_smem ? by_regs : by_smem;
   return c > 1 ? c : 1;
 }
@@ -575,7 +583,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
                      const uint16_t* __restrict__ c16, const int* __restrict__ anchor, const int* __restrict__ dict,
                      const S* __restrict__ vals, const S* __restrict__ x, S* __restrict__ y, S alpha,
                      S beta, YExtra ex) {
-  using Smem = TileSmem<S, CAP, STAGES>;
+  using Smem = CsrTileRing<S, CAP, STAGES>;
   using PatCols = TilePatCols<CAP, STAGES>;
   static_assert(sizeof(PatCols) <= sizeof(int) * STAGES * CAP, "the pattern form's columns must fit the 32-bit ring");
   constexpr int RCAP = Smem::RCAP;
@@ -595,15 +603,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
     const int dl = dict[DCAP];  // used length
     for (int i = threadIdx.x; i < dl; i += blockDim.x) pc.dict[i] = dict[i];
   }
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&sm.full[s], 1);    // producer's arrive.expect_tx (+ TMA byte count)
-      mbar_init(&sm.empty[s], NW);  // one arrive per consumer warp
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
+  tile_ring_init(sm, NW);
 
   if (warp == NW) {
     // ------------------------- producer warp ------------------------------
@@ -730,21 +730,13 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
     // ------------------------- consumer warps -----------------------------
     constexpr int RPW = 32 / LPR;
     const int sub = lane / LPR, sl = lane % LPR;
-    for (int it = 0;; ++it) {
-      const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-      if (tile >= n_tiles) break;
-      const int stage = it % STAGES;
-      const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-      mbar_wait(&sm.full[stage], ph);
-      const int4 d = sm.desc[stage];
-      const int r0 = d.x, r1 = d.y;
-      const int s_al = d.z & ~(EAL - 1);
-      const int r0_al = r0 & ~(RAL - 1);
+    for (int it = 0; tile_ring_more(it, n_tiles); ++it) {
+      const TileView tv = tile_ring_acquire<EAL, RAL>(sm, it);
+      const int stage = tv.stage, r0 = tv.r0, r1 = tv.r1, s_al = tv.s_al;
       const S* sv = sm.vals[stage];
       const int* sc = sm.cols[stage];
       const uint16_t* sd = reinterpret_cast<const uint16_t*>(sc);
       const int* sa = PAT ? pc.anchor[stage] : reinterpret_cast<const int*>(sd + CAP);
-      const int* sr = sm.rows[stage];
       // absolute row groups of RPW rows are dealt round-robin to the warps
       const int g_first = r0 / RPW;
       int g = g_first + ((warp - g_first % NW) + NW) % NW;
@@ -753,15 +745,11 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
         const bool valid = (r >= r0) && (r < r1);
         int rs = 0, re = 0, col = 0, pb = 0;
         if (valid) {
-          const int o = r - r0_al;
-          if (o + 1 < RCAP) {
-            rs = sr[o];
-            re = sr[o + 1];
+          const int o = r - tv.r0_al;
+          if (tile_row_bounds(sm, stage, row_ptr, r, o, rs, re)) {
             if (COLS != COLS_I32) col = sa[o];
             if (PAT) pb = pc.pid[stage][o];
           } else {
-            rs = row_ptr[r];
-            re = row_ptr[r + 1];
             if (COLS != COLS_I32) col = anchor[r];
             if (PAT) pb = c16[r];
           }
@@ -808,9 +796,11 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
 #pragma unroll
             for (int u = 0; u < UNR; ++u) sum += av[u] * xv[u];
           }
-        } else if constexpr (PAT) {
-          // the 32-bit form's loop with col + dict[pb + k] for the column of the row's entry k: the rows of a warp mostly
-          // share a pattern, so the dictionary reads are mostly broadcasts
+        } else {
+          // UNR predicated entries per lane per pass: all gathers of a row (<= UNR*LPR entries) are
+          // in flight together -- one memory latency per row instead of one per remainder step.  PAT: the column of the
+          // row's entry k is col + dict[pb + k]; the rows of a warp mostly share a pattern, so the dictionary reads are
+          // mostly broadcasts
           const int db = pb - (rs - s_al);
           for (int j0 = rs + sl - s_al; j0 < jend; j0 += UNR * LPR) {
             int c[UNR];
@@ -819,25 +809,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
             for (int u = 0; u < UNR; ++u) {
               const int j = j0 + u * LPR;
               const bool ok = j < jend;
-              c[u] = ok ? col + pc.dict[db + j] : 0;
-              av[u] = ok ? sv[j] : S(0);
-            }
-#pragma unroll
-            for (int u = 0; u < UNR; ++u) xv[u] = (j0 + u * LPR < jend) ? ldg(x + c[u]) : S(0);
-#pragma unroll
-            for (int u = 0; u < UNR; ++u) sum += av[u] * xv[u];
-          }
-        } else {
-          // UNR predicated entries per lane per pass: all gathers of a row (<= UNR*LPR entries) are
-          // in flight together -- one memory latency per row instead of one per remainder step
-          for (int j0 = rs + sl - s_al; j0 < jend; j0 += UNR * LPR) {
-            int c[UNR];
-            S av[UNR], xv[UNR];
-#pragma unroll
-            for (int u = 0; u < UNR; ++u) {
-              const int j = j0 + u * LPR;
-              const bool ok = j < jend;
-              c[u] = ok ? sc[j] : 0;
+              if constexpr (PAT) c[u] = ok ? col + pc.dict[db + j] : 0;
+              else c[u] = ok ? sc[j] : 0;
               av[u] = ok ? sv[j] : S(0);
             }
 #pragma unroll
@@ -849,8 +822,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
         sum = subwarp_sum<LPR>(sum);
         if (valid && !is_long && sl == 0) store_y(y, r, sum, alpha, beta, ex);
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.empty[stage]);
+      tile_ring_release(sm, stage, lane);
     }
   }
 }
@@ -1145,20 +1117,16 @@ static int plan_analyse(b200sp_spmv_plan* p, cudaStream_t st, int cfg, int m, in
     return B200SP_OK;
   plan_release_analysis(p, st);
   const TileCfg c = kCfgs[cfg];
-  p->LMAX = c.cap / 4;
-  p->T = c.cap - p->LMAX - 8;
-  p->n_tiles = (int)(nnz / p->T) + 1;
-  // every long row holds more than LMAX entries
-  p->long_cap = (int)(nnz / (p->LMAX + 1)) + 1;
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->tiles, sizeof(int4) * (size_t)p->n_tiles, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->long_rows, sizeof(int) * (size_t)p->long_cap, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->n_long, sizeof(int), st));
-  B200SP_CUDA_TRY(cudaMemsetAsync(p->n_long, 0, sizeof(int), st));
-  build_tiles_kernel<<<(p->n_tiles + 255) / 256, 256, 0, st>>>(m, row_ptr, p->n_tiles, p->T, c.cap, p->tiles);
-  B200SP_LAUNCH_CHECK();
-  find_long_rows_kernel<<<std::max(1, std::min((m + 255) / 256, sm_count() * 8)), 256, 0, st>>>(m, row_ptr, p->LMAX,
-                                                                                                p->long_rows, p->n_long);
-  B200SP_LAUNCH_CHECK();
+  TileAnalysis a;
+  const int rc = tile_analyse(st, m, nnz, row_ptr, c.cap, c.cap / 4, &a);
+  p->tiles = a.tiles;
+  p->n_tiles = a.n_tiles;
+  p->T = a.T;
+  p->LMAX = a.LMAX;
+  p->long_rows = a.long_rows;
+  p->n_long = a.n_long;
+  p->long_cap = a.long_cap;
+  if (rc != B200SP_OK) return rc;
   if (!p->n_long_host) B200SP_CUDA_TRY(cudaMallocHost((void**)&p->n_long_host, sizeof(int)));
   if (!p->n_long_event) B200SP_CUDA_TRY(cudaEventCreateWithFlags(&p->n_long_event, cudaEventDisableTiming));
   *p->n_long_host = -1;
@@ -1316,24 +1284,20 @@ int plan_analyse_mm(b200sp_spmv_plan* p, cudaStream_t st, int cap, int lmax, int
         p->mm_key_lmax == lmax)) {
     plan_release_mm(p, st);
     p->mm_cap = cap;
-    p->mm_LMAX = lmax;
-    p->mm_T = cap - lmax - 8;
-    p->mm_n_tiles = (int)(nnz / p->mm_T) + 1;
-    const int long_cap = (int)(nnz / (lmax + 1)) + 1;  // every long row holds more than lmax entries
-    p->mm_seg_cap = (int)(nnz / seg) + long_cap + 1;
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->mm_tiles, sizeof(int4) * (size_t)p->mm_n_tiles, st));
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->mm_long_rows, sizeof(int) * (size_t)long_cap, st));
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->mm_n_long, sizeof(int), st));
+    TileAnalysis a;
+    const int rc = tile_analyse(st, m, nnz, row_ptr, cap, lmax, &a);
+    p->mm_tiles = a.tiles;
+    p->mm_n_tiles = a.n_tiles;
+    p->mm_T = a.T;
+    p->mm_LMAX = a.LMAX;
+    p->mm_long_rows = a.long_rows;
+    p->mm_n_long = a.n_long;
+    if (rc != B200SP_OK) return rc;
+    p->mm_seg_cap = (int)(nnz / seg) + a.long_cap + 1;
     B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->mm_segs, sizeof(int4) * (size_t)p->mm_seg_cap, st));
     B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->mm_n_seg, sizeof(int), st));
-    B200SP_CUDA_TRY(cudaMemsetAsync(p->mm_n_long, 0, sizeof(int), st));
     B200SP_CUDA_TRY(cudaMemsetAsync(p->mm_n_seg, 0, sizeof(int), st));
-    build_tiles_kernel<<<(p->mm_n_tiles + 255) / 256, 256, 0, st>>>(m, row_ptr, p->mm_n_tiles, p->mm_T, cap, p->mm_tiles);
-    B200SP_LAUNCH_CHECK();
-    find_long_rows_kernel<<<std::max(1, std::min((m + 255) / 256, sm_count() * 8)), 256, 0, st>>>(m, row_ptr, lmax, p->mm_long_rows,
-                                                                                                  p->mm_n_long);
-    B200SP_LAUNCH_CHECK();
-    build_segments_kernel<<<std::max(1, std::min((long_cap + 255) / 256, sm_count() * 4)), 256, 0, st>>>(
+    build_segments_kernel<<<std::max(1, std::min((a.long_cap + 255) / 256, sm_count() * 4)), 256, 0, st>>>(
         p->mm_long_rows, p->mm_n_long, row_ptr, seg, p->mm_segs, p->mm_n_seg);
     B200SP_LAUNCH_CHECK();
     p->mm_key_row_ptr = row_ptr;
@@ -1370,7 +1334,7 @@ int spmv_lanes_per_row(int64_t m, int64_t nnz) {  // also used by spmv64.cu: one
 template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, int COLS>
 static int launch_tile_form(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr,
                             const int* col_idx, const S* vals, const S* x, S* y, S alpha, S beta) {
-  using Smem = TileSmem<S, CAP, STAGES>;
+  using Smem = CsrTileRing<S, CAP, STAGES>;
   auto kern = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, COLS, false>;
   const uint16_t* c16 = COLS == COLS_PAT ? p->pat_pid : p->idx16_d;
   const int* anchor = p->idx16_anchor;

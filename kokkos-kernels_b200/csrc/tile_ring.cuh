@@ -1,28 +1,34 @@
-// tile_ring.cuh -- the shared-memory ring of row-aligned CSR tiles that a producer warp fills with
-// 1-D TMA bulk copies (cp.async.bulk + mbarrier), as used by spmv_tile_kernel (spmv.cu, DESIGN.md 3.1).
-// The producer loop here is the one of spmv_tile_kernel, factored out for the rank-2 kernel
-// (spmm.cu); the tile descriptors are the plan's (build_tiles_kernel, spmv.cu).
+// tile_ring.cuh -- the shared-memory ring of row-aligned tiles that a producer warp fills with 1-D TMA bulk copies
+// (cp.async.bulk + mbarrier) for the consumer warps of the tile kernels: spmv_tile_kernel (spmv.cu, DESIGN.md 3.1),
+// spmm_tile_kernel (spmm.cu) and the BsrMatrix tile kernels (bsr.cu), whose entries are blocks of bs*bs values.  The
+// tile descriptors are made once for all of them by tile_analyse (build_tiles_kernel, spmv.cu).
 #pragma once
 #include "common.cuh"
 
 namespace b200sp {
 
-template <typename S, int CAP, int STAGES>
+// STAGES stages of VCAP values, CCAP 32-bit columns (entries) and RCAP row_ptr entries
+template <typename S_, int VCAP_, int CCAP_, int RCAP_, int STAGES_>
 struct TileRing {
-  static constexpr int RCAP = CAP / 2;  // staged row_ptr entries per tile
-  alignas(128) S vals[STAGES][CAP];
-  alignas(128) int cols[STAGES][CAP];
+  using S = S_;
+  static constexpr int VCAP = VCAP_, CCAP = CCAP_, RCAP = RCAP_, STAGES = STAGES_;
+  alignas(128) S vals[STAGES][VCAP];
+  alignas(128) int cols[STAGES][CCAP];
   alignas(128) int rows[STAGES][RCAP];
   int4 desc[STAGES];
   alignas(8) uint64_t full[STAGES];
   alignas(8) uint64_t empty[STAGES];
 };
 
+// the ring of the CSR kernels: CAP entries per stage, row_ptr entries for CAP/2 rows
 template <typename S, int CAP, int STAGES>
-__device__ __forceinline__ void tile_ring_init(TileRing<S, CAP, STAGES>& sm, int n_consumer_warps) {
+using CsrTileRing = TileRing<S, CAP, CAP, CAP / 2, STAGES>;
+
+template <typename Ring>
+__device__ __forceinline__ void tile_ring_init(Ring& sm, int n_consumer_warps) {
   if (threadIdx.x == 0) {
 #pragma unroll
-    for (int s = 0; s < STAGES; ++s) {
+    for (int s = 0; s < Ring::STAGES; ++s) {
       mbar_init(&sm.full[s], 1);                    // producer's arrive.expect_tx (+ TMA byte count)
       mbar_init(&sm.empty[s], n_consumer_warps);    // one arrive per consumer warp
     }
@@ -31,76 +37,177 @@ __device__ __forceinline__ void tile_ring_init(TileRing<S, CAP, STAGES>& sm, int
   __syncthreads();
 }
 
-// Runs in ONE warp (all 32 lanes).  Tile `it` of this CTA is tiles[blockIdx.x + it*gridDim.x]:
-// descriptor {r0, r1, s, e}; stage layout: entries [s & ~3, e) at vals/cols[0..), row_ptr[r0 & ~3 ..] at
-// rows[0..) (at most RCAP entries).  Sources are aligned down to 16 bytes; the last < 4 entries of an
-// array are copied with plain loads so that no bulk copy reads past the allocation.
-template <typename S, int CAP, int STAGES>
-__device__ __forceinline__ void tile_ring_produce(TileRing<S, CAP, STAGES>& sm, int lane, int m, int64_t nnz, int n_tiles,
-                                                  const int4* __restrict__ tiles, const int* __restrict__ row_ptr,
-                                                  const int* __restrict__ col_idx, const S* __restrict__ vals) {
-  constexpr int RCAP = TileRing<S, CAP, STAGES>::RCAP;
-  const uint64_t pol = l2_policy_evict_first();
-  const int64_t nnz_al = nnz & ~(int64_t)3;  // bulk copies stay below this entry
-  const int rp_al_end = (m + 1) & ~3;        // ... and below this row_ptr entry
-  int4 mine = make_int4(0, 0, 0, 0);
-  for (int it = 0;; ++it) {
-    const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-    if (tile >= n_tiles) break;
-    if ((it & 31) == 0) {
-      const int64_t t = blockIdx.x + (int64_t)(it + lane) * gridDim.x;
-      if (t < n_tiles) mine = tiles[t];
-    }
-    int4 d;
-    d.x = __shfl_sync(0xffffffffu, mine.x, it & 31);
-    d.y = __shfl_sync(0xffffffffu, mine.y, it & 31);
-    d.z = __shfl_sync(0xffffffffu, mine.z, it & 31);
-    d.w = __shfl_sync(0xffffffffu, mine.w, it & 31);
-    const int stage = it % STAGES;
-    const uint32_t ph = (uint32_t)(it / STAGES) & 1u;
-    mbar_wait(&sm.empty[stage], ph ^ 1u);
+// Tile `it` of this CTA is tiles[blockIdx.x + it*gridDim.x]; it goes to stage it % STAGES.
+__device__ __forceinline__ bool tile_ring_more(int it, int n_tiles) { return blockIdx.x + (int64_t)it * gridDim.x < n_tiles; }
 
-    const int r0 = d.x, r1 = d.y, s = d.z, e = d.w;
-    S* sv = sm.vals[stage];
-    int* sc = sm.cols[stage];
-    int* sr = sm.rows[stage];
-    const int s_al = s & ~3;
-    const int e_up = (e + 3) & ~3;
-    const int64_t bulk_end64 = (int64_t)e_up < nnz_al ? (int64_t)e_up : nnz_al;
-    const int bulk_end = (int)bulk_end64;
-    const int nb = (r1 > r0 && bulk_end > s_al) ? bulk_end - s_al : 0;
-    if (r1 > r0 && (int64_t)e > nnz_al) {
-      const int t0 = (int)((int64_t)s_al > nnz_al ? (int64_t)s_al : nnz_al);
+// ---------------------------------------------------------------------------------------------------------------------
+// producer: ONE warp (all 32 lanes)
+// ---------------------------------------------------------------------------------------------------------------------
+// Descriptor {r0, r1, s, e} of tile `it` into d (the descriptors of 32 tiles are loaded at a time, one per lane, and handed
+// out by shuffles), then waits until the consumers have left its stage.  False past this CTA's last tile.
+template <typename Ring>
+__device__ __forceinline__ bool tile_ring_next(Ring& sm, int it, int lane, int n_tiles, const int4* __restrict__ tiles, int4& mine,
+                                               int4& d) {
+  if (!tile_ring_more(it, n_tiles)) return false;
+  if ((it & 31) == 0) {
+    const int64_t t = blockIdx.x + (int64_t)(it + lane) * gridDim.x;
+    if (t < n_tiles) mine = tiles[t];
+  }
+  d.x = __shfl_sync(0xffffffffu, mine.x, it & 31);
+  d.y = __shfl_sync(0xffffffffu, mine.y, it & 31);
+  d.z = __shfl_sync(0xffffffffu, mine.z, it & 31);
+  d.w = __shfl_sync(0xffffffffu, mine.w, it & 31);
+  const int stage = it % Ring::STAGES;
+  const uint32_t ph = (uint32_t)(it / Ring::STAGES) & 1u;
+  mbar_wait(&sm.empty[stage], ph ^ 1u);
+  return true;
+}
+
+// what tile_ring_stage leaves to lane 0's bulk copies
+struct TileStage {
+  int s_al, r0_al;  // first staged entry, first staged row_ptr entry
+  int nb, nrp;      // entries and row_ptr entries copied in bulk
+};
+
+// Stages tile d: entries [s_al, e) -- vpe values each and their 32-bit columns -- at vals/cols[0..), and row_ptr[r0_al ..]
+// at rows[0..) (at most RCAP entries), where s_al = s & ~3 and r0_al = r0 & ~3.  Bulk copies stay below entry
+// nnz_al = nnz & ~3 and row_ptr entry rp_al_end = (m + 1) & ~3, which keeps them inside the arrays and every length a
+// multiple of 16 bytes; here the rest of the tile is copied with plain loads, and tile_ring_issue then issues the bulk part.
+template <typename Ring>
+__device__ __forceinline__ TileStage tile_ring_stage(Ring& sm, int stage, int4 d, int lane, int64_t nnz_al, int rp_al_end, int vpe,
+                                                     const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
+                                                     const typename Ring::S* __restrict__ vals) {
+  constexpr int RCAP = Ring::RCAP;
+  const int r0 = d.x, r1 = d.y, s = d.z, e = d.w;
+  typename Ring::S* sv = sm.vals[stage];
+  int* sc = sm.cols[stage];
+  int* sr = sm.rows[stage];
+  TileStage ts;
+  ts.s_al = s & ~3;
+  const int e_up = (e + 3) & ~3;
+  const int64_t bulk_end64 = (int64_t)e_up < nnz_al ? (int64_t)e_up : nnz_al;
+  const int bulk_end = (int)bulk_end64;
+  ts.nb = (r1 > r0 && bulk_end > ts.s_al) ? bulk_end - ts.s_al : 0;
+  if (r1 > r0 && (int64_t)e > nnz_al) {
+    const int t0 = (int)((int64_t)ts.s_al > nnz_al ? (int64_t)ts.s_al : nnz_al);
+    if constexpr (Ring::CCAP == Ring::VCAP) {  // a column slot per value: one value per entry (CSR, vpe == 1)
       for (int i = t0 + lane; i < e; i += 32) {
-        sv[i - s_al] = vals[i];
-        sc[i - s_al] = col_idx[i];
+        sv[i - ts.s_al] = vals[i];
+        sc[i - ts.s_al] = col_idx[i];
       }
+    } else {
+      for (int b = t0 + lane; b < e; b += 32) sc[b - ts.s_al] = col_idx[b];
+      const int64_t v0 = (int64_t)t0 * vpe, v1 = (int64_t)e * vpe, voff = (int64_t)ts.s_al * vpe;
+      for (int64_t q = v0 + lane; q < v1; q += 32) sv[q - voff] = vals[q];
     }
-    const int r0_al = r0 & ~3;
-    int nrp = 0;
-    if (r1 > r0) {
-      const int want_end = min(r1 + 1, r0_al + RCAP);  // exclusive
-      const int want_up = (want_end + 3) & ~3;
-      const int rbulk_end = min(min(want_up, r0_al + RCAP), rp_al_end);
-      nrp = rbulk_end > r0_al ? rbulk_end - r0_al : 0;
-      if (want_end > rp_al_end) {
-        const int t0 = max(r0_al, rp_al_end);
-        for (int i = t0 + lane; i < want_end; i += 32) sr[i - r0_al] = row_ptr[i];
-      }
+  }
+  ts.r0_al = r0 & ~3;
+  ts.nrp = 0;
+  if (r1 > r0) {
+    const int want_end = min(r1 + 1, ts.r0_al + RCAP);  // exclusive
+    const int want_up = (want_end + 3) & ~3;
+    const int rbulk_end = min(min(want_up, ts.r0_al + RCAP), rp_al_end);
+    ts.nrp = rbulk_end > ts.r0_al ? rbulk_end - ts.r0_al : 0;
+    if (want_end > rp_al_end) {
+      const int t0 = max(ts.r0_al, rp_al_end);
+      for (int i = t0 + lane; i < want_end; i += 32) sr[i - ts.r0_al] = row_ptr[i];
     }
+  }
+  return ts;
+}
+
+// Lane 0, after a __syncwarp behind tile_ring_stage: publishes the descriptor, arms the stage's `full` barrier with the bytes
+// of the bulk copies and issues them.
+template <typename Ring>
+__device__ __forceinline__ void tile_ring_issue(Ring& sm, int stage, int4 d, const TileStage& ts, int vpe, const int* __restrict__ row_ptr,
+                                                const int* __restrict__ col_idx, const typename Ring::S* __restrict__ vals,
+                                                uint64_t pol) {
+  sm.desc[stage] = d;
+  const uint32_t vbytes = (uint32_t)((size_t)ts.nb * vpe * sizeof(typename Ring::S));
+  mbar_arrive_expect_tx(&sm.full[stage], vbytes + (uint32_t)(ts.nb * 4) + (uint32_t)(ts.nrp * 4));
+  if (ts.nb > 0) {
+    bulk_g2s(sm.vals[stage], vals + (int64_t)ts.s_al * vpe, vbytes, &sm.full[stage], pol);
+    bulk_g2s(sm.cols[stage], col_idx + ts.s_al, (uint32_t)(ts.nb * 4), &sm.full[stage], pol);
+  }
+  if (ts.nrp > 0) bulk_g2s(sm.rows[stage], row_ptr + ts.r0_al, (uint32_t)(ts.nrp * 4), &sm.full[stage], pol);
+}
+
+// The producer of spmm_tile_kernel and the BSR tile kernels (vpe values per entry: 1 for CSR, bs*bs for BSR).
+// spmv_tile_kernel has its own, which also streams its 16-bit column forms.
+template <typename Ring>
+__device__ __forceinline__ void tile_ring_produce(Ring& sm, int lane, int m, int64_t nnz, int vpe, int n_tiles,
+                                                  const int4* __restrict__ tiles, const int* __restrict__ row_ptr,
+                                                  const int* __restrict__ col_idx, const typename Ring::S* __restrict__ vals) {
+  const uint64_t pol = l2_policy_evict_first();
+  const int64_t nnz_al = nnz & ~(int64_t)3;
+  const int rp_al_end = (m + 1) & ~3;
+  int4 mine = make_int4(0, 0, 0, 0), d;
+  for (int it = 0; tile_ring_next(sm, it, lane, n_tiles, tiles, mine, d); ++it) {
+    const int stage = it % Ring::STAGES;
+    const TileStage ts = tile_ring_stage(sm, stage, d, lane, nnz_al, rp_al_end, vpe, row_ptr, col_idx, vals);
     __syncwarp();
-    if (lane == 0) {
-      sm.desc[stage] = d;
-      mbar_arrive_expect_tx(&sm.full[stage], (uint32_t)(nb * (sizeof(S) + 4) + nrp * 4));
-      if (nb > 0) {
-        bulk_g2s(sv, vals + s_al, (uint32_t)(nb * sizeof(S)), &sm.full[stage], pol);
-        bulk_g2s(sc, col_idx + s_al, (uint32_t)(nb * 4), &sm.full[stage], pol);
-      }
-      if (nrp > 0) bulk_g2s(sr, row_ptr + r0_al, (uint32_t)(nrp * 4), &sm.full[stage], pol);
-    }
+    if (lane == 0) tile_ring_issue(sm, stage, d, ts, vpe, row_ptr, col_idx, vals, pol);
     __syncwarp();
   }
 }
+
+// ---------------------------------------------------------------------------------------------------------------------
+// consumers
+// ---------------------------------------------------------------------------------------------------------------------
+// the stage of tile `it`, once the producer's copies have landed: its rows [r0, r1) and where its entries (s_al) and row_ptr
+// entries (r0_al) start, aligned as tile_ring_stage aligned them
+struct TileView {
+  int stage, r0, r1, s_al, r0_al;
+};
+
+template <int EAL, int RAL, typename Ring>
+__device__ __forceinline__ TileView tile_ring_acquire(Ring& sm, int it) {
+  TileView t;
+  t.stage = it % Ring::STAGES;
+  const uint32_t ph = (uint32_t)(it / Ring::STAGES) & 1u;
+  mbar_wait(&sm.full[t.stage], ph);
+  const int4 d = sm.desc[t.stage];
+  t.r0 = d.x;
+  t.r1 = d.y;
+  t.s_al = d.z & ~(EAL - 1);
+  t.r0_al = t.r0 & ~(RAL - 1);
+  return t;
+}
+
+// every lane of the warp: the warp is done with the stage
+template <typename Ring>
+__device__ __forceinline__ void tile_ring_release(Ring& sm, int stage, int lane) {
+  __syncwarp();
+  if (lane == 0) mbar_arrive(&sm.empty[stage]);
+}
+
+// row_ptr[r] and row_ptr[r + 1] of row r of the tile: from the stage when both are staged (o = r - r0_al), else from global
+// memory.  Returns whether they were staged.
+template <typename Ring>
+__device__ __forceinline__ bool tile_row_bounds(const Ring& sm, int stage, const int* __restrict__ row_ptr, int r, int o, int& rs,
+                                                int& re) {
+  if (o + 1 < Ring::RCAP) {
+    rs = sm.rows[stage][o];
+    re = sm.rows[stage][o + 1];
+    return true;
+  }
+  rs = row_ptr[r];
+  re = row_ptr[r + 1];
+  return false;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// tile analysis (spmv.cu): tile b owns the rows whose first entry lies in [b*T, (b+1)*T), T = cap - lmax - 8; rows longer
+// than lmax are listed for the caller's long-row kernel.  Stream-ordered, no host synchronisation.
+// ---------------------------------------------------------------------------------------------------------------------
+struct TileAnalysis {
+  int4* tiles = nullptr;  // {r0, r1, s, e} per tile
+  int n_tiles = 0, T = 0, LMAX = 0;
+  int* long_rows = nullptr;  // long_cap entries, *n_long of them used
+  int* n_long = nullptr;
+  int long_cap = 0;
+};
+int tile_analyse(cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int cap, int lmax, TileAnalysis* out);
 
 // what plan_analyse_mm (spmv.cu) hands to the rank-2 tile kernel (spmm.cu)
 struct MMTileView {
