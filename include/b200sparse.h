@@ -300,6 +300,44 @@ int b200sp_bspgemm_numeric_f32_i32(b200sp_spgemm_plan* plan, void* stream, int m
                                    const int* row_ptr_B, const int* col_idx_B, const float* vals_B,
                                    const int* row_ptr_C, int* col_idx_C, float* vals_C);
 
+/* ---- SpGEMM on 64-bit offsets (products past 2^31 entries) -------------- */
+/* Replaces the (int ordinal, size_t offset) instantiations of SPGEMM_SYMBOLIC / SPGEMM_NUMERIC, Kokkos' default offsets
+ * in a Trilinos build (cmake/kokkoskernels_eti_offsets.cmake:1-11), which the cuSPARSE slot cannot take
+ * (sparse/tpls/KokkosSparse_spgemm_numeric_tpl_spec_avail.hpp:38-41).  row_ptr_A / row_ptr_B / row_ptr_C have m+1 /
+ * n+1 / m+1 int64 entries (size_t offsets below 2^63 read the same); column indices stay int32.  Any nnz(A) and nnz(C);
+ * nnz(B) must not exceed 2^31-65537 (every window reads all of B; B200SP_ERR_OVERFLOW, naming B), nor may one row of A
+ * hold more entries or products than the window limit (B200SP_ERR_OVERFLOW).  m, n, k and each row's entries stay below 2^31, as on the 32-bit path.
+ * Symbolic reads the 64-bit structure once: B's row map is narrowed to int32 (4 B per row of B), the rows of A are cut
+ * into at most 4096 windows of consecutive rows holding at most `limit` products and entries (an int64 scan and a
+ * search), and every window runs b200sp_spgemm_symbolic_i32 on a child plan with a row map relative to its first entry
+ * (4 B per row of A) and keeps its relative C row map (4 B per row of C).  Otherwise the contract is that of
+ * b200sp_spgemm_symbolic_i32: all m+1 entries of row_ptr_C are written, c_nnz is the sum over the windows and
+ * c_max_row_nnz the maximum, one handle serves one product (B200SP_ERR_STATE for another, also for a plan whose
+ * symbolic had 32-bit offsets; the same product again is idempotent), synchronises `stream`. */
+int b200sp_spgemm_symbolic_i64(b200sp_spgemm_plan* plan, void* stream, int m, int n, int k,
+                               const int64_t* row_ptr_A, const int* col_idx_A, const int64_t* row_ptr_B,
+                               const int* col_idx_B, int64_t* row_ptr_C, int64_t* c_nnz, int* c_max_row_nnz);
+/* Numeric on the windows symbolic cut: b200sp_spgemm_numeric_*_i32 per window on the relative row maps and on
+ * col_idx / vals of A and C shifted by the window's first entry.  Each row runs the kernel the 32-bit entry points run it
+ * on: row map and columns equal theirs, and so do the values, bit for bit, of every row of at most 8192 products (and
+ * 4096 entries of A).  Longer rows go to hash kernels that add with atomics on the GPU, so their values may differ in
+ * the last bits from one run to the next, on either path.  Asynchronous on `stream`, re-runnable with new value
+ * pointers.  B200SP_ERR_STATE when the plan's symbolic had 32-bit offsets or was not called; conversely the 32-bit
+ * numeric, spgemm_jacobi and block numeric entries return B200SP_ERR_STATE on a plan whose symbolic had 64-bit offsets
+ * (spgemm_jacobi and block SpGEMM are not provided on 64-bit offsets). */
+int b200sp_spgemm_numeric_f64_i64(b200sp_spgemm_plan* plan, void* stream, int m, int n, int k,
+                                  const int64_t* row_ptr_A, const int* col_idx_A, const double* vals_A,
+                                  const int64_t* row_ptr_B, const int* col_idx_B, const double* vals_B,
+                                  const int64_t* row_ptr_C, int* col_idx_C, double* vals_C);
+int b200sp_spgemm_numeric_f32_i64(b200sp_spgemm_plan* plan, void* stream, int m, int n, int k,
+                                  const int64_t* row_ptr_A, const int* col_idx_A, const float* vals_A,
+                                  const int64_t* row_ptr_B, const int* col_idx_B, const float* vals_B,
+                                  const int64_t* row_ptr_C, int* col_idx_C, float* vals_C);
+/* Window limit of the next 64-bit symbolic on this plan: products and entries of A per window, 8 .. 2^31-65537 (the
+ * default); smaller limits only make sense for tests.  _windows: the windows of the last 64-bit symbolic (0 for none). */
+int b200sp_spgemm_plan_set_window(b200sp_spgemm_plan* plan, int64_t max_entries);
+int b200sp_spgemm_plan_windows(const b200sp_spgemm_plan* plan);
+
 /* ---- CrsMatrix utilities either side of the hot path (SURVEY.md section 8f) ----------------- */
 /* sort_crs_matrix / sort_crs_graph (sparse/src/KokkosSparse_SortCrs.hpp:43-120,209-270): every row
  * sorted ascending by column, values permuted along, IN PLACE.  The sort is stable (entries with the

@@ -66,6 +66,11 @@ SPARSE_API = {
     "b200sp_spgemm_numeric_f32_i32": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "b200sp_spgemm_jacobi_f64_i32": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, f64, vp]),
     "b200sp_spgemm_jacobi_f32_i32": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, f32, vp]),
+    "b200sp_spgemm_symbolic_i64": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, C.POINTER(i64), C.POINTER(i32)]),
+    "b200sp_spgemm_numeric_f64_i64": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "b200sp_spgemm_numeric_f32_i64": (i32, [vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "b200sp_spgemm_plan_set_window": (i32, [vp, i64]),
+    "b200sp_spgemm_plan_windows": (i32, [vp]),
     "b200sp_bspgemm_numeric_f64_i32": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "b200sp_bspgemm_numeric_f32_i32": (i32, [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "b200sp_sort_crs_f64_i32": (i32, [vp, i32, vp, vp, vp]),

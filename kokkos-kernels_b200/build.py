@@ -16,7 +16,7 @@ NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
-CU_SOURCES = ["spmv.cu", "spmv64.cu", "spmm.cu", "spgemm.cu", "bspgemm.cu", "crs_utils.cu", "bsr.cu", "cg.cu", "gmres.cu", "gs.cu", "gs2.cu", "sptrsv.cu", "crs_io.cpp"]
+CU_SOURCES = ["spmv.cu", "spmv64.cu", "spmm.cu", "spgemm.cu", "spgemm64.cu", "bspgemm.cu", "crs_utils.cu", "bsr.cu", "cg.cu", "gmres.cu", "gs.cu", "gs2.cu", "sptrsv.cu", "crs_io.cpp"]
 
 
 def _newer(target, sources):
@@ -104,6 +104,17 @@ def _build_locked(force, verbose):
     if os.path.exists(bsrc) and (force or not _newer(bdrv, [bsrc, out] + bdeps + shim)):
         cmd = [_nvcc(), "-std=c++17", "-O1", "-Wno-deprecated-gpu-targets", "-I", os.path.join(root, "tests", "shim_mock"),
                "-I", os.path.join(HERE, "kokkos_shim"), "-I", os.path.join(root, "include"), bsrc, "-o", bdrv,
+               "-L", LIB, "-lb200sparse", "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN"]
+        if verbose:
+            print("[build]", " ".join(cmd), flush=True)
+        subprocess.check_call(cmd)
+    # the same for the (int, size_t) SPGEMM_SYMBOLIC / SPGEMM_NUMERIC specialisations (64-bit offsets)
+    sdrv = os.path.join(LIB, "shim_spgemm64_driver")
+    ssrc = os.path.join(root, "tests", "shim_mock", "shim_spgemm64_driver.cpp")
+    sdeps = [os.path.join(root, "tests", "shim_mock", "Kokkos_Mock.hpp")]
+    if os.path.exists(ssrc) and (force or not _newer(sdrv, [ssrc, out] + sdeps + shim)):
+        cmd = [_nvcc(), "-std=c++17", "-O1", "-Wno-deprecated-gpu-targets", "-I", os.path.join(root, "tests", "shim_mock"),
+               "-I", os.path.join(HERE, "kokkos_shim"), "-I", os.path.join(root, "include"), ssrc, "-o", sdrv,
                "-L", LIB, "-lb200sparse", "-Xlinker", "-rpath", "-Xlinker", "$ORIGIN"]
         if verbose:
             print("[build]", " ".join(cmd), flush=True)

@@ -334,6 +334,10 @@ template <typename S>
 static int bspgemm_impl(b200sp_spgemm_plan* plan, cudaStream_t st, int mb, int nb, int kb, int bs, const int* rpA, const int* ciA,
                         const S* vA, const int* rpB, const int* ciB, const S* vB, const int* rpC, int* ciC, S* vC) {
   const SpgemmPlanView v = spgemm_plan_view(plan);
+  if (spgemm64_holds_product(*v.s64)) {
+    set_error("block_spgemm_numeric: not provided on 64-bit offsets (the symbolic phase on this handle had them)");
+    return B200SP_ERR_STATE;
+  }
   if (!v.symbolic_done) {
     set_error("KokkosSparse::block_spgemm_numeric: must first call spgemm_symbolic with the same handle.");
     return B200SP_ERR_STATE;

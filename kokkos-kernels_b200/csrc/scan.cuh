@@ -120,4 +120,66 @@ static inline int launch_exclusive_scan(cudaStream_t st, int m, const int* count
   return B200SP_OK;
 }
 
+// ---- the same scan into int64 offsets, for totals past 2^31 (spgemm64.cu) ----------------------------------------------
+// Templates on the count type so that only the translation units that use them compile them.
+template <typename Cnt>
+static __global__ void __launch_bounds__(256) scan64_local_kernel(int m, const Cnt* __restrict__ cnt, int64_t* __restrict__ out,
+                                                                  long long* __restrict__ block_sum, int* __restrict__ block_max) {
+  __shared__ long long wsum[8];
+  const int base = blockIdx.x * SCAN_ITEMS + threadIdx.x * 8;
+  long long v[8];
+  long long s = 0;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    v[i] = (base + i < m) ? (long long)cnt[base + i] : 0;
+    s += v[i];
+  }
+  long long inc = s;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    long long t = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += t;
+  }
+  if (lane == 31) wsum[w] = inc;
+  __syncthreads();
+  long long run = inc - s;
+  for (int i = 0; i < w; ++i) run += wsum[i];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    if (base + i < m) out[base + i] = run;
+    run += v[i];
+  }
+  if (threadIdx.x == 255) {
+    long long tot = 0;
+    for (int i = 0; i < 8; ++i) tot += wsum[i];
+    block_sum[blockIdx.x] = tot;
+    block_max[blockIdx.x] = 0;
+  }
+}
+template <typename Cnt>
+static __global__ void __launch_bounds__(256) scan64_add_kernel(int m, int64_t* __restrict__ out, const long long* __restrict__ block_off,
+                                                                const long long* __restrict__ total) {
+  const long long off = block_off[blockIdx.x];
+  const int base = blockIdx.x * SCAN_ITEMS + threadIdx.x * 8;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    if (base + i < m) out[base + i] += off;
+  if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) out[m] = *total;
+}
+
+// counts[0..m) -> out[0..m] as int64 (exclusive offsets, out[m] = *d_total = total); scratch as launch_exclusive_scan's.
+template <typename Cnt>
+static inline int launch_exclusive_scan64(cudaStream_t st, int m, const Cnt* counts, int64_t* out, long long* block_sum,
+                                          int* block_max, long long* d_total, int* d_max) {
+  const int nblocks = scan_blocks(m);  // m > 0
+  scan64_local_kernel<Cnt><<<nblocks, 256, 0, st>>>(m, counts, out, block_sum, block_max);
+  B200SP_LAUNCH_CHECK();
+  scan_blocks_kernel<<<1, 1024, 0, st>>>(nblocks, block_sum, block_max, d_total, d_max);
+  B200SP_LAUNCH_CHECK();
+  scan64_add_kernel<Cnt><<<nblocks, 256, 0, st>>>(m, out, block_sum, d_total);
+  B200SP_LAUNCH_CHECK();
+  return B200SP_OK;
+}
+
 }  // namespace b200sp

@@ -1030,6 +1030,7 @@ struct b200sp_spgemm_plan {
   void* fb_vals = nullptr;
   size_t fb_vals_bytes = 0;
   b200sp::BspState* bsp = nullptr;  // block-row grouping of the block numeric phase (bspgemm.cu), built on first use
+  b200sp::Spgemm64State* s64 = nullptr;  // a product with 64-bit offsets (spgemm64.cu): the 32-bit entries refuse the plan
 };
 
 namespace b200sp {
@@ -1052,7 +1053,7 @@ static void spgemm_release(b200sp_spgemm_plan* p, cudaStream_t st) {
 }
 
 SpgemmPlanView spgemm_plan_view(b200sp_spgemm_plan* p) {
-  return SpgemmPlanView{p->symbolic_done, p->m, p->n, p->k, p->c_nnz, p->c_max, p->flops, &p->bsp};
+  return SpgemmPlanView{p->symbolic_done, p->m, p->n, p->k, p->c_nnz, p->c_max, p->flops, &p->bsp, &p->s64};
 }
 
 static int bin_rows(cudaStream_t st, int m, const int* key, const BinSpec& spec, int* d_counts /*MAXBINS*/,
@@ -1221,6 +1222,10 @@ template <typename S>
 static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int k, const int* rpA, const int* ciA,
                         const S* vA, const int* rpB, const int* ciB, const S* vB, const int* rpC, int* ciC, S* vC) {
   B200SP_REQUIRE(p != nullptr, "spgemm_numeric: null plan");
+  if (spgemm64_holds_product(p->s64)) {
+    set_error("spgemm_numeric: the symbolic phase on this handle had 64-bit offsets; use the _i64 numeric");
+    return B200SP_ERR_STATE;
+  }
   if (!p->symbolic_done) {
     set_error("Call spgemm symbolic before spgemm numeric");
     return B200SP_ERR_STATE;
@@ -1357,6 +1362,10 @@ static int jacobi_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int
                        const S* vA, const int* rpB, const int* ciB, const S* vB, const int* rpC, int* ciC, S* vC, S omega,
                        const S* dinv) {
   B200SP_REQUIRE(p != nullptr, "spgemm_jacobi: null plan");
+  if (spgemm64_holds_product(p->s64)) {
+    set_error("spgemm_jacobi: not provided on 64-bit offsets (the symbolic phase on this handle had them)");
+    return B200SP_ERR_STATE;
+  }
   if (!p->symbolic_done) {
     set_error("KokkosSparse::spgemm_jacobi: must first call spgemm_symbolic with the same handle.");
     return B200SP_ERR_STATE;
@@ -1415,6 +1424,7 @@ int b200sp_spgemm_plan_create(b200sp_spgemm_plan** plan) {
 int b200sp_spgemm_plan_destroy(b200sp_spgemm_plan* p, void* stream) {
   if (!p) return B200SP_OK;
   spgemm_release(p, (cudaStream_t)stream);
+  spgemm64_state_free(p->s64, (cudaStream_t)stream);
   delete p;
   return B200SP_OK;
 }
@@ -1426,6 +1436,10 @@ int b200sp_spgemm_symbolic_i32(b200sp_spgemm_plan* p, void* stream, int m, int n
   B200SP_REQUIRE(m >= 0 && n >= 0 && k >= 0, "spgemm_symbolic: negative dimension");
   B200SP_REQUIRE(rpC != nullptr, "spgemm_symbolic: row_ptr_C is null");
   cudaStream_t st = (cudaStream_t)stream;
+  if (spgemm64_holds_product(p->s64)) {
+    set_error("spgemm_symbolic: handle was already used for a product with 64-bit offsets; create a new handle");
+    return B200SP_ERR_STATE;
+  }
   if (p->symbolic_done) {
     // one handle, one product (reference debug build throws std::invalid_argument, spgemm_handle.hpp:706-746)
     if (p->m != m || p->n != n || p->k != k || p->rpA != rpA || p->ciA != ciA || p->rpB != rpB || p->ciB != ciB) {

@@ -42,11 +42,26 @@ _ALGO_TO_C = {SPMV_DEFAULT: 0, SPMV_FAST_SETUP: 1, SPMV_NATIVE: 1, SPMV_MERGE_PA
 
 
 def _idx(t):
-    """Device pointer of a 32-bit index array: every entry point but spmv's 64-bit ones reads int32 ordinals and offsets."""
+    """Device pointer of a 32-bit index array: every entry point but spmv's and spgemm's 64-bit ones reads int32 ordinals and
+    offsets."""
     if t is not None and t.dtype != torch.int32:
         raise B200SparseError(f"b200sparse: this operation takes int32 row maps / entries, got {t.dtype} "
-                              "(only spmv accepts 64-bit offsets)")
+                              "(only spmv and spgemm accept 64-bit offsets)")
     return _ptr(t)
+
+
+def _spgemm_wide(row_maps, entries):
+    """True when a point SpGEMM runs on 64-bit offsets (spgemm64.cu): the row maps of A, B and C share one dtype, int32 or
+    int64, and the entries are int32 (the (int, size_t) instantiation; 64-bit ordinals are not provided)."""
+    dts = {t.dtype for t in row_maps if t is not None}
+    if len(dts) > 1:
+        raise B200SparseError(f"KokkosSparse::spgemm: the row maps of A, B and C must share one dtype, got {sorted(map(str, dts))}")
+    if dts - {torch.int32, torch.int64}:
+        raise B200SparseError(f"KokkosSparse::spgemm: row maps must be int32 or int64, got {dts.pop()}")
+    for t in entries:
+        if t is not None and t.dtype != torch.int32:
+            raise B200SparseError(f"KokkosSparse::spgemm: 64-bit ordinals are not provided (entries must be int32, got {t.dtype})")
+    return dts == {torch.int64}
 
 
 def _ptr(t):
@@ -61,7 +76,8 @@ class CrsMatrix:
     """graph.row_map / graph.entries / values / numCols (0-based CSR; rows need
     not be sorted, duplicates are legal for spmv).  Ordinal / offset types: (int32, int32) everywhere; spmv also takes 64-bit
     offsets -- row_map int64 with int32 or int64 entries, the (int64_t, size_t) instantiation of the reference's cuSPARSE slot
-    (sparse/tpls/KokkosSparse_spmv_tpl_spec_decl.hpp:246-257) -- for matrices past 2^31 entries."""
+    (sparse/tpls/KokkosSparse_spmv_tpl_spec_decl.hpp:246-257) -- for matrices past 2^31 entries, and spgemm takes row_map
+    int64 with int32 entries, Kokkos' (int, size_t), for products past 2^31 entries."""
 
     def __init__(self, row_map, entries, values, ncols):
         assert (row_map.dtype == torch.int32 and entries.dtype == torch.int32) or (
@@ -737,6 +753,15 @@ class SPGEMMHandle:
     def get_c_nnz(self): return self._c_nnz
     def get_max_result_nnz(self): return self._max_nnz
 
+    def set_window(self, max_entries):
+        """64-bit offsets only: products and entries of A per 32-bit window of the next symbolic (default 2^31 - 65537;
+        smaller values are for tests)."""
+        check(_lib.sparse().b200sp_spgemm_plan_set_window(self._plan, int(max_entries)))
+
+    def windows(self):
+        """Windows of the last symbolic on 64-bit offsets (0 otherwise)."""
+        return _lib.sparse().b200sp_spgemm_plan_windows(self._plan)
+
     def __del__(self):
         try:
             if self._plan:
@@ -851,10 +876,12 @@ def spgemm_symbolic_views(kh, m, n, k, row_mapA, entriesA, transposeA, row_mapB,
         raise B200SparseInvalidArgument("spgemm_symbolic: create_spgemm_handle() was not called")
     if row_mapC.numel() != m + 1:
         raise B200SparseError("spgemm_symbolic: row_mapC must have m+1 entries")
+    wide = _spgemm_wide((row_mapA, row_mapB, row_mapC), (entriesA, entriesB))
     c_nnz, c_max = C.c_int64(0), C.c_int(0)
-    check(_lib.sparse().b200sp_spgemm_symbolic_i32(
-        sh._plan, _stream(), m, n, k, _idx(row_mapA), _idx(entriesA), _idx(row_mapB), _idx(entriesB),
-        C.c_void_p(row_mapC.data_ptr()), C.byref(c_nnz), C.byref(c_max)))
+    fn = _lib.sparse().b200sp_spgemm_symbolic_i64 if wide else _lib.sparse().b200sp_spgemm_symbolic_i32
+    rp = _ptr if wide else _idx
+    check(fn(sh._plan, _stream(), m, n, k, rp(row_mapA), _idx(entriesA), rp(row_mapB), _idx(entriesB),
+             C.c_void_p(row_mapC.data_ptr()), C.byref(c_nnz), C.byref(c_max)))
     sh._c_nnz, sh._max_nnz = c_nnz.value, c_max.value
     sh._symbolic = True
     sh._rowptrs = True
@@ -875,10 +902,16 @@ def spgemm_numeric_views(kh, m, n, k, row_mapA, entriesA, valuesA, transposeA, r
         _bspgemm_numeric(sh, m, n, k, int(block_dim), row_mapA, entriesA, valuesA, row_mapB, entriesB, valuesB, row_mapC,
                          entriesC, valuesC)
         return
+    wide = _spgemm_wide((row_mapA, row_mapB, row_mapC), (entriesA, entriesB, entriesC))
     f64 = valuesA.dtype == torch.float64
-    fn = _lib.sparse().b200sp_spgemm_numeric_f64_i32 if f64 else _lib.sparse().b200sp_spgemm_numeric_f32_i32
-    check(fn(sh._plan, _stream(), m, n, k, _idx(row_mapA), _idx(entriesA), _ptr(valuesA), _idx(row_mapB),
-             _idx(entriesB), _ptr(valuesB), _idx(row_mapC), _idx(entriesC), _ptr(valuesC)))
+    L = _lib.sparse()
+    if wide:
+        fn = L.b200sp_spgemm_numeric_f64_i64 if f64 else L.b200sp_spgemm_numeric_f32_i64
+    else:
+        fn = L.b200sp_spgemm_numeric_f64_i32 if f64 else L.b200sp_spgemm_numeric_f32_i32
+    rp = _ptr if wide else _idx
+    check(fn(sh._plan, _stream(), m, n, k, rp(row_mapA), _idx(entriesA), _ptr(valuesA), rp(row_mapB),
+             _idx(entriesB), _ptr(valuesB), rp(row_mapC), _idx(entriesC), _ptr(valuesC)))
     sh._numeric = True
     sh._entries = True
 
@@ -888,7 +921,7 @@ def spgemm_symbolic(kh, A, Amode, B, Bmode, C_out=None):
     uninitialised, runs symbolic, sizes entries/values from get_c_nnz().  Returns C."""
     m, n, k = A.numRows(), A.numCols(), B.numCols()
     dev = A.row_map.device
-    row_mapC = torch.empty(m + 1, dtype=torch.int32, device=dev)
+    row_mapC = torch.empty(m + 1, dtype=A.row_map.dtype, device=dev)
     spgemm_symbolic_views(kh, m, n, k, A.row_map, A.entries, Amode, B.row_map, B.entries, Bmode, row_mapC)
     c_nnz = kh.get_spgemm_handle().get_c_nnz()
     entriesC = torch.empty(c_nnz, dtype=torch.int32, device=dev)
@@ -908,6 +941,8 @@ def spgemm_jacobi(kh, A, Amode, B, Bmode, Cm, omega, dinv):
     per row (the reference passes an m x 1 view)."""
     if Amode or Bmode:
         raise B200SparseError("KokkosSparse::spgemm_jacobi: transposing A or B is not supported")
+    if any(t.dtype == torch.int64 for t in (A.row_map, B.row_map, Cm.row_map)):
+        raise B200SparseError("KokkosSparse::spgemm_jacobi: not provided on 64-bit offsets (int32 row maps only)")
     sh = kh.get_spgemm_handle()
     if sh is None or not sh.is_symbolic_called():
         raise B200SparseError("KokkosSparse::spgemm_jacobi: must first call spgemm_symbolic with the same handle.")
