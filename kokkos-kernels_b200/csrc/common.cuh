@@ -8,6 +8,7 @@
 #endif
 #include <stdint.h>
 #include <stdio.h>
+#include <algorithm>
 #include <atomic>
 #include "../../include/b200sparse.h"
 
@@ -47,6 +48,11 @@ extern std::atomic<long long> g_launches;
   } while (0)
 
 int sm_count();  // SMs of the current device (cached per device)
+
+// CTAs of `per_block` threads for a grid-stride loop over `work` items: one item per thread, at most per_sm CTAs per SM
+inline int grid_for(int64_t work, int per_block = 256, int per_sm = 8) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((work + per_block - 1) / per_block, (int64_t)sm_count() * per_sm));
+}
 // Scratch is allocated with cudaMallocAsync.  The default pool hands unused memory back to the driver at every synchronisation
 // point (release threshold 0), and the symbolic phases synchronise by contract (they return counts to the host): each call would
 // then map its scratch again, which can cost more than its kernels (spadd_symbolic most of all).  Keeps the pool's memory (once per device); called by every scratch allocation scope (DevTmp) and by the plans that own

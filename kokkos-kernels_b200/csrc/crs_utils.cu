@@ -718,10 +718,6 @@ __global__ void __launch_bounds__(256)
     t_vals[j] = vals[t_src[j]];
 }
 
-static inline int grid_for(int64_t work, int per_block = 256, int mult = 8) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((work + per_block - 1) / per_block, (int64_t)sm_count() * mult));
-}
-
 // structure of the transpose + source entry of every transposed entry (t_src); nnz = row_ptr[m] (host value)
 int transpose_structure(cudaStream_t st, int m, int n, int64_t nnz, const int* rp, const int* ci, int* trp, int* tci,
                         int* t_src) {

@@ -232,8 +232,6 @@ void gs_release(b200sp_gs_plan* p, cudaStream_t st) {
   p->symbolic_done = p->numeric_done = false;
 }
 
-int blocks_for(int n) { return std::max(1, std::min((n + 255) / 256, sm_count() * 8)); }
-
 template <typename S>
 int gs_numeric_impl(b200sp_gs_plan* p, cudaStream_t st, int n, const int* rp, const int* ci, const S* v) {
   B200SP_REQUIRE(p != nullptr, "gauss_seidel_numeric: null plan");
@@ -257,7 +255,7 @@ int gs_numeric_impl(b200sp_gs_plan* p, cudaStream_t st, int n, const int* rp, co
   int* missing = nullptr;
   B200SP_CUDA_TRY(tmp.alloc(&missing, 1));
   B200SP_CUDA_TRY(cudaMemsetAsync(missing, 0, sizeof(int), st));
-  gs_inverse_diagonal_kernel<S><<<blocks_for(n), 256, 0, st>>>(n, rp, ci, v, (S*)p->dinv, missing);
+  gs_inverse_diagonal_kernel<S><<<grid_for(n), 256, 0, st>>>(n, rp, ci, v, (S*)p->dinv, missing);
   B200SP_LAUNCH_CHECK();
   int h_missing = 0;
   B200SP_CUDA_TRY(cudaMemcpyAsync(&h_missing, missing, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -379,7 +377,7 @@ int b200sp_gs_symbolic_nc_i32(b200sp_gs_plan* p, void* stream, int n, int ncols,
   B200SP_CUDA_TRY(cudaMemsetAsync(p->colors, 0xFF, sizeof(int) * (size_t)n, st));  // -1: uncoloured
   int* cur = p->colors;
   int* nxt = next;
-  const int grid = blocks_for(n);
+  const int grid = grid_for(n);
   for (int round = 0;; ++round) {
     B200SP_CUDA_TRY(cudaMemsetAsync(remaining, 0, sizeof(int), st));
     gs_color_round_kernel<<<grid, 256, 0, st>>>(n, row_ptr, col_idx, trp, tci, cur, nxt, remaining);

@@ -216,8 +216,6 @@ __global__ void __launch_bounds__(256) gs2_update_kernel(int n, const S* __restr
 }
 #undef GS2_ROWS
 
-inline int vec_blocks(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8)); }
-
 void release_parts(b200sp_gs2_plan* p, cudaStream_t st) {
   for (int q = 0; q < 4; ++q) {
     if (p->rp[q]) cudaFreeAsync(p->rp[q], st);
@@ -286,7 +284,7 @@ int numeric_impl(b200sp_gs2_plan* p, cudaStream_t st, int n, int ncols, const in
   }
   if (n > 0) {
     B200SP_REQUIRE(vals != nullptr, "gs2_numeric: null values");
-    gs2_values_kernel<S><<<vec_blocks(n), 256, 0, st>>>(n, row_ptr, col_idx, vals, given_dinv, p->rp[kL], (S*)p->v[kL], p->rp[kU], (S*)p->v[kU],
+    gs2_values_kernel<S><<<grid_for(n), 256, 0, st>>>(n, row_ptr, col_idx, vals, given_dinv, p->rp[kL], (S*)p->v[kL], p->rp[kU], (S*)p->v[kU],
                                                          p->rp[kLa], (S*)p->v[kLa], p->rp[kUa], (S*)p->v[kUa], (S*)p->D, (S*)p->Da,
                                                          p->compact ? 1 : 0);
     B200SP_LAUNCH_CHECK();
@@ -331,7 +329,7 @@ int apply_impl(b200sp_gs2_plan* p, void* stream, int n, int ncols, const int* ro
   }
   S *R = (S*)p->R, *T = (S*)p->T, *Z = (S*)p->Z;
   const S *D = (const S*)p->D, *Da = (const S*)p->Da;
-  const dim3 nb((unsigned)vec_blocks(n), (unsigned)k);  // blockIdx.y = right-hand side
+  const dim3 nb((unsigned)grid_for(n), (unsigned)k);  // blockIdx.y = right-hand side
   if (k == 1) {
     ldx = ncols;
     ldb = n;
@@ -479,7 +477,7 @@ int b200sp_gs2_symbolic_i32(b200sp_gs2_plan* p, void* stream, int n, int ncols, 
   B200SP_CUDA_TRY(tmp.alloc(&bsum, (size_t)scan_blocks(n)));
   B200SP_CUDA_TRY(tmp.alloc(&dtotal, 4));
   B200SP_CUDA_TRY(cudaMemsetAsync(nodiag, 0x7F, sizeof(int), st));
-  gs2_count_kernel<<<vec_blocks(n), 256, 0, st>>>(n, row_ptr, col_idx, cnt[0], cnt[1], cnt[2], cnt[3], compact ? 1 : 0, nodiag);
+  gs2_count_kernel<<<grid_for(n), 256, 0, st>>>(n, row_ptr, col_idx, cnt[0], cnt[1], cnt[2], cnt[3], compact ? 1 : 0, nodiag);
   B200SP_LAUNCH_CHECK();
   for (int q = 0; q < parts; ++q) {
     B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->rp[q], sizeof(int) * ((size_t)n + 4), st));
@@ -502,7 +500,7 @@ int b200sp_gs2_symbolic_i32(b200sp_gs2_plan* p, void* stream, int n, int ncols, 
     p->cnt[q] = h_total[q];
     B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->ci[q], sizeof(int) * (size_t)std::max<int64_t>(p->cnt[q], 1), st));
   }
-  gs2_entries_kernel<<<vec_blocks(n), 256, 0, st>>>(n, row_ptr, col_idx, p->rp[kL], p->ci[kL], p->rp[kU], p->ci[kU], p->rp[kLa], p->ci[kLa],
+  gs2_entries_kernel<<<grid_for(n), 256, 0, st>>>(n, row_ptr, col_idx, p->rp[kL], p->ci[kL], p->rp[kU], p->ci[kU], p->rp[kLa], p->ci[kLa],
                                                     p->rp[kUa], p->ci[kUa], compact ? 1 : 0);
   B200SP_LAUNCH_CHECK();
   if (!p->two_stage) {  // classic form: level sets of the lower and the upper triangle of A (sptrsv_symbolic, :685-697)

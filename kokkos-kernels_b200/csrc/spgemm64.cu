@@ -6,7 +6,8 @@
 // runs them on the native KokkosSPGEMM.
 //
 // C is the array that outgrows int32 first.  Every row of C is computed on its own, so the rows can be cut into windows
-// that each fit 32-bit offsets and run through the 32-bit entry points (spgemm.cu), as spmv64.cu does for SpMV:
+// that each fit 32-bit offsets and run through the 32-bit entry points (spgemm.cu), on the row windows of spmv64.cu
+// (windows64.cuh):
 //   * B's row map is narrowed to int32 once (nnz(B) must stay within 2^31 - 65537: every window reads all of B);
 //   * per row of A: its entries and its products sum_{j in A_i} len(B_{col_j}), scanned into int64 prefixes;
 //   * windows of consecutive rows with at most `limit` products and at most `limit` entries of A -- the products bound
@@ -24,45 +25,25 @@
 #include "common.cuh"
 #include "scan.cuh"
 #include "bspgemm.cuh"
-
-namespace {
-constexpr int kMaxWindows = 4096;
-constexpr int64_t kDefaultWindow = (int64_t)INT32_MAX - 65536;  // products / entries per window, as spmv64.cu
-
-struct Window {
-  int r0 = 0, r1 = 0;      // rows [r0, r1)
-  int64_t a_base = 0;      // row_ptr_A[r0]
-  int64_t c_base = 0;      // row_ptr_C[r0]
-  int64_t c_nnz = 0;       // entries of C in the window
-  int64_t rel_off = 0;     // offset of the window's relative row maps (r1 - r0 + 1 entries) in rel_a / rel_c
-  b200sp_spgemm_plan* plan = nullptr;
-};
-}  // namespace
+#include "windows64.cuh"
 
 namespace b200sp {
 
 struct Spgemm64State {
-  int64_t window = kDefaultWindow;
+  int64_t window = kDefaultWindow;  // products / entries of A per window
   bool done = false;  // a 64-bit symbolic completed on this plan
   int m = 0, n = 0, k = 0;
   const void *rpA = nullptr, *ciA = nullptr, *rpB = nullptr, *ciB = nullptr;
   int64_t c_nnz = 0;
   int c_max = 0;
-  std::vector<Window> win;
-  int* rel_a = nullptr;  // device: relative row maps of A, all windows (4 B per row)
-  int* rel_c = nullptr;  // device: relative row maps of C, all windows (4 B per row)
+  RowWindows cut;                           // windows of A's rows, bases not rounded; cut.rel: relative row maps of A
+  std::vector<int64_t> c_base;              // per window: row_ptr_C[r0]
+  std::vector<b200sp_spgemm_plan*> plans;   // per window: the 32-bit product
+  int* rel_c = nullptr;  // device: relative row maps of C, laid out as cut.rel (4 B per row)
   int* rp_b = nullptr;   // device: B's row map narrowed to int32 (4 B per row)
 };
 
 namespace {
-
-__global__ void __launch_bounds__(256) s64g_fill_kernel(int64_t n, int64_t* __restrict__ p) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = 0;
-}
-
-__global__ void __launch_bounds__(256) s64g_narrow_kernel(int64_t n, const int64_t* __restrict__ in, int* __restrict__ out) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = (int)in[i];
-}
 
 // products per row of A, 8 lanes per row; a row past INT_MAX products is clamped (it exceeds every window limit)
 __global__ void __launch_bounds__(256) s64g_products_kernel(int m, const int64_t* __restrict__ rpA, const int* __restrict__ ciA,
@@ -80,64 +61,15 @@ __global__ void __launch_bounds__(256) s64g_products_kernel(int m, const int64_t
   if (r < m && sl == 0) prod[r] = (int)min(f, (long long)INT_MAX);
 }
 
-// One thread, one binary search per window over the prefixes P (products) and rpA (entries): window k starts at row R_k
-// and ends at the largest R' with P[R'] - P[R_k] <= limit and rpA[R'] - rpA[R_k] <= limit.  out[3k .. 3k+2] = (R_k,
-// R_{k+1}, rpA[R_k]); *n_out = windows, -1 when one row alone exceeds the limit (out[0] = that row), -2 when there are more
-// than max_windows.
-__global__ void s64g_windows_kernel(int64_t m, const int64_t* __restrict__ P, const int64_t* __restrict__ rpA, int64_t limit,
-                                    int max_windows, int64_t* __restrict__ out, int* __restrict__ n_out) {
-  if (blockIdx.x != 0 || threadIdx.x != 0) return;
-  int k = 0;
-  int64_t R = 0;
-  while (R < m) {
-    const int64_t ptop = P[R] + limit, atop = rpA[R] + limit;
-    int64_t lo = R, hi = m;
-    while (lo < hi) {
-      const int64_t mid = lo + ((hi - lo + 1) >> 1);
-      if (P[mid] <= ptop && rpA[mid] <= atop) lo = mid;
-      else hi = mid - 1;
-    }
-    if (lo == R) {
-      *n_out = -1;
-      out[0] = R;
-      return;
-    }
-    if (k == max_windows) {
-      *n_out = -2;
-      return;
-    }
-    out[3 * k] = R;
-    out[3 * k + 1] = lo;
-    out[3 * k + 2] = rpA[R];
-    ++k;
-    R = lo;
-  }
-  *n_out = k;
-}
-
-__global__ void __launch_bounds__(256) s64g_relative_kernel(int64_t r0, int64_t count, int64_t base, const int64_t* __restrict__ rp,
-                                                            int* __restrict__ rel) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-    rel[i] = (int)(rp[r0 + i] - base);
-}
-
-__global__ void __launch_bounds__(256) s64g_widen_kernel(int64_t r0, int64_t count, int64_t base, const int* __restrict__ rel,
-                                                         int64_t* __restrict__ rp) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-    rp[r0 + i] = base + rel[i];
-}
-
-inline int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8)); }
-
 // frees the windows, their child plans and the narrowed arrays; keeps the window limit
 void release_windows(Spgemm64State* s, cudaStream_t st) {
-  for (Window& w : s->win)
-    if (w.plan) b200sp_spgemm_plan_destroy(w.plan, (void*)st);
-  s->win.clear();
-  void* ptrs[] = {s->rel_a, s->rel_c, s->rp_b};
-  for (void* q : ptrs)
+  for (b200sp_spgemm_plan* pl : s->plans) b200sp_spgemm_plan_destroy(pl, (void*)st);
+  s->plans.clear();
+  s->c_base.clear();
+  s->cut.release(st);
+  for (int* q : {s->rel_c, s->rp_b})
     if (q) cudaFreeAsync(q, st);
-  s->rel_a = s->rel_c = s->rp_b = nullptr;
+  s->rel_c = s->rp_b = nullptr;
   s->done = false;
   s->c_nnz = 0;
   s->c_max = 0;
@@ -185,8 +117,7 @@ int symbolic64(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int k, cons
   }
   // degenerate shapes: zero row_ptr, c_nnz = 0, no windows (symbolic_spec.hpp:101-107)
   if (m == 0 || n == 0 || k == 0 || nnzA == 0 || nnzB == 0) {
-    s64g_fill_kernel<<<grid_for((int64_t)m + 1), 256, 0, st>>>((int64_t)m + 1, rpC);
-    B200SP_LAUNCH_CHECK();
+    B200SP_CUDA_TRY(cudaMemsetAsync(rpC, 0, sizeof(int64_t) * ((size_t)m + 1), st));
     B200SP_CUDA_TRY(cudaStreamSynchronize(st));
     s->done = true;
     if (c_nnz) *c_nnz = 0;
@@ -202,8 +133,8 @@ int symbolic64(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int k, cons
   B200SP_REQUIRE(ciA && ciB, "spgemm_symbolic: null column index array");
 
   DevTmp tmp(st);
-  int *prod, *block_max, *d_max, *d_n;
-  int64_t *P, *d_win;
+  int *prod, *block_max, *d_max;
+  int64_t* P;
   long long *block_sum, *d_total;
   const int nblocks = scan_blocks(m);
   B200SP_CUDA_TRY(tmp.alloc(&prod, m));
@@ -212,64 +143,41 @@ int symbolic64(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int k, cons
   B200SP_CUDA_TRY(tmp.alloc(&block_max, nblocks));
   B200SP_CUDA_TRY(tmp.alloc(&d_total, 1));
   B200SP_CUDA_TRY(tmp.alloc(&d_max, 1));
-  B200SP_CUDA_TRY(tmp.alloc(&d_win, (size_t)3 * kMaxWindows));
-  B200SP_CUDA_TRY(tmp.alloc(&d_n, 1));
   B200SP_CUDA_TRY(cudaMallocAsync((void**)&s->rp_b, sizeof(int) * ((size_t)n + 1), st));
-  s64g_narrow_kernel<<<grid_for((int64_t)n + 1), 256, 0, st>>>((int64_t)n + 1, rpB, s->rp_b);
+  win64_narrow_kernel<<<grid_for((int64_t)n + 1), 256, 0, st>>>((int64_t)n + 1, rpB, s->rp_b, nullptr);
   B200SP_LAUNCH_CHECK();
   s64g_products_kernel<<<(unsigned)(((int64_t)m * 8 + 255) / 256), 256, 0, st>>>(m, rpA, ciA, s->rp_b, prod);
   B200SP_LAUNCH_CHECK();
   if (int rc = launch_exclusive_scan64<int>(st, m, prod, P, block_sum, block_max, d_total, d_max)) return rc;
-  s64g_windows_kernel<<<1, 32, 0, st>>>(m, P, rpA, s->window, kMaxWindows, d_win, d_n);
-  B200SP_LAUNCH_CHECK();
-  int nw = 0;
-  B200SP_CUDA_TRY(cudaMemcpyAsync(&nw, d_n, sizeof(int), cudaMemcpyDeviceToHost, st));
-  B200SP_CUDA_TRY(cudaStreamSynchronize(st));
-  if (nw == -1) {
-    int64_t row = 0;
-    B200SP_CUDA_TRY(cudaMemcpyAsync(&row, d_win, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    B200SP_CUDA_TRY(cudaStreamSynchronize(st));
+  int64_t row = 0;
+  const int rc = cut_windows(st, m, rpA, P, s->window, 1, &s->cut, &row);
+  if (rc == kWindowRowOverLimit) {
     release_windows(s, st);
     set_error("spgemm_symbolic (64-bit offsets): row %lld holds more than %lld entries or products (window limit)",
               (long long)row, (long long)s->window);
     return B200SP_ERR_OVERFLOW;
   }
-  if (nw == -2) {
+  if (rc == kWindowsOverCap) {
     release_windows(s, st);
     set_error("spgemm_symbolic (64-bit offsets): more than %d windows of %lld products", kMaxWindows, (long long)s->window);
     return B200SP_ERR_OVERFLOW;
   }
-  std::vector<int64_t> h_win((size_t)3 * nw);
-  B200SP_CUDA_TRY(cudaMemcpyAsync(h_win.data(), d_win, sizeof(int64_t) * 3 * (size_t)nw, cudaMemcpyDeviceToHost, st));
-  B200SP_CUDA_TRY(cudaStreamSynchronize(st));
-  s->win.resize((size_t)nw);
-  int64_t total = 0;
-  for (int w = 0; w < nw; ++w) {
-    Window& x = s->win[(size_t)w];
-    x.r0 = (int)h_win[3 * (size_t)w];
-    x.r1 = (int)h_win[3 * (size_t)w + 1];
-    x.a_base = h_win[3 * (size_t)w + 2];
-    x.rel_off = total;
-    total += (int64_t)(x.r1 - x.r0) + 1;
-  }
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&s->rel_a, sizeof(int) * (size_t)total, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&s->rel_c, sizeof(int) * (size_t)total, st));
+  if (rc) return rc;
+  B200SP_CUDA_TRY(cudaMallocAsync((void**)&s->rel_c, sizeof(int) * (size_t)s->cut.rel_size, st));
   int64_t c_base = 0;
   int c_max = 0;
-  for (Window& x : s->win) {
+  for (const RowWindow& x : s->cut.win) {
     const int wm = x.r1 - x.r0;
     const int64_t count = (int64_t)wm + 1;
-    s64g_relative_kernel<<<grid_for(count), 256, 0, st>>>(x.r0, count, x.a_base, rpA, s->rel_a + x.rel_off);
-    B200SP_LAUNCH_CHECK();
-    if (int rc = b200sp_spgemm_plan_create(&x.plan)) return rc;
+    s->plans.push_back(nullptr);
+    if (int rc = b200sp_spgemm_plan_create(&s->plans.back())) return rc;
     int64_t w_nnz = 0;
     int w_max = 0;
-    if (int rc = b200sp_spgemm_symbolic_i32(x.plan, (void*)st, wm, n, k, s->rel_a + x.rel_off, ciA + x.a_base, s->rp_b, ciB,
-                                            s->rel_c + x.rel_off, &w_nnz, &w_max))
+    if (int rc = b200sp_spgemm_symbolic_i32(s->plans.back(), (void*)st, wm, n, k, s->cut.rel + x.rel_off, ciA + x.base, s->rp_b,
+                                            ciB, s->rel_c + x.rel_off, &w_nnz, &w_max))
       return rc;
-    x.c_base = c_base;
-    x.c_nnz = w_nnz;
-    s64g_widen_kernel<<<grid_for(count), 256, 0, st>>>(x.r0, count, c_base, s->rel_c + x.rel_off, rpC);
+    s->c_base.push_back(c_base);
+    win64_widen_kernel<<<grid_for(count), 256, 0, st>>>(x.r0, count, c_base, s->rel_c + x.rel_off, rpC);
     B200SP_LAUNCH_CHECK();
     c_base += w_nnz;
     c_max = std::max(c_max, w_max);
@@ -310,9 +218,10 @@ int numeric64(b200sp_spgemm_plan* p, void* stream, int m, int n, int k, const in
   if (m == 0 || s->c_nnz == 0) return B200SP_OK;
   B200SP_REQUIRE(rpA && ciA && vA && rpB && ciB && vB && rpC && ciC && vC, "spgemm_numeric: null pointer argument");
   // the windows' relative row maps stand for rpA / rpB / rpC, which symbolic has read
-  for (const Window& x : s->win) {
-    if (int rc = call32(x.plan, stream, x.r1 - x.r0, n, k, s->rel_a + x.rel_off, ciA + x.a_base, vA + x.a_base, s->rp_b, ciB, vB,
-                        s->rel_c + x.rel_off, ciC + x.c_base, vC + x.c_base))
+  for (size_t w = 0; w < s->cut.win.size(); ++w) {
+    const RowWindow& x = s->cut.win[w];
+    if (int rc = call32(s->plans[w], stream, x.r1 - x.r0, n, k, s->cut.rel + x.rel_off, ciA + x.base, vA + x.base, s->rp_b, ciB,
+                        vB, s->rel_c + x.rel_off, ciC + s->c_base[w], vC + s->c_base[w]))
       return rc;
   }
   return B200SP_OK;
@@ -334,8 +243,7 @@ extern "C" {
 
 int b200sp_spgemm_plan_set_window(b200sp_spgemm_plan* plan, int64_t max_entries) {
   B200SP_REQUIRE(plan != nullptr, "spgemm_plan_set_window: null plan");
-  B200SP_REQUIRE(max_entries >= 8 && max_entries <= kDefaultWindow, "spgemm_plan_set_window: %lld not in [8, %lld]",
-                 (long long)max_entries, (long long)kDefaultWindow);
+  if (int rc = b200sp::check_window_limit("spgemm_plan_set_window", max_entries)) return rc;
   b200sp::Spgemm64State* s = b200sp::state_of(plan, true);
   if (!s) {
     b200sp::set_error("spgemm_plan_set_window: out of host memory");
@@ -348,7 +256,7 @@ int b200sp_spgemm_plan_set_window(b200sp_spgemm_plan* plan, int64_t max_entries)
 int b200sp_spgemm_plan_windows(const b200sp_spgemm_plan* plan) {
   if (!plan) return 0;
   const b200sp::Spgemm64State* s = b200sp::state_of(const_cast<b200sp_spgemm_plan*>(plan), false);
-  return s ? (int)s->win.size() : 0;
+  return s ? (int)s->cut.win.size() : 0;
 }
 
 int b200sp_spgemm_symbolic_i64(b200sp_spgemm_plan* plan, void* stream, int m, int n, int k, const int64_t* row_ptr_A,

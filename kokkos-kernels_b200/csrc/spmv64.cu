@@ -8,7 +8,7 @@
 // 180 GB of HBM3e hold about 15e9 fp64 entries with 32-bit columns: seven times what an int32 row map addresses.  A kernel
 // that streamed the caller's 64-bit arrays would move 16 B per entry (8 B value + 8 B column) against the 12 B of the
 // 32-bit path, i.e. run at 3/4 of its speed on an HBM-bound product.  So the 64-bit structure is read ONCE, at analysis:
-//   * the rows are cut into windows of consecutive rows holding < 2^31 entries each;
+//   * the rows are cut into windows of consecutive rows holding < 2^31 entries each (windows64.cuh);
 //   * per window the plan keeps a 32-bit row map RELATIVE to the window's first (4-aligned) entry   -- 4 B per row;
 //   * 64-bit columns are narrowed to 32 bits (the matrix must have < 2^31 columns)                  -- 4 B per entry,
 //     32-bit columns are used where they lie (nothing copied);
@@ -16,37 +16,24 @@
 //     scatter kernel for the transposed modes) per window, on `values + base` and `columns + base`.
 // Traffic per product: 12 B per entry (fp64), as for a 32-bit matrix; the results are those of the 32-bit path on each
 // window, i.e. bit-identical to it on any matrix both can take.
-#include <algorithm>
 #include <cstdlib>
 #include <new>
 #include <vector>
 
 #include "common.cuh"
-
-namespace {
-constexpr int kMaxWindows = 4096;
-constexpr int64_t kDefaultWindow = (int64_t)INT32_MAX - 65536;  // entries per window, room for the kernels' round-ups
-
-struct Window {
-  int r0 = 0, r1 = 0;  // rows [r0, r1)
-  int64_t base = 0;    // first entry the window's pointers are shifted by (multiple of 4: 16-byte aligned bulk copies)
-  int64_t end = 0;     // row_ptr[r1]
-  int64_t rel_off = 0; // offset of the window's relative row map inside plan->rel (multiple of 4)
-  b200sp_spmv_plan* plan = nullptr;
-};
-}  // namespace
+#include "windows64.cuh"
 
 struct b200sp_spmv64_plan {
   int algo = 0;
-  int64_t window_nnz = kDefaultWindow;
+  int64_t window_nnz = b200sp::kDefaultWindow;
   // key of the analysed matrix
   const void* key_rp = nullptr;
   const void* key_ci = nullptr;
   int64_t key_m = -1, key_n = -1, key_nnz = -1;
   int key_bits = 0;
-  // analysis products
-  std::vector<Window> win;
-  int* rel = nullptr;    // device: relative row maps of all windows
+  // analysis products: windows based on multiples of 4 entries (16-byte aligned bulk copies), one plan per window
+  b200sp::RowWindows cut;
+  std::vector<b200sp_spmv_plan*> plans;
   int* col32 = nullptr;  // device: narrowed columns (64-bit input only)
   char last_kernel[128] = "none";
 };
@@ -55,66 +42,11 @@ namespace b200sp {
 int spmv_lanes_per_row(int64_t m, int64_t nnz);  // spmv.cu
 namespace {
 
-// One thread walks the row map: window k starts at row R_k, base_k = row_ptr[R_k] & ~3, and ends before the first row that
-// would push it past `limit` entries.  out[4k .. 4k+3] = (R_k, R_{k+1}, base_k, row_ptr[R_{k+1}]); *n_out = windows, or -1 when one row alone
-// exceeds the limit, -2 when there are more than max_windows.
-__global__ void s64_windows_kernel(int64_t m, const int64_t* __restrict__ rp, int64_t limit, int max_windows,
-                                   int64_t* __restrict__ out, int* __restrict__ n_out) {
-  if (blockIdx.x != 0 || threadIdx.x != 0) return;
-  int k = 0;
-  int64_t R = 0;
-  while (R < m) {
-    const int64_t base = rp[R] & ~(int64_t)3;
-    const int64_t top = base + limit;
-    // largest R2 in (R, m] with rp[R2] <= top
-    int64_t lo = R, hi = m;  // rp[lo] <= top always (rp[R] - base <= 3 <= limit)
-    while (lo < hi) {
-      const int64_t mid = lo + ((hi - lo + 1) >> 1);
-      if (rp[mid] <= top) lo = mid;
-      else hi = mid - 1;
-    }
-    if (lo == R) {
-      *n_out = -1;
-      return;
-    }
-    if (k == max_windows) {
-      *n_out = -2;
-      return;
-    }
-    out[4 * k] = R;
-    out[4 * k + 1] = lo;
-    out[4 * k + 2] = base;
-    out[4 * k + 3] = rp[lo];
-    ++k;
-    R = lo;
-  }
-  *n_out = k;
-}
-
-__global__ void __launch_bounds__(256) s64_relative_kernel(int64_t r0, int64_t count, int64_t base, const int64_t* __restrict__ rp,
-                                                           int* __restrict__ rel) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-    rel[i] = (int)(rp[r0 + i] - base);
-}
-
-__global__ void __launch_bounds__(256) s64_narrow_kernel(int64_t nnz, const int64_t* __restrict__ ci, int* __restrict__ out,
-                                                         int* __restrict__ bad) {
-  bool any = false;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nnz; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t c = ci[i];
-    any |= (c < 0 || c > (int64_t)INT32_MAX);
-    out[i] = (int)c;
-  }
-  if (any) *bad = 1;
-}
-
 void release(b200sp_spmv64_plan* p, cudaStream_t st) {
-  for (Window& w : p->win)
-    if (w.plan) b200sp_spmv_plan_destroy(w.plan, (void*)st);
-  p->win.clear();
-  if (p->rel) cudaFreeAsync(p->rel, st);
+  for (b200sp_spmv_plan* pl : p->plans) b200sp_spmv_plan_destroy(pl, (void*)st);
+  p->plans.clear();
+  p->cut.release(st);
   if (p->col32) cudaFreeAsync(p->col32, st);
-  p->rel = nullptr;
   p->col32 = nullptr;
   p->key_rp = nullptr;
 }
@@ -125,69 +57,40 @@ int analyse(b200sp_spmv64_plan* p, cudaStream_t st, int64_t m, int64_t n, int64_
       p->key_bits == col_bits)
     return B200SP_OK;
   release(p, st);
-  DevTmp tmp(st);
-  int64_t* d_win = nullptr;
-  int* d_n = nullptr;
-  B200SP_CUDA_TRY(tmp.alloc(&d_win, (size_t)4 * kMaxWindows));
-  B200SP_CUDA_TRY(tmp.alloc(&d_n, 2));
-  B200SP_CUDA_TRY(cudaMemsetAsync(d_n, 0, 2 * sizeof(int), st));
-  s64_windows_kernel<<<1, 32, 0, st>>>(m, row_ptr, p->window_nnz, kMaxWindows, d_win, d_n);
-  B200SP_LAUNCH_CHECK();
-  if (col_bits == 64) {
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->col32, sizeof(int) * (size_t)std::max<int64_t>(nnz, 1), st));
-    const int64_t want = (nnz + 255) / 256;
-    const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>(want, (int64_t)sm_count() * 16));
-    s64_narrow_kernel<<<blocks, 256, 0, st>>>(nnz, (const int64_t*)col_idx, p->col32, d_n + 1);
-    B200SP_LAUNCH_CHECK();
-  }
-  int h_n[2] = {0, 0};
-  B200SP_CUDA_TRY(cudaMemcpyAsync(h_n, d_n, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-  B200SP_CUDA_TRY(cudaStreamSynchronize(st));
-  if (h_n[0] == -1) {
-    release(p, st);
+  int64_t row = 0;
+  int rc = cut_windows(st, m, row_ptr, nullptr, p->window_nnz, 4, &p->cut, &row);
+  if (rc == kWindowRowOverLimit) {
     set_error("spmv (64-bit offsets): a row holds more than %lld entries (window limit)", (long long)p->window_nnz);
     return B200SP_ERR_OVERFLOW;
   }
-  if (h_n[0] == -2) {
-    release(p, st);
+  if (rc == kWindowsOverCap) {
     set_error("spmv (64-bit offsets): more than %d windows of %lld entries", kMaxWindows, (long long)p->window_nnz);
     return B200SP_ERR_OVERFLOW;
   }
-  if (h_n[1] != 0) {
-    release(p, st);
-    set_error("spmv (64-bit columns): a column index does not fit 31 bits");
-    return B200SP_ERR_OVERFLOW;
-  }
-  const int nw = h_n[0];
-  std::vector<int64_t> h_win((size_t)4 * std::max(nw, 1));
-  if (nw > 0) {
-    B200SP_CUDA_TRY(cudaMemcpyAsync(h_win.data(), d_win, sizeof(int64_t) * 4 * (size_t)nw, cudaMemcpyDeviceToHost, st));
-    B200SP_CUDA_TRY(cudaStreamSynchronize(st));
-  }
-  p->win.resize((size_t)nw);
-  int64_t total = 0;
-  for (int k = 0; k < nw; ++k) {
-    Window& w = p->win[(size_t)k];
-    w.r0 = (int)h_win[4 * (size_t)k];
-    w.r1 = (int)h_win[4 * (size_t)k + 1];
-    w.base = h_win[4 * (size_t)k + 2];
-    w.end = h_win[4 * (size_t)k + 3];
-    w.rel_off = total;
-    total += (((int64_t)(w.r1 - w.r0) + 1) + 3) & ~(int64_t)3;
-  }
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->rel, sizeof(int) * (size_t)std::max<int64_t>(total, 4), st));
-  for (int k = 0; k < nw; ++k) {
-    Window& w = p->win[(size_t)k];
-    const int64_t count = (int64_t)(w.r1 - w.r0) + 1;
-    const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>((count + 255) / 256, (int64_t)sm_count() * 8));
-    s64_relative_kernel<<<blocks, 256, 0, st>>>(w.r0, count, w.base, row_ptr, p->rel + w.rel_off);
+  if (rc) return rc;
+  if (col_bits == 64) {
+    DevTmp tmp(st);
+    int* d_bad = nullptr;
+    int bad = 0;
+    B200SP_CUDA_TRY(tmp.alloc(&d_bad, 1));
+    B200SP_CUDA_TRY(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
+    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->col32, sizeof(int) * (size_t)std::max<int64_t>(nnz, 1), st));
+    win64_narrow_kernel<<<grid_for(nnz, 256, 16), 256, 0, st>>>(nnz, (const int64_t*)col_idx, p->col32, d_bad);
     B200SP_LAUNCH_CHECK();
-    int rc = b200sp_spmv_plan_create(&w.plan, p->algo);
-    if (rc) return rc;
+    B200SP_CUDA_TRY(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    B200SP_CUDA_TRY(cudaStreamSynchronize(st));
+    if (bad) {
+      release(p, st);
+      set_error("spmv (64-bit columns): a column index does not fit 31 bits");
+      return B200SP_ERR_OVERFLOW;
+    }
+  }
+  p->plans.assign(p->cut.win.size(), nullptr);
+  for (b200sp_spmv_plan*& pl : p->plans) {
+    if ((rc = b200sp_spmv_plan_create(&pl, p->algo))) return rc;
     // lanes per row chosen once from the WHOLE matrix: the summation order of a row, hence the result, does not depend
     // on where the windows fall, and equals the 32-bit entry points' on a matrix both can take
-    rc = b200sp_spmv_plan_tune(w.plan, -1, spmv_lanes_per_row(m, nnz), -1);
-    if (rc) return rc;
+    if ((rc = b200sp_spmv_plan_tune(pl, -1, spmv_lanes_per_row(m, nnz), -1))) return rc;
   }
   p->key_rp = row_ptr;
   p->key_ci = col_idx;
@@ -251,22 +154,23 @@ int spmv64_impl(b200sp_spmv64_plan* p, void* stream, char mode, int64_t m, int64
   const int* cols = col_bits == 64 ? p->col32 : (const int*)col_idx;
   // row r of X / Y starts r*ld elements in when the rows are contiguous (LayoutRight), r elements in otherwise
   const int64_t xstep = mv ? (xrm ? ldx : 1) : 1, ystep = mv ? (yrm ? ldy : 1) : 1;
-  bool first = true;
-  for (Window& w : p->win) {
+  const size_t nw = p->cut.win.size();
+  for (size_t i = 0; i < nw; ++i) {
+    const RowWindow& w = p->cut.win[i];
     const int wm = w.r1 - w.r0;
     const int64_t w_nnz = w.end - w.base;  // the window's entries counted from its base = its relative row map's last value
-    const int* rp = p->rel + w.rel_off;
+    const int* rp = p->cut.rel + w.rel_off;
     const S* xw = trans ? x + w.r0 * xstep : x;  // T / H: the window's rows of x, all of y (accumulated window by window)
     S* yw = trans ? y : y + w.r0 * ystep;        // N / C: all of x, the window's rows of y
-    const S bw = (trans && !first) ? S(1) : beta;
+    const S bw = (trans && i > 0) ? S(1) : beta;
     const char md = trans ? 'T' : 'N';
-    if (mv) rc = call32mm(w.plan, stream, md, wm, (int)n, w_nnz, k, alpha, rp, cols + w.base, vals + w.base, xw, ldx, xrm, bw, yw, ldy, yrm);
-    else rc = call32(w.plan, stream, md, wm, (int)n, w_nnz, alpha, rp, cols + w.base, vals + w.base, xw, bw, yw);
+    b200sp_spmv_plan* pl = p->plans[i];
+    if (mv) rc = call32mm(pl, stream, md, wm, (int)n, w_nnz, k, alpha, rp, cols + w.base, vals + w.base, xw, ldx, xrm, bw, yw, ldy, yrm);
+    else rc = call32(pl, stream, md, wm, (int)n, w_nnz, alpha, rp, cols + w.base, vals + w.base, xw, bw, yw);
     if (rc) return rc;
-    first = false;
   }
-  snprintf(p->last_kernel, sizeof(p->last_kernel), "%d window%s x %.90s", (int)p->win.size(), p->win.size() == 1 ? "" : "s",
-           p->win.empty() ? "none" : b200sp_spmv_last_kernel(p->win[0].plan));
+  snprintf(p->last_kernel, sizeof(p->last_kernel), "%d window%s x %.90s", (int)nw, nw == 1 ? "" : "s",
+           nw == 0 ? "none" : b200sp_spmv_last_kernel(p->plans[0]));
   return B200SP_OK;
 }
 
@@ -297,14 +201,13 @@ int b200sp_spmv64_plan_destroy(b200sp_spmv64_plan* p, void* stream) {
 
 int b200sp_spmv64_plan_set_window(b200sp_spmv64_plan* p, int64_t max_entries) {
   B200SP_REQUIRE(p != nullptr, "spmv64_plan_set_window: null plan");
-  B200SP_REQUIRE(max_entries >= 8 && max_entries <= kDefaultWindow, "spmv64_plan_set_window: %lld not in [8, %lld]",
-                 (long long)max_entries, (long long)kDefaultWindow);
+  if (int rc = b200sp::check_window_limit("spmv64_plan_set_window", max_entries)) return rc;
   p->window_nnz = max_entries;
   p->key_rp = nullptr;  // next call analyses again
   return B200SP_OK;
 }
 
-int b200sp_spmv64_plan_windows(const b200sp_spmv64_plan* p) { return p ? (int)p->win.size() : 0; }
+int b200sp_spmv64_plan_windows(const b200sp_spmv64_plan* p) { return p ? (int)p->cut.win.size() : 0; }
 const char* b200sp_spmv64_last_kernel(const b200sp_spmv64_plan* p) { return p ? p->last_kernel : "none"; }
 
 int b200sp_spmv_f64_i64(b200sp_spmv64_plan* plan, void* stream, char mode, int64_t m, int64_t n, int64_t nnz, double alpha,

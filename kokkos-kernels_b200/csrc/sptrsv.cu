@@ -60,8 +60,6 @@ inline bool tr_chain_enabled() {
   return !(e && e[0] == '0');
 }
 
-inline int tr_blocks(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 8)); }
-
 // one relaxation sweep: rows whose dependencies all had a level BEFORE this sweep get theirs; counts the rows resolved and flags
 // entries on the wrong side of the diagonal
 __global__ void __launch_bounds__(256) tr_level_sweep_kernel(int n, const int* __restrict__ rp, const int* __restrict__ ci, int lower,
@@ -210,7 +208,7 @@ void tr_launch_solve(const b200sp_sptrsv_plan* p, cudaStream_t st, int n, const 
     }
     const int q0 = p->level_ptr_host[sg.l0], cntl = p->level_ptr_host[sg.l1] - q0;
     if (cntl <= 0) continue;
-    tr_solve_level_kernel<S, G><<<tr_blocks((int64_t)cntl * G), 256, 0, st>>>(cntl, p->level_rows + q0, n, ci, v, b, x, side, dinv);
+    tr_solve_level_kernel<S, G><<<grid_for((int64_t)cntl * G), 256, 0, st>>>(cntl, p->level_rows + q0, n, ci, v, b, x, side, dinv);
   }
 }
 
@@ -246,7 +244,7 @@ int sptrsv_symbolic_impl(b200sp_sptrsv_plan* p, cudaStream_t st, int n, const in
   B200SP_CUDA_TRY(tmp.alloc(&lv[0], n));
   B200SP_CUDA_TRY(tmp.alloc(&lv[1], n));
   B200SP_CUDA_TRY(tmp.alloc(&cnt, 3));
-  tr_fill_kernel<<<tr_blocks(n), 256, 0, st>>>(n, lv[0], -1);
+  tr_fill_kernel<<<grid_for(n), 256, 0, st>>>(n, lv[0], -1);
   B200SP_LAUNCH_CHECK();
   int h[3] = {0, n, -1};  // rows resolved so far, smallest offending row, highest level handed out
   int nnz = 0;
@@ -264,7 +262,7 @@ int sptrsv_symbolic_impl(b200sp_sptrsv_plan* p, cudaStream_t st, int n, const in
   while (done < n) {
     // a sweep resolves exactly the rows of the next level; sweeps after the last one copy the levels unchanged
     for (int k = 0; k < TR_SWEEP_BATCH; ++k) {
-      tr_level_sweep_kernel<<<tr_blocks(n), 256, 0, st>>>(n, rp, ci, lower ? 1 : 0, filter ? 1 : 0, lv[cur], lv[cur ^ 1], cnt, cnt + 1,
+      tr_level_sweep_kernel<<<grid_for(n), 256, 0, st>>>(n, rp, ci, lower ? 1 : 0, filter ? 1 : 0, lv[cur], lv[cur ^ 1], cnt, cnt + 1,
                                                            cnt + 2);
       B200SP_LAUNCH_CHECK();
       cur ^= 1;
@@ -288,7 +286,7 @@ int sptrsv_symbolic_impl(b200sp_sptrsv_plan* p, cudaStream_t st, int n, const in
   B200SP_CUDA_TRY(tmp.alloc(&count, levels + 1));
   B200SP_CUDA_TRY(tmp.alloc(&cursor, levels + 1));
   B200SP_CUDA_TRY(cudaMemsetAsync(count, 0, sizeof(int) * (size_t)(levels + 1), st));
-  tr_hist_kernel<<<tr_blocks(n), 256, 0, st>>>(n, lv[cur], count);
+  tr_hist_kernel<<<grid_for(n), 256, 0, st>>>(n, lv[cur], count);
   B200SP_LAUNCH_CHECK();
   p->level_ptr_host = new (std::nothrow) int[levels + 1];
   if (!p->level_ptr_host) {
@@ -312,7 +310,7 @@ int sptrsv_symbolic_impl(b200sp_sptrsv_plan* p, cudaStream_t st, int n, const in
   delete[] hc;
   B200SP_CUDA_TRY(cudaMemcpyAsync(cursor, p->level_ptr_host, sizeof(int) * (size_t)(levels + 1), cudaMemcpyHostToDevice, st));
   B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->level_rows, sizeof(int4) * (size_t)n, st));
-  tr_place_kernel<<<tr_blocks(n), 256, 0, st>>>(n, rp, lv[cur], cursor, p->level_rows);
+  tr_place_kernel<<<grid_for(n), 256, 0, st>>>(n, rp, lv[cur], cursor, p->level_rows);
   B200SP_LAUNCH_CHECK();
   B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->level_ptr_dev, sizeof(int) * (size_t)(levels + 1), st));
   B200SP_CUDA_TRY(cudaMemcpyAsync(p->level_ptr_dev, p->level_ptr_host, sizeof(int) * (size_t)(levels + 1), cudaMemcpyHostToDevice, st));

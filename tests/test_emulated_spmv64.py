@@ -28,6 +28,34 @@ def random_crs(m, n, mean, seed, long_rows=0, empty_frac=0.1):
     return rp, ci, v
 
 
+def expected_windows(rp, limit):
+    """The greedy cut the library documents: consecutive rows, each window ending at the last row whose offset lies within
+    `limit` entries of the window's base, its first offset rounded down to a multiple of 4."""
+    m, R, count = len(rp) - 1, 0, 0
+    while R < m:
+        end = np.searchsorted(rp, (int(rp[R]) & ~3) + limit, "right") - 1
+        assert end > R
+        count += 1
+        R = end
+    return count
+
+
+@pytest.mark.parametrize("seed", [0, 1])
+@pytest.mark.parametrize("long_rows", [0, 4])
+def test_window_count_of_the_aligned_cut(emu, seed, long_rows):
+    """Limits from the longest row plus the base's rounding upwards, on row maps with empty rows (and rows of 600 to 1500
+    entries): the window count is the greedy cut's."""
+    m, n = 3000, 2000
+    rp, ci, v = random_crs(m, n, 6.0, seed=seed, long_rows=long_rows, empty_frac=0.3)
+    x, y = np.ones(n), np.zeros(m)
+    lo = int(np.diff(rp).max()) + 3
+    for limit in (lo, lo + 1, lo + 2, 2 * lo, len(ci) // 7):
+        p = E.Spmv64Plan(window=limit)
+        E.spmv64(p, "N", m, n, rp, ci, v, x, y, 1.0, 0.0)
+        assert p.windows() == expected_windows(rp, limit), limit
+        p.close()
+
+
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
 @pytest.mark.parametrize("col_bits", [32, 64])
 @pytest.mark.parametrize("window", [None, 40000, 2000])
