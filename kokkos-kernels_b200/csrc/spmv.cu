@@ -30,6 +30,7 @@
 #include <string.h>
 #include <algorithm>
 #include <mutex>
+#include <type_traits>
 
 namespace b200sp {
 
@@ -545,27 +546,34 @@ __global__ void pattern_assign_kernel(int m, const int* __restrict__ row_ptr, co
 __device__ __forceinline__ int64_t dmin64(int64_t a, int64_t b) { return a < b ? a : b; }
 __device__ __forceinline__ int64_t dmax64(int64_t a, int64_t b) { return a > b ? a : b; }
 
-// column area of the ring (TileRing::cols) in the pattern form: per stage RCAP anchors and RCAP pattern starts, 3*CAP of its
-// 4*CAP bytes, and one dictionary in the STAGES*CAP bytes that frees (>= 5 KB in every configuration).  The ring is no larger
-// than in the 32-bit form, so occupancy is the same.
-template <int CAP, int STAGES>
-struct TilePatCols {
-  int anchor[STAGES][CAP / 2];
-  uint16_t pid[STAGES][CAP / 2];
-  int dict[DCAP];
-};
-
 // which columns the tiled kernel reads: col_idx, the plan's 16-bit deltas + anchors (section 3.5), or its pattern starts +
 // anchors + dictionary (section 3.6)
 enum TileCols { COLS_I32 = 0, COLS_DELTA = 1, COLS_PAT = 2 };
 
+// The pattern form's layout, for every configuration (DESIGN.md sections 3.6 and 7): stages of PAT_CAP entries with PAT_RCAP
+// row slots, two CTAs of 16 consumer warps per SM in f64.  The form streams no per-entry columns, so a stage holds only values
+// and row slots -- row_ptr (TileRing::rows), anchor (cols[0, RCAP)) and pattern start (cols[RCAP, 3*RCAP/2) as uint16) --
+// and the dictionary follows the ring, once per CTA.  Rows of a tile past the row slots read the three from global memory.
+constexpr int PAT_CAP = 4096, PAT_STAGES = 3, PAT_RCAP = 256;
+// The form's value copies start and end on 128-byte lines (EAL below), so that two tiles never split a line between them:
+// up to 2 * (32 - 1) entries of f32 more than the tile, which its tiles leave room for (tile_analyse's T = cap - LMAX - 8).
+constexpr int PAT_TILE_CAP = PAT_CAP - 2 * 32 + 8;
+template <typename S, int CAP, int RCAP, int STAGES>
+using PatTileRing = TileRing<S, CAP, RCAP * 3 / 2, RCAP, STAGES>;
+
+// the ring of spmv_tile_kernel in each column form, and the dynamic shared memory past it (the pattern form's dictionary)
+template <typename S, int CAP, int STAGES, int COLS>
+using TileSmem = std::conditional_t<COLS == COLS_PAT, PatTileRing<S, CAP, PAT_RCAP, STAGES>, CsrTileRing<S, CAP, STAGES>>;
+template <int COLS>
+constexpr int tile_smem_extra() { return COLS == COLS_PAT ? (int)sizeof(int) * DCAP : 0; }
+
 // CTAs per SM with 56 registers per thread and the kernel's ring.  Both column forms are held to it: left alone, the compiler
 // gives the 16-bit form's decode up to 91 registers, and the 32-bit form 80 once both share this kernel -- one CTA per SM
 // instead of two in the default configuration.
-template <typename S, int NW, int STAGES, int CAP>
+template <typename S, int NW, int STAGES, int CAP, int COLS>
 constexpr int tile_ctas_per_sm() {
   const int by_regs = 65536 / ((NW + 1) * 32 * 56);
-  const int by_smem = (227 * 1024) / (int)(sizeof(CsrTileRing<S, CAP, STAGES>) + 128 + 1024);
+  const int by_smem = (227 * 1024) / (int)(sizeof(TileSmem<S, CAP, STAGES, COLS>) + tile_smem_extra<COLS>() + 128 + 1024);
   const int c = by_regs < by_smem ? by_regs : by_smem;
   return c > 1 ? c : 1;
 }
@@ -577,31 +585,30 @@ constexpr int tile_ctas_per_sm() {
 // row instead of 4 per entry.  COLS_PAT: from c16 (pattern starts) / anchor / dict (pattern_*_kernel): 6 bytes per row.
 // Same lanes, same entries per lane, same order: the same bits as the 32-bit form.
 template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, int COLS = COLS_I32, bool FWD = false>
-__global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES, CAP>())
+__global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES, CAP, COLS>())
     spmv_tile_kernel(int m, int64_t nnz, int n_tiles, int LMAX, const int4* __restrict__ tiles,
                      const int* __restrict__ row_ptr, const int* __restrict__ col_idx,
                      const uint16_t* __restrict__ c16, const int* __restrict__ anchor, const int* __restrict__ dict,
                      const S* __restrict__ vals, const S* __restrict__ x, S* __restrict__ y, S alpha,
                      S beta, YExtra ex) {
-  using Smem = CsrTileRing<S, CAP, STAGES>;
-  using PatCols = TilePatCols<CAP, STAGES>;
-  static_assert(sizeof(PatCols) <= sizeof(int) * STAGES * CAP, "the pattern form's columns must fit the 32-bit ring");
+  using Smem = TileSmem<S, CAP, STAGES, COLS>;
   constexpr int RCAP = Smem::RCAP;
   constexpr bool IDX16 = COLS == COLS_DELTA, PAT = COLS == COLS_PAT;
-  // a stage starts at an entry that is a multiple of EAL: 16 bytes of the narrowest entry stream (bulk-copy alignment)
-  constexpr int EAL = IDX16 ? 8 : 4;
+  // a stage starts at an entry that is a multiple of EAL: 16 bytes of the narrowest entry stream (bulk-copy alignment), and
+  // in the pattern form, whose only entry stream is the values, a 128-byte line of them (PAT_TILE_CAP)
+  constexpr int EAL = IDX16 ? 8 : PAT ? 128 / (int)sizeof(S) : 4;
   // ... and at a row that is a multiple of RAL: 16 bytes of the narrowest row stream
   constexpr int RAL = PAT ? 8 : 4;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
-  PatCols& pc = *reinterpret_cast<PatCols*>(&sm.cols[0][0]);
+  int* sdict = reinterpret_cast<int*>(smem_raw + sizeof(Smem));  // PAT: the dictionary, after the ring
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   if constexpr (PAT) {
     const int dl = dict[DCAP];  // used length
-    for (int i = threadIdx.x; i < dl; i += blockDim.x) pc.dict[i] = dict[i];
+    for (int i = threadIdx.x; i < dl; i += blockDim.x) sdict[i] = dict[i];
   }
   tile_ring_init(sm, NW);
 
@@ -643,7 +650,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
       int* sc = sm.cols[stage];
       int* sr = sm.rows[stage];
       uint16_t* sd = reinterpret_cast<uint16_t*>(sc);  // IDX16: deltas, then anchors
-      int* sa = PAT ? pc.anchor[stage] : reinterpret_cast<int*>(sd + CAP);
+      int* sa = PAT ? sc : reinterpret_cast<int*>(sd + CAP);
+      uint16_t* sp = reinterpret_cast<uint16_t*>(sc + RCAP);  // PAT: pattern starts, after the anchors
       // entries [s_al, e) -> smem[0 ..); bulk part [s_al, bulk_end), tail by plain loads.  nnz_al is a multiple of 4 and
       // s_al of EAL, so every bulk length is a multiple of 16 bytes.  The delta stream is padded to a multiple of 8 entries
       // by the plan: its copy [s_al, e_up) is always whole.
@@ -686,7 +694,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
           if (COLS == COLS_I32) bulk_g2s(sc, col_idx + s_al, (uint32_t)(nb * 4), &sm.full[stage], pol);
         }
         if (nd > 0) bulk_g2s(sd, c16 + s_al, (uint32_t)(nd * 2), &sm.full[stage], pol);
-        if (np > 0) bulk_g2s(pc.pid[stage], c16 + r0_al, (uint32_t)(np * 2), &sm.full[stage], pol);
+        if (np > 0) bulk_g2s(sp, c16 + r0_al, (uint32_t)(np * 2), &sm.full[stage], pol);
         if (na > 0) bulk_g2s(sa, anchor + r0_al, (uint32_t)(na * 4), &sm.full[stage], pol);
         if (nrp > 0) bulk_g2s(sr, row_ptr + r0_al, (uint32_t)(nrp * 4), &sm.full[stage], pol);
       }
@@ -736,7 +744,8 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
       const S* sv = sm.vals[stage];
       const int* sc = sm.cols[stage];
       const uint16_t* sd = reinterpret_cast<const uint16_t*>(sc);
-      const int* sa = PAT ? pc.anchor[stage] : reinterpret_cast<const int*>(sd + CAP);
+      const int* sa = PAT ? sc : reinterpret_cast<const int*>(sd + CAP);
+      const uint16_t* sp = reinterpret_cast<const uint16_t*>(sc + RCAP);
       // absolute row groups of RPW rows are dealt round-robin to the warps
       const int g_first = r0 / RPW;
       int g = g_first + ((warp - g_first % NW) + NW) % NW;
@@ -748,7 +757,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
           const int o = r - tv.r0_al;
           if (tile_row_bounds(sm, stage, row_ptr, r, o, rs, re)) {
             if (COLS != COLS_I32) col = sa[o];
-            if (PAT) pb = pc.pid[stage][o];
+            if (PAT) pb = sp[o];
           } else {
             if (COLS != COLS_I32) col = anchor[r];
             if (PAT) pb = c16[r];
@@ -809,7 +818,7 @@ __global__ void __launch_bounds__((NW + 1) * 32, tile_ctas_per_sm<S, NW, STAGES,
             for (int u = 0; u < UNR; ++u) {
               const int j = j0 + u * LPR;
               const bool ok = j < jend;
-              if constexpr (PAT) c[u] = ok ? col + pc.dict[db + j] : 0;
+              if constexpr (PAT) c[u] = ok ? col + sdict[db + j] : 0;
               else c[u] = ok ? sc[j] : 0;
               av[u] = ok ? sv[j] : S(0);
             }
@@ -974,6 +983,8 @@ struct b200sp_spmv_plan {
   int* idx16_anchor = nullptr;     // m anchors, padded to a multiple of 4 rows
   uint16_t* pat_pid = nullptr;     // m pattern starts, padded to a multiple of 8 rows
   int* pat_dict = nullptr;         // DCAP offsets + the used length
+  int4* pat_tiles = nullptr;       // the pattern form's tiles (PAT_TILE_CAP entries, the cfg's LMAX), built with its verdict
+  int pat_n_tiles = 0;
   int* idx16_bad = nullptr;        // device flags: [0] deltas, [1] patterns
   int* idx16_bad_host = nullptr;   // pinned mirror, valid once idx16_event completed
   cudaEvent_t idx16_event = nullptr;
@@ -1024,7 +1035,7 @@ struct b200sp_spmv_plan {
   int t_key_m = -1, t_key_n = -1;
   int64_t t_key_nnz = -1;
   b200sp_spmv_plan* tplan = nullptr;
-  char last_kernel[96] = "none";
+  char last_kernel[160] = "none";
   b200sp::YExtra extra = {{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, 0};
   // self-tuning between the tiled and the row-vector kernel (same bits, different speed by matrix):
   // call 0 tile, call 1 tile timed, call 2 vector timed, then the faster one (DESIGN.md section 3.3)
@@ -1065,6 +1076,9 @@ static void plan_release_idx16_arrays(b200sp_spmv_plan* p, cudaStream_t st) {
   p->pat_pid = nullptr;
   p->pat_dict = nullptr;
   p->idx16_bad = nullptr;
+  if (p->pat_tiles) cudaFreeAsync(p->pat_tiles, st);
+  p->pat_tiles = nullptr;
+  p->pat_n_tiles = 0;
 }
 
 static void plan_release_analysis(b200sp_spmv_plan* p, cudaStream_t st) {
@@ -1113,7 +1127,7 @@ template <typename S>
 static int plan_analyse(b200sp_spmv_plan* p, cudaStream_t st, int cfg, int m, int n, int64_t nnz,
                         const int* row_ptr) {
   if (p->key_row_ptr == row_ptr && p->key_m == m && p->key_n == n && p->key_nnz == nnz &&
-      p->key_cfg == cfg && p->tiles)
+      p->key_cfg == cfg && p->long_rows)
     return B200SP_OK;
   plan_release_analysis(p, st);
   const TileCfg c = kCfgs[cfg];
@@ -1207,6 +1221,23 @@ static int plan_idx16(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, 
   if (p->idx16_state < 0 && cudaEventQuery(p->idx16_event) == cudaSuccess) {
     const int* bad = p->idx16_bad_host;
     p->idx16_state = (p->pat_pid && bad[1] == 0) ? COLS_PAT : bad[0] == 0 ? COLS_DELTA : COLS_I32;
+    if (p->idx16_state == COLS_PAT) {
+      // the pattern form's own tiles, for its larger stages, ahead of its first launch; its long rows are the cfg's (same
+      // LMAX), so the analysis's copy of them is dropped.  A table that cannot be built leaves the matrix on the deltas.
+      TileAnalysis a;
+      const int rc = tile_analyse(st, m, nnz, row_ptr, PAT_TILE_CAP, p->LMAX, &a);
+      if (a.long_rows) cudaFreeAsync(a.long_rows, st);
+      if (a.n_long) cudaFreeAsync(a.n_long, st);
+      p->pat_tiles = a.tiles;
+      p->pat_n_tiles = a.n_tiles;
+      if (rc != B200SP_OK) {
+        (void)cudaGetLastError();
+        if (a.tiles) cudaFreeAsync(a.tiles, st);
+        p->pat_tiles = nullptr;
+        p->pat_n_tiles = 0;
+        p->idx16_state = COLS_DELTA;
+      }
+    }
     if (p->idx16_state == COLS_I32) plan_release_idx16_arrays(p, st);  // the key stays: not built again for this matrix
     if (p->idx16_state == COLS_DELTA) {
       if (p->pat_pid) cudaFreeAsync(p->pat_pid, st);
@@ -1216,6 +1247,39 @@ static int plan_idx16(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, 
     }
   }
   return B200SP_OK;
+}
+
+// The column form of the next tiled launch (p->cols_launch), and so its tile table (plan_tiles).
+// B200SP_SPMV_IDX16=0: the 32-bit columns (A/B comparisons; the 16-bit streams are not built for this call).
+static int plan_cols(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, const int* col_idx) {
+  const char* i16 = getenv("B200SP_SPMV_IDX16");
+  p->cols_launch = COLS_I32;
+  if (!(i16 && i16[0] == '0')) {
+    const int rc = plan_idx16(p, st, m, nnz, row_ptr, col_idx);
+    if (rc) return rc;
+    if (p->idx16_state > 0) p->cols_launch = p->idx16_state;
+  }
+  // one tile table at a time: the pattern form's while it runs, else the cfg's, cut again when a call goes back to them
+  if (p->cols_launch == COLS_PAT) {
+    if (p->tiles) cudaFreeAsync(p->tiles, st);
+    p->tiles = nullptr;
+    p->n_tiles = 0;
+  } else if (!p->tiles) {
+    TileAnalysis a;
+    const int rc = tile_analyse(st, m, nnz, row_ptr, kCfgs[p->key_cfg].cap, p->LMAX, &a);
+    if (a.long_rows) cudaFreeAsync(a.long_rows, st);
+    if (a.n_long) cudaFreeAsync(a.n_long, st);
+    p->tiles = a.tiles;
+    p->n_tiles = a.n_tiles;
+    if (rc != B200SP_OK) return rc;
+  }
+  return B200SP_OK;
+}
+
+static const int4* plan_tiles(const b200sp_spmv_plan* p, int* n_tiles) {
+  const bool pat = p->cols_launch == COLS_PAT;
+  *n_tiles = pat ? p->pat_n_tiles : p->n_tiles;
+  return pat ? p->pat_tiles : p->tiles;
 }
 
 // rank-2 scratch + bookkeeping used by spmm.cu
@@ -1331,45 +1395,53 @@ int spmv_lanes_per_row(int64_t m, int64_t nnz) {  // also used by spmv64.cu: one
   return 32;
 }
 
+// STAGES and CAP are the cfg's; the pattern form runs its own layout (PAT_STAGES stages of PAT_CAP) on the plan's pattern
+// tiles, and reports it after the cfg's label
 template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR, int COLS>
 static int launch_tile_form(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr,
                             const int* col_idx, const S* vals, const S* x, S* y, S alpha, S beta) {
-  using Smem = CsrTileRing<S, CAP, STAGES>;
-  auto kern = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, COLS, false>;
-  const uint16_t* c16 = COLS == COLS_PAT ? p->pat_pid : p->idx16_d;
+  constexpr bool PAT = COLS == COLS_PAT;
+  constexpr int KSTAGES = PAT ? PAT_STAGES : STAGES, KCAP = PAT ? PAT_CAP : CAP;
+  using Smem = TileSmem<S, KCAP, KSTAGES, COLS>;
+  auto kern = spmv_tile_kernel<S, LPR, NW, KSTAGES, KCAP, UNR, COLS, false>;
+  const uint16_t* c16 = PAT ? p->pat_pid : p->idx16_d;
   const int* anchor = p->idx16_anchor;
   const int* dict = p->pat_dict;
-  const size_t smem = sizeof(Smem) + 128;
+  int n_tiles = 0;
+  const int4* tiles = plan_tiles(p, &n_tiles);
+  const size_t smem = sizeof(Smem) + tile_smem_extra<COLS>() + 128;
   static KernelSetup ks;
   int occ_dev = 1;
   if (int rc = kernel_setup(ks, kern, (NW + 1) * 32, smem, &occ_dev)) return rc;
   int per_sm = p->ctas_per_sm;
   if (per_sm <= 0) per_sm = occ_dev;
   const int lo = p->range_hi < 0 ? 0 : p->range_lo;
-  const int hi = p->range_hi < 0 ? p->n_tiles : p->range_hi;
+  const int hi = p->range_hi < 0 ? n_tiles : p->range_hi;
   int grid = std::min(hi - lo, sm_count() * per_sm);
   if (grid < 1) grid = 1;
   bool launched = false;
   if constexpr (sizeof(S) == 8 && NW == 16 && STAGES == 4 && CAP == 2048 && UNR == 8) {
     // the forwarding form exists for the default configuration; elsewhere the consumers store to the destination themselves
     if (p->extra.n < 0) {
-      auto kf = spmv_tile_kernel<S, LPR, NW, STAGES, CAP, UNR, COLS, true>;
+      auto kf = spmv_tile_kernel<S, LPR, NW, KSTAGES, KCAP, UNR, COLS, true>;
       static KernelSetup ksf;
       int occ_f = 1;
       if (int rc = kernel_setup(ksf, kf, (NW + 1) * 32, smem, &occ_f)) return rc;
-      kf<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals,
-                                            x, y, alpha, beta, p->extra);
+      kf<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals, x,
+                                            y, alpha, beta, p->extra);
       launched = true;
     }
   }
   if (!launched)
-    kern<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, p->tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals,
-                                            x, y, alpha, beta, direct_extra(p->extra));
+    kern<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals, x,
+                                            y, alpha, beta, direct_extra(p->extra));
   B200SP_LAUNCH_CHECK();
   // the pattern form is a sub-form of the 16-bit column data (pattern starts + anchors): IDX=u16, and COLS names the source
   static const char* const kColsLabel[] = {"IDX=i32", "IDX=u16,COLS=delta", "IDX=u16,COLS=pat"};
-  snprintf(p->last_kernel, sizeof(p->last_kernel), "tile<%s,LPR=%d,NW=%d,STAGES=%d,CAP=%d,UNR=%d,%s>grid=%d",
-           sizeof(S) == 8 ? "f64" : "f32", LPR, NW, STAGES, CAP, UNR, kColsLabel[COLS], grid);
+  char layout[48] = "";
+  if (PAT) snprintf(layout, sizeof(layout), "pat<STAGES=%d,CAP=%d,RCAP=%d>", KSTAGES, KCAP, PAT_RCAP);
+  snprintf(p->last_kernel, sizeof(p->last_kernel), "tile<%s,LPR=%d,NW=%d,STAGES=%d,CAP=%d,UNR=%d,%s>%sgrid=%d",
+           sizeof(S) == 8 ? "f64" : "f32", LPR, NW, STAGES, CAP, UNR, kColsLabel[COLS], layout, grid);
   return B200SP_OK;
 }
 
@@ -1548,13 +1620,10 @@ static int spmv_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   const int cfg = p->cfg >= 0 ? p->cfg : 8;  // CAP=2048, 4 stages, 16 consumer warps, 2 CTAs/SM
   int rc = plan_analyse<S>(p, st, cfg, m, n, nnz, row_ptr);
   if (rc) return rc;
-  // B200SP_SPMV_IDX16=0: the 32-bit columns (A/B comparisons; the 16-bit streams are not built for this call)
-  const char* i16 = getenv("B200SP_SPMV_IDX16");
-  p->cols_launch = COLS_I32;
-  if (!(i16 && i16[0] == '0')) {
-    rc = plan_idx16(p, st, m, nnz, row_ptr, col_idx);
+  // a piece of the host-vector pipeline runs the form its call settled on, with the tiles its bounds were cut from
+  if (p->range_hi < 0) {
+    rc = plan_cols(p, st, m, nnz, row_ptr, col_idx);
     if (rc) return rc;
-    if (p->idx16_state > 0) p->cols_launch = p->idx16_state;
   }
   const int lpr = p->lpr > 0 ? p->lpr : lpr_auto;
   // ---- self-tuning (only for untuned plans on whole-matrix launches)
@@ -1947,7 +2016,12 @@ int b200sp_spmv_hostvec_f64_i32(b200sp_spmv_plan* p, void* stream, char mode, in
   const int cfg = p->cfg >= 0 ? p->cfg : 8;
   int rc = plan_analyse<double>(p, st, cfg, m, n, nnz, row_ptr);
   if (rc) return rc;
-  if (q.key != row_ptr || q.key_cfg != cfg || q.key_m != m || q.key_nnz != nnz || q.key_tiles != (const void*)p->tiles) {
+  // the column form is settled once per call, so that every piece launches on the table the bounds come from
+  rc = plan_cols(p, st, m, nnz, row_ptr, col_idx);
+  if (rc) return rc;
+  int n_tiles = 0;
+  const int4* tiles = plan_tiles(p, &n_tiles);
+  if (q.key != row_ptr || q.key_cfg != cfg || q.key_m != m || q.key_nnz != nnz || q.key_tiles != (const void*)tiles) {
     q.nc = 4;  // pieces of y that go down while the next piece is computed (B200SP_HOSTVEC_PIECES: 1..8, tuning)
     if (const char* e = getenv("B200SP_HOSTVEC_PIECES")) {
       const int v = atoi(e);
@@ -1955,8 +2029,8 @@ int b200sp_spmv_hostvec_f64_i32(b200sp_spmv_plan* p, void* stream, char mode, in
     }
     int4 d[9];
     for (int c = 0; c <= q.nc; ++c) {
-      q.tile_b[c] = (int)(((int64_t)p->n_tiles * c) / q.nc);
-      if (c < q.nc) B200SP_CUDA_TRY(cudaMemcpyAsync(&d[c], p->tiles + q.tile_b[c], sizeof(int4), cudaMemcpyDeviceToHost, st));
+      q.tile_b[c] = (int)(((int64_t)n_tiles * c) / q.nc);
+      if (c < q.nc) B200SP_CUDA_TRY(cudaMemcpyAsync(&d[c], tiles + q.tile_b[c], sizeof(int4), cudaMemcpyDeviceToHost, st));
     }
     B200SP_CUDA_TRY(cudaStreamSynchronize(st));
     for (int c = 0; c < q.nc; ++c) q.row_b[c] = d[c].x;  // first row of the first tile of piece c
@@ -1966,7 +2040,7 @@ int b200sp_spmv_hostvec_f64_i32(b200sp_spmv_plan* p, void* stream, char mode, in
     q.key_cfg = cfg;
     q.key_m = m;
     q.key_nnz = nnz;
-    q.key_tiles = (const void*)p->tiles;
+    q.key_tiles = (const void*)tiles;
   }
   const int b = (int)(q.call & 1ull);
   if (q.defer && q.call >= 2) {
