@@ -49,7 +49,7 @@ def build(force=False, verbose=True):
 def _build_locked(force, verbose):
     out = os.path.join(LIB, "libb200sparse.so")
     srcs = [os.path.join(CSRC, s) for s in CU_SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scan.cuh"), os.path.join(CSRC, "tile_ring.cuh"), os.path.join(CSRC, "spgemm_esc.cuh"), os.path.join(CSRC, "bspgemm.cuh"), os.path.join(CSRC, "spmm_items.h"), os.path.join(CSRC, "windows64.cuh"), os.path.join(HERE, "..", "include", "b200sparse.h")]
+    deps = srcs + [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "scan.cuh"), os.path.join(CSRC, "tile_ring.cuh"), os.path.join(CSRC, "spgemm_esc.cuh"), os.path.join(CSRC, "bspgemm.cuh"), os.path.join(CSRC, "spmv_plan.h"), os.path.join(CSRC, "windows64.cuh"), os.path.join(HERE, "..", "include", "b200sparse.h")]
     if force or not _newer(out, deps):
         objs = []
         procs = []

@@ -43,17 +43,16 @@ static constexpr int kBspLongCtas = 32;
 static constexpr int kBspAStage = 24 * 1024;  // bytes of A blocks staged per CTA
 
 struct BspState {
-  int* rows = nullptr;  // block rows grouped by bin: [<= CAP0 | <= CAP1 | long]
+  DevArray<int> rows;  // block rows grouped by bin: [<= CAP0 | <= CAP1 | long]
   int off[4] = {0, 0, 0, 0};
   int long_log2 = 1;    // keys per long-row CTA: 2^long_log2 >= the longest row's products and A entries
-  void* scratch = nullptr;
-  size_t scratch_bytes = 0;
+  DevArray<unsigned char> scratch;
 };
 
 void bsp_state_free(BspState* s, cudaStream_t st) {
   if (!s) return;
-  if (s->rows) cudaFreeAsync(s->rows, st);
-  if (s->scratch) cudaFreeAsync(s->scratch, st);
+  s->rows.release(st);
+  s->scratch.release(st);
   delete s;
 }
 
@@ -275,7 +274,7 @@ static int bsp_state_build(const SpgemmPlanView& v, cudaStream_t st, const int* 
   int* d;  // counts[3] | cursors[3] | maxkey
   cudaError_t e = tmp.alloc(&d, 8);
   if (e == cudaSuccess) e = cudaMemsetAsync(d, 0, sizeof(int) * 8, st);
-  if (e == cudaSuccess) e = cudaMallocAsync((void**)&s->rows, sizeof(int) * (size_t)std::max(m, 1), st);
+  if (e == cudaSuccess) e = s->rows.alloc((size_t)std::max(m, 1), st);
   if (e != cudaSuccess) {
     bsp_state_free(s, st);
     set_error("bspgemm_numeric: %s", cudaGetErrorString(e));
@@ -302,8 +301,7 @@ static int bsp_state_build(const SpgemmPlanView& v, cudaStream_t st, const int* 
     s->long_log2 = lg;
     const size_t cap = (size_t)1 << lg;
     const size_t slice = (sizeof(unsigned long long) * cap + sizeof(int) * (cap * 5 + 2 + 40) + 15) & ~(size_t)15;
-    s->scratch_bytes = slice * (size_t)std::min(h[2], kBspLongCtas);
-    e = cudaMallocAsync(&s->scratch, s->scratch_bytes, st);
+    e = s->scratch.alloc(slice * (size_t)std::min(h[2], kBspLongCtas), st);
   }
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);  // s->off (pageable) consumed by the copy above
   g_launches.fetch_add(2, std::memory_order_relaxed);
@@ -368,7 +366,7 @@ static int bspgemm_impl(b200sp_spgemm_plan* plan, cudaStream_t st, int mb, int n
     static KernelSetup ks;
     int occ = 1;
     if ((rc = kernel_setup(ks, kern, 512, smem, &occ))) return rc;
-    kern<<<std::min(nlong, kBspLongCtas), 512, smem, st>>>(nlong, s.rows + s.off[2], (int)cap, (unsigned char*)s.scratch, slice, bs,
+    kern<<<std::min(nlong, kBspLongCtas), 512, smem, st>>>(nlong, s.rows + s.off[2], (int)cap, s.scratch, slice, bs,
                                                            rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC);
     B200SP_LAUNCH_CHECK();
   }

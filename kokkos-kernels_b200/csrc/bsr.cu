@@ -483,15 +483,8 @@ extern "C" int b200sp_spmv_plan_create(b200sp_spmv_plan** plan, int algo);
 extern "C" int b200sp_spmv_plan_destroy(b200sp_spmv_plan* p, void* stream);
 
 struct b200sp_bsr_plan {
-  // cache key of the analysed structure
-  const int* key_row_ptr = nullptr;
-  int key_mb = -1, key_bs = -1, key_capb = -1;
-  int64_t key_nnzb = -1;
-  // analysis products (device)
-  int4* tiles = nullptr;
-  int n_tiles = 0, T = 0, lmaxb = 0;
-  int* long_rows = nullptr;
-  int* n_long = nullptr;
+  b200sp::TileAnalysis a;  // of the block rows, blocks for entries
+  b200sp::PlanKey key;     // of the analysed structure
   // blockDim() == 1 is a CrsMatrix (KokkosSparse_spmv.hpp:169-185): forwarded to the CSR path
   b200sp_spmv_plan* crs = nullptr;
   int algo = 0;  // B200SP_BSR_ALGO_*: 1 = tensor cores for the multivector product (SPMV_BSR_TC)
@@ -501,34 +494,14 @@ struct b200sp_bsr_plan {
 namespace b200sp {
 namespace {
 
-void bsr_release(b200sp_bsr_plan* p, cudaStream_t st) {
-  if (p->tiles) cudaFreeAsync(p->tiles, st);
-  if (p->long_rows) cudaFreeAsync(p->long_rows, st);
-  if (p->n_long) cudaFreeAsync(p->n_long, st);
-  p->tiles = nullptr;
-  p->long_rows = nullptr;
-  p->n_long = nullptr;
-  p->key_row_ptr = nullptr;
-}
-
 int bsr_analyse(b200sp_bsr_plan* p, cudaStream_t st, int mb, int64_t nnzb, int bs, int capb, const int* row_ptr) {
-  if (p->tiles && p->key_row_ptr == row_ptr && p->key_mb == mb && p->key_nnzb == nnzb && p->key_bs == bs && p->key_capb == capb)
-    return B200SP_OK;
-  bsr_release(p, st);
-  TileAnalysis a;
-  const int rc = tile_analyse(st, mb, nnzb, row_ptr, capb, capb / 4, &a);  // blocks for entries
-  p->tiles = a.tiles;
-  p->n_tiles = a.n_tiles;
-  p->T = a.T;
-  p->lmaxb = a.LMAX;
-  p->long_rows = a.long_rows;
-  p->n_long = a.n_long;
+  const PlanKey key{row_ptr, nullptr, mb, -1, nnzb, bs, capb};
+  if (p->key == key) return B200SP_OK;
+  p->key = PlanKey();
+  p->a.release(st);
+  const int rc = tile_analyse(st, mb, nnzb, row_ptr, capb, capb / 4, &p->a);  // blocks for entries
   if (rc != B200SP_OK) return rc;
-  p->key_row_ptr = row_ptr;
-  p->key_mb = mb;
-  p->key_nnzb = nnzb;
-  p->key_bs = bs;
-  p->key_capb = capb;
+  p->key = key;
   return B200SP_OK;
 }
 
@@ -560,12 +533,12 @@ int launch_tile(b200sp_bsr_plan* p, cudaStream_t st, int mb, int64_t nnzb, int b
   if (rc != B200SP_OK) return rc;
   const double avg = mb > 0 ? (double)nnzb * bs / (double)mb : 0.0;
   const int lpr = pick_lpr(avg, bs, 32);
-  const int grid = std::max(1, std::min(p->n_tiles, sm_count() * occ_dev));
-  kern<<<grid, (NW + 1) * 32, smem, st>>>(mb, nnzb, bs, lpr, p->lmaxb, p->n_tiles, p->tiles, rp, ci, v, x, y, alpha, beta);
+  const int grid = std::max(1, std::min(p->a.n_tiles, sm_count() * occ_dev));
+  kern<<<grid, (NW + 1) * 32, smem, st>>>(mb, nnzb, bs, lpr, p->a.LMAX, p->a.n_tiles, p->a.tiles, rp, ci, v, x, y, alpha, beta);
   B200SP_LAUNCH_CHECK();
   // block rows longer than a stage: one warp per point row, list and count stay on the device
   const int lblocks = sm_count() * 2;
-  bsr_vector_kernel<S><<<lblocks, 256, 0, st>>>(mb, bs, 32, rp, ci, v, x, y, alpha, beta, p->long_rows, p->n_long);
+  bsr_vector_kernel<S><<<lblocks, 256, 0, st>>>(mb, bs, 32, rp, ci, v, x, y, alpha, beta, p->a.long_rows, p->a.n_long);
   B200SP_LAUNCH_CHECK();
   snprintf(p->last_kernel, sizeof(p->last_kernel), "bsr_tile<%s,bs=%d,LPR=%d,NW=%d,STAGES=%d,VCAP=%d>grid=%d", sizeof(S) == 8 ? "f64" : "f32",
            bs, lpr, NW, STAGES, VCAP, grid);
@@ -585,10 +558,10 @@ int launch_tile_e(b200sp_bsr_plan* p, cudaStream_t st, int mb, int64_t nnzb, con
   const int capb = std::min(Smem::CCAP, VCAP / (BS * BS)) & ~3;
   int rc = bsr_analyse(p, st, mb, nnzb, BS, capb, rp);
   if (rc != B200SP_OK) return rc;
-  const int grid = std::max(1, std::min(p->n_tiles, sm_count() * occ_dev));
-  kern<<<grid, (NW + 1) * 32, smem, st>>>(mb, nnzb, p->lmaxb, p->n_tiles, p->tiles, rp, ci, v, x, y, alpha, beta);
+  const int grid = std::max(1, std::min(p->a.n_tiles, sm_count() * occ_dev));
+  kern<<<grid, (NW + 1) * 32, smem, st>>>(mb, nnzb, p->a.LMAX, p->a.n_tiles, p->a.tiles, rp, ci, v, x, y, alpha, beta);
   B200SP_LAUNCH_CHECK();
-  bsr_vector_kernel<S><<<sm_count() * 2, 256, 0, st>>>(mb, BS, 32, rp, ci, v, x, y, alpha, beta, p->long_rows, p->n_long);
+  bsr_vector_kernel<S><<<sm_count() * 2, 256, 0, st>>>(mb, BS, 32, rp, ci, v, x, y, alpha, beta, p->a.long_rows, p->a.n_long);
   B200SP_LAUNCH_CHECK();
   snprintf(p->last_kernel, sizeof(p->last_kernel), "bsr_tile_e<%s,BS=%d,NW=%d,STAGES=%d,VCAP=%d>grid=%d", sizeof(S) == 8 ? "f64" : "f32", BS,
            NW, STAGES, VCAP, grid);
@@ -788,7 +761,7 @@ int b200sp_bsr_plan_create(b200sp_bsr_plan** plan) {
 
 int b200sp_bsr_plan_destroy(b200sp_bsr_plan* p, void* stream) {
   if (!p) return B200SP_OK;
-  bsr_release(p, (cudaStream_t)stream);
+  p->a.release((cudaStream_t)stream);
   if (p->crs) b200sp_spmv_plan_destroy(p->crs, stream);
   delete p;
   return B200SP_OK;

@@ -8,6 +8,7 @@
 #endif
 #include <stdint.h>
 #include <stdio.h>
+#include <assert.h>
 #include <algorithm>
 #include <atomic>
 #include "../../include/b200sparse.h"
@@ -100,6 +101,57 @@ struct DevTmp {  // frees stream-ordered on scope exit
     *out = (T*)q;
     return e;
   }
+};
+
+// stream-ordered device memory a plan keeps between calls: one owner, freed by release() on the caller's stream.  The
+// destructor frees nothing (a plan is destroyed with the stream its memory goes back on).  Buffers whose scalar type is
+// chosen per call are DevArray<char>, sized in bytes.  A move leaves the source empty; the target must be empty (asserted:
+// a block it held would be lost).
+template <typename T>
+struct DevArray {
+  T* ptr = nullptr;
+  size_t count = 0;
+  DevArray() = default;
+  DevArray(const DevArray&) = delete;
+  DevArray& operator=(const DevArray&) = delete;
+  DevArray(DevArray&& o) noexcept : ptr(o.ptr), count(o.count) { o.ptr = nullptr, o.count = 0; }
+  DevArray& operator=(DevArray&& o) noexcept {
+    assert(ptr == nullptr);
+    ptr = o.ptr, count = o.count;
+    o.ptr = nullptr, o.count = 0;
+    return *this;
+  }
+  operator T*() const { return ptr; }
+  template <typename U>
+  U* as() const {
+    return reinterpret_cast<U*>(ptr);
+  }
+  void release(cudaStream_t st) {
+    if (ptr) cudaFreeAsync(ptr, st);
+    ptr = nullptr;
+    count = 0;
+  }
+  // exactly n elements, in place of what the array held
+  cudaError_t alloc(size_t n, cudaStream_t st) {
+    release(st);
+    const cudaError_t e = cudaMallocAsync((void**)&ptr, sizeof(T) * n, st);
+    if (e == cudaSuccess) count = n;
+    else ptr = nullptr;
+    return e;
+  }
+  // at least n elements: the block is kept when it is large enough
+  cudaError_t grow(size_t n, cudaStream_t st) { return n <= count ? cudaSuccess : alloc(n, st); }
+};
+
+// what a plan's cached product was built from, compared whole; the default key matches no call (row_ptr is never null there)
+struct PlanKey {
+  const void* row_ptr = nullptr;
+  const void* col_idx = nullptr;
+  int64_t m = -1, n = -1, nnz = -1, a = -1, b = -1;  // a, b: the product's own parameters (cfg, stage, row limit, ...)
+  bool operator==(const PlanKey& o) const {
+    return row_ptr == o.row_ptr && col_idx == o.col_idx && m == o.m && n == o.n && nnz == o.nnz && a == o.a && b == o.b;
+  }
+  bool operator!=(const PlanKey& o) const { return !(*this == o); }
 };
 
 #ifdef B200SP_EMU

@@ -784,16 +784,15 @@ struct b200sp_spadd_plan {
   int m = 0, n = 0;
   int64_t c_nnz = 0;
   int64_t nnzA = 0, nnzB = 0;
-  int *apos = nullptr, *bpos = nullptr;  // unsorted path: position of every A / B entry in its C row
-  int* simple = nullptr;                 // unsorted path, per row: no repeated column inside A_i or inside B_i
+  b200sp::DevArray<int> apos, bpos;  // unsorted path: position of every A / B entry in its C row
+  b200sp::DevArray<int> simple;       // unsorted path, per row: no repeated column inside A_i or inside B_i
 };
 
 namespace b200sp {
 static void spadd_release(b200sp_spadd_plan* p, cudaStream_t st) {
-  if (p->apos) cudaFreeAsync(p->apos, st);
-  if (p->bpos) cudaFreeAsync(p->bpos, st);
-  if (p->simple) cudaFreeAsync(p->simple, st);
-  p->apos = p->bpos = p->simple = nullptr;
+  p->apos.release(st);
+  p->bpos.release(st);
+  p->simple.release(st);
   p->symbolic_done = false;
 }
 
@@ -993,9 +992,9 @@ int b200sp_spadd_symbolic_i32(b200sp_spadd_plan* p, void* stream, int m, int n, 
     B200SP_LAUNCH_CHECK();
     rc = sort_crs_impl<int, 2>(st, m, rpU, ciU, perm, ub);
     if (rc) return rc;
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->apos, sizeof(int) * (size_t)std::max(lastA, 1), st));
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->bpos, sizeof(int) * (size_t)std::max(lastB, 1), st));
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->simple, sizeof(int) * (size_t)m, st));
+    B200SP_CUDA_TRY(p->apos.alloc((size_t)std::max(lastA, 1), st));
+    B200SP_CUDA_TRY(p->bpos.alloc((size_t)std::max(lastB, 1), st));
+    B200SP_CUDA_TRY(p->simple.alloc((size_t)m, st));
     spadd_merge_entries_kernel<<<grid_for((int64_t)m * 8), 256, 0, st>>>(m, rpA, rpB, rpU, ciU, perm, counts, p->apos, p->bpos, p->simple);
     B200SP_LAUNCH_CHECK();
     rc = counts_to_offsets(st, m, counts, rpC, &total, nullptr);

@@ -209,11 +209,11 @@ struct b200sp_gs_plan {
   int ncols = 0;  // num_cols of the matrix symbolic saw (>= n: columns beyond n are ghost entries of x)
   int n = -1;
   int num_colors = 0;
-  int* colors = nullptr;      // device, n
-  int* color_ptr = nullptr;   // device, num_colors + 1
-  int* color_rows = nullptr;  // device, n
+  DevArray<int> colors;      // n
+  DevArray<int> color_ptr;   // num_colors + 1
+  DevArray<int> color_rows;  // n
   std::vector<int> h_color_ptr;
-  void* dinv = nullptr;  // device, n scalars of the numeric call's type
+  DevArray<char> dinv;  // n scalars of the numeric call's type
   int dinv_bytes_per = 0;
   bool symbolic_done = false, numeric_done = false;
   int lpr = 4;
@@ -223,12 +223,10 @@ namespace b200sp {
 namespace {
 
 void gs_release(b200sp_gs_plan* p, cudaStream_t st) {
-  if (p->colors) cudaFreeAsync(p->colors, st);
-  if (p->color_ptr) cudaFreeAsync(p->color_ptr, st);
-  if (p->color_rows) cudaFreeAsync(p->color_rows, st);
-  if (p->dinv) cudaFreeAsync(p->dinv, st);
-  p->colors = p->color_ptr = p->color_rows = nullptr;
-  p->dinv = nullptr;
+  p->colors.release(st);
+  p->color_ptr.release(st);
+  p->color_rows.release(st);
+  p->dinv.release(st);
   p->symbolic_done = p->numeric_done = false;
 }
 
@@ -245,17 +243,13 @@ int gs_numeric_impl(b200sp_gs_plan* p, cudaStream_t st, int n, const int* rp, co
     return B200SP_OK;
   }
   B200SP_REQUIRE(rp && ci && v, "gauss_seidel_numeric: null array");
-  if (p->dinv && p->dinv_bytes_per != (int)sizeof(S)) {
-    cudaFreeAsync(p->dinv, st);
-    p->dinv = nullptr;
-  }
-  if (!p->dinv) B200SP_CUDA_TRY(cudaMallocAsync(&p->dinv, sizeof(S) * (size_t)n, st));
+  B200SP_CUDA_TRY(p->dinv.grow(sizeof(S) * (size_t)n, st));
   p->dinv_bytes_per = (int)sizeof(S);
   DevTmp tmp(st);
   int* missing = nullptr;
   B200SP_CUDA_TRY(tmp.alloc(&missing, 1));
   B200SP_CUDA_TRY(cudaMemsetAsync(missing, 0, sizeof(int), st));
-  gs_inverse_diagonal_kernel<S><<<grid_for(n), 256, 0, st>>>(n, rp, ci, v, (S*)p->dinv, missing);
+  gs_inverse_diagonal_kernel<S><<<grid_for(n), 256, 0, st>>>(n, rp, ci, v, p->dinv.as<S>(), missing);
   B200SP_LAUNCH_CHECK();
   int h_missing = 0;
   B200SP_CUDA_TRY(cudaMemcpyAsync(&h_missing, missing, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -282,7 +276,7 @@ int gs_apply_impl(b200sp_gs_plan* p, cudaStream_t st, int n, const int* rp, cons
   B200SP_REQUIRE(rp && ci && v && x && y, "gauss_seidel_apply: null array");
   if (init_zero_x)  // all of x, ghost entries included, as the reference's zero_vector(num_cols, ...) does (gauss_seidel_impl.hpp:1426-1428)
     B200SP_CUDA_TRY(cudaMemsetAsync(x, 0, sizeof(S) * (size_t)std::max(n, p->ncols), st));
-  const S* dinv = (const S*)p->dinv;
+  const S* dinv = p->dinv.as<const S>();
   for (int s = 0; s < sweeps; ++s) {
     for (int backward = 0; backward < 2; ++backward) {
       if (!backward && direction == 2) continue;
@@ -363,8 +357,8 @@ int b200sp_gs_symbolic_nc_i32(b200sp_gs_plan* p, void* stream, int n, int ncols,
     const int rc = transpose_structure(st, n, ncols, nnz, row_ptr, col_idx, trp, tci, tsrc);
     if (rc != B200SP_OK) return rc;
   }
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->colors, sizeof(int) * (size_t)n, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->color_rows, sizeof(int) * (size_t)n, st));
+  B200SP_CUDA_TRY(p->colors.alloc((size_t)n, st));
+  B200SP_CUDA_TRY(p->color_rows.alloc((size_t)n, st));
   B200SP_CUDA_TRY(tmp.alloc(&next, (size_t)n));
   B200SP_CUDA_TRY(tmp.alloc(&remaining, 1));
   B200SP_CUDA_TRY(tmp.alloc(&flag, (size_t)n));
@@ -430,7 +424,7 @@ int b200sp_gs_symbolic_nc_i32(b200sp_gs_plan* p, void* stream, int n, int ncols,
   }
   // the row list of every set (stream compaction per colour: rows stay ascending inside a set)
   p->num_colors = h_max + 1;
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->color_ptr, sizeof(int) * (size_t)(p->num_colors + 1), st));
+  B200SP_CUDA_TRY(p->color_ptr.alloc((size_t)(p->num_colors + 1), st));
   B200SP_CUDA_TRY(cudaMemsetAsync(p->color_ptr, 0, sizeof(int) * (size_t)(p->num_colors + 1), st));
   for (int c = 0; c < p->num_colors; ++c) {
     gs_flag_kernel<<<grid, 256, 0, st>>>(n, p->colors, c, flag);

@@ -49,12 +49,12 @@ struct b200sp_gs2_plan {
   int64_t nnz = 0;
   const int *key_rp = nullptr, *key_ci = nullptr;
   int scalar_bytes = 0;
-  int* rp[4] = {nullptr, nullptr, nullptr, nullptr};  // L, U, La, Ua
-  int* ci[4] = {nullptr, nullptr, nullptr, nullptr};
-  void* v[4] = {nullptr, nullptr, nullptr, nullptr};
+  b200sp::DevArray<int> rp[4];  // L, U, La, Ua
+  b200sp::DevArray<int> ci[4];
+  b200sp::DevArray<char> v[4];  // values and vectors below: scalars of the numeric call's type
   int64_t cnt[4] = {0, 0, 0, 0};
-  void *D = nullptr, *Da = nullptr;
-  void *R = nullptr, *T = nullptr, *Z = nullptr;
+  b200sp::DevArray<char> D, Da;
+  b200sp::DevArray<char> R, T, Z;
   int work_cols = 0;  // right-hand sides R, T, Z are sized for
   b200sp_spmv_plan* plan[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // L, U, La, Ua, A
 };
@@ -218,18 +218,12 @@ __global__ void __launch_bounds__(256) gs2_update_kernel(int n, const S* __restr
 
 void release_parts(b200sp_gs2_plan* p, cudaStream_t st) {
   for (int q = 0; q < 4; ++q) {
-    if (p->rp[q]) cudaFreeAsync(p->rp[q], st);
-    if (p->ci[q]) cudaFreeAsync(p->ci[q], st);
-    if (p->v[q]) cudaFreeAsync(p->v[q], st);
-    p->rp[q] = p->ci[q] = nullptr;
-    p->v[q] = nullptr;
+    p->rp[q].release(st);
+    p->ci[q].release(st);
+    p->v[q].release(st);
     p->cnt[q] = 0;
   }
-  void** vecs[] = {&p->D, &p->Da, &p->R, &p->T, &p->Z};
-  for (void** q : vecs) {
-    if (*q) cudaFreeAsync(*q, st);
-    *q = nullptr;
-  }
+  for (DevArray<char>* q : {&p->D, &p->Da, &p->R, &p->T, &p->Z}) q->release(st);
   p->symbolic = p->numeric = false;
   p->scalar_bytes = 0;
   p->work_cols = 0;
@@ -270,22 +264,16 @@ int numeric_impl(b200sp_gs2_plan* p, cudaStream_t st, int n, int ncols, const in
     return B200SP_ERR_STATE;
   }
   if (p->scalar_bytes != (int)sizeof(S)) {
-    void** bufs[] = {&p->v[0], &p->v[1], &p->v[2], &p->v[3], &p->D, &p->Da, &p->R, &p->T, &p->Z};
-    for (void** q : bufs) {
-      if (*q) cudaFreeAsync(*q, st);
-      *q = nullptr;
-    }
     for (int q = 0; q < 4; ++q)
-      if (q < 2 || p->compact) B200SP_CUDA_TRY(cudaMallocAsync(&p->v[q], sizeof(S) * (size_t)std::max<int64_t>(p->cnt[q], 1), st));
-    void** vecs[] = {&p->D, &p->Da, &p->R, &p->T, &p->Z};
-    for (void** q : vecs) B200SP_CUDA_TRY(cudaMallocAsync(q, sizeof(S) * (size_t)std::max(n, 1), st));
+      if (q < 2 || p->compact) B200SP_CUDA_TRY(p->v[q].grow(sizeof(S) * (size_t)std::max<int64_t>(p->cnt[q], 1), st));
+    for (DevArray<char>* q : {&p->D, &p->Da, &p->R, &p->T, &p->Z}) B200SP_CUDA_TRY(q->grow(sizeof(S) * (size_t)std::max(n, 1), st));
     p->scalar_bytes = (int)sizeof(S);
     p->work_cols = 1;
   }
   if (n > 0) {
     B200SP_REQUIRE(vals != nullptr, "gs2_numeric: null values");
-    gs2_values_kernel<S><<<grid_for(n), 256, 0, st>>>(n, row_ptr, col_idx, vals, given_dinv, p->rp[kL], (S*)p->v[kL], p->rp[kU], (S*)p->v[kU],
-                                                         p->rp[kLa], (S*)p->v[kLa], p->rp[kUa], (S*)p->v[kUa], (S*)p->D, (S*)p->Da,
+    gs2_values_kernel<S><<<grid_for(n), 256, 0, st>>>(n, row_ptr, col_idx, vals, given_dinv, p->rp[kL], p->v[kL].as<S>(), p->rp[kU], p->v[kU].as<S>(),
+                                                         p->rp[kLa], p->v[kLa].as<S>(), p->rp[kUa], p->v[kUa].as<S>(), p->D.as<S>(), p->Da.as<S>(),
                                                          p->compact ? 1 : 0);
     B200SP_LAUNCH_CHECK();
   }
@@ -318,17 +306,12 @@ int apply_impl(b200sp_gs2_plan* p, void* stream, int n, int ncols, const int* ro
   const int k = nrhs;
   const int64_t total = (int64_t)n * k;
   if (k > p->work_cols) {  // work vectors for k right-hand sides (numeric sizes them for one)
-    void** vecs[] = {&p->R, &p->T, &p->Z};
-    for (void** q : vecs) {
-      if (*q) cudaFreeAsync(*q, st);
-      *q = nullptr;
-    }
     p->work_cols = 0;
-    for (void** q : vecs) B200SP_CUDA_TRY(cudaMallocAsync(q, sizeof(S) * (size_t)total, st));
+    for (DevArray<char>* q : {&p->R, &p->T, &p->Z}) B200SP_CUDA_TRY(q->grow(sizeof(S) * (size_t)total, st));
     p->work_cols = k;
   }
-  S *R = (S*)p->R, *T = (S*)p->T, *Z = (S*)p->Z;
-  const S *D = (const S*)p->D, *Da = (const S*)p->Da;
+  S *R = p->R.as<S>(), *T = p->T.as<S>(), *Z = p->Z.as<S>();
+  const S *D = p->D.as<const S>(), *Da = p->Da.as<const S>();
   const dim3 nb((unsigned)grid_for(n), (unsigned)k);  // blockIdx.y = right-hand side
   if (k == 1) {
     ldx = ncols;
@@ -346,7 +329,7 @@ int apply_impl(b200sp_gs2_plan* p, void* stream, int n, int ncols, const int* ro
     if (sweep > 0 || !init_zero_x) {
       if (p->compact) {
         const int q = forward ? kUa : kLa;
-        rc = product<S>(p->plan[q], stream, n, ncols, p->cnt[q], k, -one, p->rp[q], p->ci[q], (const S*)p->v[q], x, ldx, one, R, n);
+        rc = product<S>(p->plan[q], stream, n, ncols, p->cnt[q], k, -one, p->rp[q], p->ci[q], p->v[q].as<const S>(), x, ldx, one, R, n);
         if (rc) return rc;
         if (omega != one) {
           gs2_diag_term_kernel<S><<<nb, 256, 0, st>>>(n, Da, x, ldx, one / omega - one, Z, R);
@@ -374,7 +357,7 @@ int apply_impl(b200sp_gs2_plan* p, void* stream, int n, int ncols, const int* ro
       gs2_copy_kernel<S><<<nb, 256, 0, st>>>(n, T, (int64_t)n, Z, (int64_t)n);
       B200SP_LAUNCH_CHECK();
       const int q = forward ? kL : kU;
-      rc = product<S>(p->plan[q], stream, n, n, p->cnt[q], k, -omega, p->rp[q], p->ci[q], (const S*)p->v[q], R, n, one, Z, n);
+      rc = product<S>(p->plan[q], stream, n, n, p->cnt[q], k, -omega, p->rp[q], p->ci[q], p->v[q].as<const S>(), R, n, one, Z, n);
       if (rc) return rc;
       const int copy_back = ii + 1 < p->inner;
       if (gamma != one) {
@@ -480,7 +463,7 @@ int b200sp_gs2_symbolic_i32(b200sp_gs2_plan* p, void* stream, int n, int ncols, 
   gs2_count_kernel<<<grid_for(n), 256, 0, st>>>(n, row_ptr, col_idx, cnt[0], cnt[1], cnt[2], cnt[3], compact ? 1 : 0, nodiag);
   B200SP_LAUNCH_CHECK();
   for (int q = 0; q < parts; ++q) {
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->rp[q], sizeof(int) * ((size_t)n + 4), st));
+    B200SP_CUDA_TRY(p->rp[q].alloc((size_t)n + 4, st));
     const int rc = launch_exclusive_scan(st, n, cnt[q], p->rp[q], bsum, bmax, dtotal + q, dmax);
     if (rc) return rc;
   }
@@ -498,7 +481,7 @@ int b200sp_gs2_symbolic_i32(b200sp_gs2_plan* p, void* stream, int n, int ncols, 
   p->nnz = h_last[0];
   for (int q = 0; q < parts; ++q) {
     p->cnt[q] = h_total[q];
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->ci[q], sizeof(int) * (size_t)std::max<int64_t>(p->cnt[q], 1), st));
+    B200SP_CUDA_TRY(p->ci[q].alloc((size_t)std::max<int64_t>(p->cnt[q], 1), st));
   }
   gs2_entries_kernel<<<grid_for(n), 256, 0, st>>>(n, row_ptr, col_idx, p->rp[kL], p->ci[kL], p->rp[kU], p->ci[kU], p->rp[kLa], p->ci[kLa],
                                                     p->rp[kUa], p->ci[kUa], compact ? 1 : 0);

@@ -1010,25 +1010,24 @@ struct b200sp_spgemm_plan {
   int c_max = 0;
   int lb = 8;  // lanes walking one B row
   // device state kept for numeric
-  int *cmin = nullptr, *cmax = nullptr;
-  int* flops = nullptr;     // products per row of A*B (numeric variant 2 parks them in shared memory)
+  b200sp::DevArray<int> cmin, cmax;
+  b200sp::DevArray<int> flops;  // products per row of A*B (numeric variant 2 parks them in shared memory)
   int numeric_variant = 7;  // 7: ESC kernels (spgemm_esc.cuh) + hash kernels for long rows; 1: two-walk num_hash_kernel, 2..6: num2_kernel flavours (B200SP_SPGEMM_NUMERIC)
-  int* num_rows = nullptr;  // rows grouped by numeric bin (hash kernels): the rows beyond the ESC kernels' capacity
+  b200sp::DevArray<int> num_rows;  // rows grouped by numeric bin (hash kernels): the rows beyond the ESC kernels' capacity
   int num_off[kNumBins + 1] = {0};
-  int* all_rows = nullptr;  // every row grouped by nnz(C_i): built on demand for the hash variants and spgemm_jacobi
+  b200sp::DevArray<int> all_rows;  // every row grouped by nnz(C_i): built on demand for the hash variants and spgemm_jacobi
   int all_off[kNumBins + 1] = {0};
   bool all_built = false;
   const int* cur_rows = nullptr;  // the grouping the hash-kernel launchers read (num_rows or all_rows)
   const int* cur_off = nullptr;
-  int* esc_key = nullptr;   // per row: max(products, 2 nnz(A_i))
-  int* esc_rows = nullptr;  // rows grouped by ESC bin
+  b200sp::DevArray<int> esc_key;   // per row: max(products, 2 nnz(A_i))
+  b200sp::DevArray<int> esc_rows;  // rows grouped by ESC bin
   int esc_off[kEscBins + 3] = {0};
-  int *fb_rows = nullptr, *fb_count = nullptr;
+  b200sp::DevArray<int> fb_rows, fb_count;
   int fb_static = 0;
   int fb_log2 = 1;
-  int* fb_keys = nullptr;
-  void* fb_vals = nullptr;
-  size_t fb_vals_bytes = 0;
+  b200sp::DevArray<int> fb_keys;
+  b200sp::DevArray<char> fb_vals;
   b200sp::BspState* bsp = nullptr;  // block-row grouping of the block numeric phase (bspgemm.cu), built on first use
   b200sp::Spgemm64State* s64 = nullptr;  // a product with 64-bit offsets (spgemm64.cu): the 32-bit entries refuse the plan
 };
@@ -1036,17 +1035,13 @@ struct b200sp_spgemm_plan {
 namespace b200sp {
 
 static void spgemm_release(b200sp_spgemm_plan* p, cudaStream_t st) {
-  void* ptrs[] = {p->cmin, p->cmax, p->flops, p->num_rows, p->fb_rows, p->fb_count, p->fb_keys, p->fb_vals,
-                  p->all_rows, p->esc_key, p->esc_rows};
-  for (void* q : ptrs)
-    if (q) cudaFreeAsync(q, st);
-  p->cmin = p->cmax = p->flops = p->num_rows = p->fb_rows = p->fb_count = p->fb_keys = nullptr;
-  p->all_rows = p->esc_key = p->esc_rows = nullptr;
+  for (DevArray<int>* q : {&p->cmin, &p->cmax, &p->flops, &p->num_rows, &p->fb_rows, &p->fb_count, &p->fb_keys, &p->all_rows,
+                           &p->esc_key, &p->esc_rows})
+    q->release(st);
+  p->fb_vals.release(st);
   p->all_built = false;
   p->cur_rows = nullptr;
   p->cur_off = nullptr;
-  p->fb_vals = nullptr;
-  p->fb_vals_bytes = 0;
   bsp_state_free(p->bsp, st);
   p->bsp = nullptr;
   p->symbolic_done = false;
@@ -1205,7 +1200,7 @@ static int ensure_all_bins(b200sp_spgemm_plan* p, cudaStream_t st, const int* rp
   int *key, *d_counts;
   B200SP_CUDA_TRY(tmp.alloc(&key, p->m));
   B200SP_CUDA_TRY(tmp.alloc(&d_counts, MAXBINS));
-  if (!p->all_rows) B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->all_rows, sizeof(int) * (size_t)p->m, st));
+  if (!p->all_rows) B200SP_CUDA_TRY(p->all_rows.alloc((size_t)p->m, st));
   const int blocks = std::max(1, std::min((p->m + 255) / 256, sm_count() * 8));
   rest_key_kernel<<<blocks, 256, 0, st>>>(p->m, nullptr, 0, rpC, 1, key);
   B200SP_LAUNCH_CHECK();
@@ -1238,12 +1233,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
   B200SP_REQUIRE(rpA && ciA && vA && rpB && ciB && vB && rpC && ciC && vC, "spgemm_numeric: null pointer argument");
   // fallback scratch for values (type-dependent; keys were sized in symbolic)
   const size_t need = sizeof(S) * (size_t)kFbCtas * ((size_t)1 << p->fb_log2);
-  if (need > p->fb_vals_bytes) {
-    if (p->fb_vals) cudaFreeAsync(p->fb_vals, st);
-    p->fb_vals = nullptr;
-    B200SP_CUDA_TRY(cudaMallocAsync(&p->fb_vals, need, st));
-    p->fb_vals_bytes = need;
-  }
+  B200SP_CUDA_TRY(p->fb_vals.grow(need, st));
   // fallback list starts as the rows that are too long for shared memory
   B200SP_CUDA_TRY(cudaMemcpyAsync(p->fb_count, &p->fb_static, sizeof(int), cudaMemcpyHostToDevice, st));
   int rc;
@@ -1277,7 +1267,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
       if ((rc = launch_num<S, 128, 4096, 128, 1024>(st, p, 2, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
       if ((rc = launch_num<S, 256, 16384, 256, 4096>(st, p, 3, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
       if ((rc = launch_num<S, 512, 32768, 512, 8192>(st, p, 4, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
-      num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, (S*)p->fb_vals, rpA,
+      num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, p->fb_vals.as<S>(), rpA,
                                                       ciA, vA, rpB, ciB, vB, rpC, ciC, vC);
       B200SP_LAUNCH_CHECK();
     }
@@ -1296,7 +1286,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
     NUM6(3, 256, 16384, 256, 4096)
     NUM6(4, 512, 32768, 512, 8192)
 #undef NUM6
-    num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, (S*)p->fb_vals, rpA,
+    num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, p->fb_vals.as<S>(), rpA,
                                                     ciA, vA, rpB, ciB, vB, rpC, ciC, vC);
     B200SP_LAUNCH_CHECK();
     return B200SP_OK;
@@ -1310,7 +1300,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
     NUM5(3, 256, 16384, 256, 4096)
     NUM5(4, 512, 32768, 512, 8192)
 #undef NUM5
-    num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, (S*)p->fb_vals, rpA,
+    num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, p->fb_vals.as<S>(), rpA,
                                                     ciA, vA, rpB, ciB, vB, rpC, ciC, vC);
     B200SP_LAUNCH_CHECK();
     return B200SP_OK;
@@ -1340,7 +1330,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
       NUM2(4, 512, 32768, 512, 8192, 0)
     }
 #undef NUM2
-    num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, (S*)p->fb_vals, rpA,
+    num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, p->fb_vals.as<S>(), rpA,
                                                     ciA, vA, rpB, ciB, vB, rpC, ciC, vC);
     B200SP_LAUNCH_CHECK();
     return B200SP_OK;
@@ -1351,7 +1341,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
   if ((rc = launch_num<S, 128, 4096, 128, 1024>(st, p, 2, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
   if ((rc = launch_num<S, 256, 16384, 256, 4096>(st, p, 3, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
   if ((rc = launch_num<S, 512, 32768, 512, 8192>(st, p, 4, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
-  num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, (S*)p->fb_vals, rpA,
+  num_fallback_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, p->fb_vals.as<S>(), rpA,
                                                   ciA, vA, rpB, ciB, vB, rpC, ciC, vC);
   B200SP_LAUNCH_CHECK();
   return B200SP_OK;
@@ -1378,12 +1368,7 @@ static int jacobi_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int
   if (m == 0 || p->c_nnz == 0) return B200SP_OK;
   B200SP_REQUIRE(rpA && ciA && vA && rpB && ciB && vB && rpC && ciC && vC && dinv, "spgemm_jacobi: null pointer argument");
   const size_t need = sizeof(S) * (size_t)kFbCtas * ((size_t)1 << p->fb_log2);
-  if (need > p->fb_vals_bytes) {
-    if (p->fb_vals) cudaFreeAsync(p->fb_vals, st);
-    p->fb_vals = nullptr;
-    B200SP_CUDA_TRY(cudaMallocAsync(&p->fb_vals, need, st));
-    p->fb_vals_bytes = need;
-  }
+  B200SP_CUDA_TRY(p->fb_vals.grow(need, st));
   B200SP_CUDA_TRY(cudaMemcpyAsync(p->fb_count, &p->fb_static, sizeof(int), cudaMemcpyHostToDevice, st));
   int rc;
   if ((rc = ensure_all_bins(p, st, rpC))) return rc;
@@ -1399,7 +1384,7 @@ static int jacobi_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int
   NUMJ(3, 256, 16384, 256, 4096)
   NUMJ(4, 512, 32768, 512, 8192)
 #undef NUMJ
-  num_fallback_jacobi_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, (S*)p->fb_vals, rpA,
+  num_fallback_jacobi_kernel<S><<<kFbCtas, 256, 0, st>>>(p->fb_rows, p->fb_count, p->fb_log2, p->fb_keys, p->fb_vals.as<S>(), rpA,
                                                          ciA, vA, rpB, ciB, vB, rpC, ciC, vC, omega, dinv);
   B200SP_LAUNCH_CHECK();
   return B200SP_OK;
@@ -1470,7 +1455,7 @@ int b200sp_spgemm_symbolic_i32(b200sp_spgemm_plan* p, void* stream, int m, int n
     nnzB = last;
   }
   // numeric needs these even for empty products
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->fb_count, sizeof(int), st));
+  B200SP_CUDA_TRY(p->fb_count.alloc(1, st));
   if (m == 0 || n == 0 || k == 0 || nnzA == 0 || nnzB == 0) {
     const int blocks = std::max(1, std::min((m + 1 + 255) / 256, sm_count() * 8));
     fill_int_kernel<<<blocks, 256, 0, st>>>((int64_t)m + 1, 0, rpC);
@@ -1497,12 +1482,12 @@ int b200sp_spgemm_symbolic_i32(b200sp_spgemm_plan* p, void* stream, int m, int n
   B200SP_CUDA_TRY(tmp.alloc(&block_max, nblocks));
   B200SP_CUDA_TRY(tmp.alloc(&d_total, 1));
   B200SP_CUDA_TRY(tmp.alloc(&d_max, 1));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->cmin, sizeof(int) * (size_t)m, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->cmax, sizeof(int) * (size_t)m, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->flops, sizeof(int) * (size_t)m, st));
+  B200SP_CUDA_TRY(p->cmin.alloc((size_t)m, st));
+  B200SP_CUDA_TRY(p->cmax.alloc((size_t)m, st));
+  B200SP_CUDA_TRY(p->flops.alloc((size_t)m, st));
   int* const flops = p->flops;
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->num_rows, sizeof(int) * (size_t)m, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->fb_rows, sizeof(int) * (size_t)m, st));
+  B200SP_CUDA_TRY(p->num_rows.alloc((size_t)m, st));
+  B200SP_CUDA_TRY(p->fb_rows.alloc((size_t)m, st));
 
   // lanes per B row from B's mean row length
   {
@@ -1530,8 +1515,8 @@ int b200sp_spgemm_symbolic_i32(b200sp_spgemm_plan* p, void* stream, int m, int n
   const int lb = p->lb;
   int big_bin;
   // ESC bins (kept on the plan: the numeric phase uses the same grouping)
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->esc_key, sizeof(int) * (size_t)m, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->esc_rows, sizeof(int) * (size_t)m, st));
+  B200SP_CUDA_TRY(p->esc_key.alloc((size_t)m, st));
+  B200SP_CUDA_TRY(p->esc_rows.alloc((size_t)m, st));
   {
     const int blocks = std::max(1, std::min((m + 255) / 256, sm_count() * 8));
     esc_key_kernel<<<blocks, 256, 0, st>>>(m, flops, rpA, p->esc_key);
@@ -1659,7 +1644,7 @@ int b200sp_spgemm_symbolic_i32(b200sp_spgemm_plan* p, void* stream, int m, int n
   int lg = 1;
   while (((long long)1 << lg) < 2LL * std::max(mx, 1)) ++lg;
   p->fb_log2 = lg;
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->fb_keys, sizeof(int) * (size_t)kFbCtas * ((size_t)1 << lg), st));
+  B200SP_CUDA_TRY(p->fb_keys.alloc((size_t)kFbCtas * ((size_t)1 << lg), st));
   B200SP_CUDA_TRY(cudaStreamSynchronize(st));
   trace.mark("hash-bin grouping + scratch");
   p->symbolic_done = true;

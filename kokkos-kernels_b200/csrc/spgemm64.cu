@@ -39,8 +39,8 @@ struct Spgemm64State {
   RowWindows cut;                           // windows of A's rows, bases not rounded; cut.rel: relative row maps of A
   std::vector<int64_t> c_base;              // per window: row_ptr_C[r0]
   std::vector<b200sp_spgemm_plan*> plans;   // per window: the 32-bit product
-  int* rel_c = nullptr;  // device: relative row maps of C, laid out as cut.rel (4 B per row)
-  int* rp_b = nullptr;   // device: B's row map narrowed to int32 (4 B per row)
+  DevArray<int> rel_c;  // relative row maps of C, laid out as cut.rel (4 B per row)
+  DevArray<int> rp_b;   // B's row map narrowed to int32 (4 B per row)
 };
 
 namespace {
@@ -67,9 +67,8 @@ void release_windows(Spgemm64State* s, cudaStream_t st) {
   s->plans.clear();
   s->c_base.clear();
   s->cut.release(st);
-  for (int* q : {s->rel_c, s->rp_b})
-    if (q) cudaFreeAsync(q, st);
-  s->rel_c = s->rp_b = nullptr;
+  s->rel_c.release(st);
+  s->rp_b.release(st);
   s->done = false;
   s->c_nnz = 0;
   s->c_max = 0;
@@ -143,7 +142,7 @@ int symbolic64(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int k, cons
   B200SP_CUDA_TRY(tmp.alloc(&block_max, nblocks));
   B200SP_CUDA_TRY(tmp.alloc(&d_total, 1));
   B200SP_CUDA_TRY(tmp.alloc(&d_max, 1));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&s->rp_b, sizeof(int) * ((size_t)n + 1), st));
+  B200SP_CUDA_TRY(s->rp_b.alloc((size_t)n + 1, st));
   win64_narrow_kernel<<<grid_for((int64_t)n + 1), 256, 0, st>>>((int64_t)n + 1, rpB, s->rp_b, nullptr);
   B200SP_LAUNCH_CHECK();
   s64g_products_kernel<<<(unsigned)(((int64_t)m * 8 + 255) / 256), 256, 0, st>>>(m, rpA, ciA, s->rp_b, prod);
@@ -163,7 +162,7 @@ int symbolic64(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int k, cons
     return B200SP_ERR_OVERFLOW;
   }
   if (rc) return rc;
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&s->rel_c, sizeof(int) * (size_t)s->cut.rel_size, st));
+  B200SP_CUDA_TRY(s->rel_c.alloc((size_t)s->cut.rel_size, st));
   int64_t c_base = 0;
   int c_max = 0;
   for (const RowWindow& x : s->cut.win) {

@@ -18,22 +18,17 @@
 // binary16 (b200sp_spmm_f16_i32, spmm_impl_f16): the item, general and relayout kernels with fp32 accumulators, and an fp32
 // scratch for T/H (DESIGN.md 4.3).
 #include <limits.h>
-#include "common.cuh"
-#include "tile_ring.cuh"
-#include "spmm_items.h"
+#include "spmv_plan.h"
 #include <algorithm>
 #include <type_traits>
 #include <atomic>
 #include <stdlib.h>
 
-struct b200sp_spmv_plan;  // defined in spmv.cu
-
 namespace b200sp {
 
-// scratch owned by the plan (spmv.cu)
-int plan_mv_scratch(b200sp_spmv_plan* p, cudaStream_t st, size_t xt_bytes, size_t yt_bytes, void** xt, void** yt);
-void plan_set_last_kernel(b200sp_spmv_plan* p, const char* s);
-MMItems* plan_mm_items(b200sp_spmv_plan* p);
+static void set_last_kernel(b200sp_spmv_plan* p, const char* s) {
+  if (p) snprintf(p->last_kernel, sizeof(p->last_kernel), "%s", s);
+}
 
 // Storage type S -> accumulator type: fp32 and fp64 accumulate in their own type, binary16 (__half) in fp32.  wide() is exact;
 // narrow() rounds once, to nearest even (a result beyond the fp16 range becomes +-inf).  Kernels that serve fp16 compute in
@@ -354,7 +349,7 @@ __device__ __forceinline__ uint4 vec_pack(const __half* a) {
 // accumulates VW adjacent columns in registers: per nonzero a broadcast read of (col, val) from shared
 // memory, one gather of the X row segment (VW = 1: 4/8-byte, VW = 4/2: 16-byte loads) and VW FMAs -- no
 // shuffles, no atomics, no row bookkeeping in the inner loop, deterministic.  Rows longer than the tile
-// row limit are cut into segments (plan_analyse_mm, spmv.cu) and done by spmm_seg_kernel.
+// row limit are cut into segments (plan_analyse_mm) and done by spmm_seg_kernel.
 // ---------------------------------------------------------------------------
 template <typename S, int VW>
 struct Acc {
@@ -793,18 +788,28 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-int plan_chunk_rows(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int Q, int** chunk_row,
-                    int* n_chunks);
+// the chunk table of the plan (once per matrix and Q)
+static int chunk_table(SpmmState& mm, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int Q) {
+  const PlanKey key{row_ptr, nullptr, m, -1, nnz, Q};
+  if (mm.chunk_key == key) return B200SP_OK;
+  mm.chunk_key = PlanKey();
+  mm.n_chunks = std::max<int>(1, (int)((nnz + Q - 1) / Q));
+  B200SP_CUDA_TRY(mm.chunk_row.alloc((size_t)mm.n_chunks, st));
+  build_chunk_rows_kernel<<<(mm.n_chunks + 255) / 256, 256, 0, st>>>(m, row_ptr, mm.n_chunks, Q, mm.chunk_row);
+  B200SP_LAUNCH_CHECK();
+  mm.chunk_key = key;
+  return B200SP_OK;
+}
 
 template <typename S>
 static int launch_split(b200sp_spmv_plan* p, cudaStream_t st, int m, int k, int64_t nnz, const int* row_ptr,
                         const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta,
                         const char** name) {
   const int Q = 256;
-  int* chunk_row = nullptr;
-  int n_chunks = 0;
-  int rc = plan_chunk_rows(p, st, m, nnz, row_ptr, Q, &chunk_row, &n_chunks);
+  int rc = chunk_table(p->mm, st, m, nnz, row_ptr, Q);
   if (rc) return rc;
+  const int* chunk_row = p->mm.chunk_row;
+  const int n_chunks = p->mm.n_chunks;
   {
     const int blocks = std::max(1, std::min((m + 255) / 256, sm_count() * 8));
     spmm_prescale_split_rows<S><<<blocks, 256, 0, st>>>(m, k, Q, row_ptr, beta, Y, ldy);
@@ -868,11 +873,65 @@ static int launch_split(b200sp_spmv_plan* p, cudaStream_t st, int m, int k, int6
   return B200SP_OK;
 }
 
-int plan_analyse_mm(b200sp_spmv_plan* p, cudaStream_t st, int cap, int lmax, int seg, int m, int64_t nnz, const int* row_ptr,
-                    MMTileView* out);
+// Segments of the rows the rank-2 tile kernel leaves out (longer than LMAX): {row, first entry, end entry,
+// flags}; flags bit 0 = the row has several segments (its pieces are combined with atomics), bit 1 = first
+// segment of its row.  One thread per long row.
+__global__ void build_segments_kernel(const int* __restrict__ long_rows, const int* __restrict__ n_long,
+                                      const int* __restrict__ row_ptr, int SEG, int4* __restrict__ segs,
+                                      int* __restrict__ n_seg) {
+  const int nl = *n_long;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += gridDim.x * blockDim.x) {
+    const int r = long_rows[i];
+    const int s = row_ptr[r], e = row_ptr[r + 1];
+    const int nseg = (e - s + SEG - 1) / SEG;
+    const int base = atomicAdd(n_seg, nseg);
+    for (int q = 0; q < nseg; ++q)
+      segs[base + q] = make_int4(r, s + q * SEG, min(e, s + (q + 1) * SEG), (nseg > 1 ? 1 : 0) | (q == 0 ? 2 : 0));
+  }
+}
+
+void SpmmState::release_tiles(cudaStream_t st) {
+  tiles.release(st);
+  segs.release(st);
+  n_seg.release(st);
+  tiles_key = PlanKey();
+}
+
+void SpmmState::reset(cudaStream_t st) {
+  release_tiles(st);
+  items.release(st);
+  chunk_row.release(st);
+  n_chunks = 0;
+  chunk_key = PlanKey();
+}
+
+void SpmmState::release(cudaStream_t st) {
+  reset(st);
+  xt.release(st);
+  yt.release(st);
+}
+
+// Tile analysis of the rank-2 tile kernel: same descriptors as the rank-1 kernel's, with its own stage capacity and row
+// limit, + the segments of its long rows; cached per matrix in the plan; stream-ordered, no host synchronisation.
+static int plan_analyse_mm(SpmmState& mm, cudaStream_t st, int cap, int lmax, int seg, int m, int64_t nnz, const int* row_ptr) {
+  const PlanKey key{row_ptr, nullptr, m, -1, nnz, cap, lmax};
+  if (mm.tiles_key == key) return B200SP_OK;
+  mm.release_tiles(st);
+  const int rc = tile_analyse(st, m, nnz, row_ptr, cap, lmax, &mm.tiles);
+  if (rc != B200SP_OK) return rc;
+  const int long_cap = mm.tiles.long_cap;
+  B200SP_CUDA_TRY(mm.segs.alloc((size_t)(nnz / seg) + long_cap + 1, st));
+  B200SP_CUDA_TRY(mm.n_seg.alloc(1, st));
+  B200SP_CUDA_TRY(cudaMemsetAsync(mm.n_seg, 0, sizeof(int), st));
+  build_segments_kernel<<<std::max(1, std::min((long_cap + 255) / 256, sm_count() * 4)), 256, 0, st>>>(
+      mm.tiles.long_rows, mm.tiles.n_long, row_ptr, seg, mm.segs, mm.n_seg);
+  B200SP_LAUNCH_CHECK();
+  mm.tiles_key = key;
+  return B200SP_OK;
+}
 
 template <typename S, int VW, int KTL, int NW, int STAGES, int CAP, int UNR>
-static int launch_mm_tile_k(cudaStream_t st, const MMTileView& tv, int m, int k, int64_t nnz, const int* row_ptr,
+static int launch_mm_tile_k(cudaStream_t st, const TileAnalysis& tv, int m, int k, int64_t nnz, const int* row_ptr,
                             const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
   using Ring = CsrTileRing<S, CAP, STAGES>;
   auto kern = spmm_tile_kernel<S, VW, KTL, NW, STAGES, CAP, UNR>;
@@ -891,7 +950,7 @@ static int launch_mm_tile_k(cudaStream_t st, const MMTileView& tv, int m, int k,
 // (B200SP_SPMM_CFG, tuning sweeps): 1 = small ring (8 consumer warps, 1024-entry stages: 5 CTAs per SM for fp32),
 // 2 = default ring with twice the gathers in flight per lane, 3 = small ring with 16 consumer warps.
 template <typename S, int VW, int KTL>
-static int launch_mm_tile_cfg(int cfg, cudaStream_t st, const MMTileView& tv, int m, int k, int64_t nnz, const int* row_ptr,
+static int launch_mm_tile_cfg(int cfg, cudaStream_t st, const TileAnalysis& tv, int m, int k, int64_t nnz, const int* row_ptr,
                               const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
   if constexpr (VW > 1) {
     switch (cfg) {
@@ -918,9 +977,11 @@ static int launch_mm_tile(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m,
     const int v = atoi(e);
     if (v >= 16 && v <= 512) LMAX = v;
   }
-  MMTileView tv;
-  int rc = plan_analyse_mm(p, st, CAP, LMAX, SEG, m, nnz, row_ptr, &tv);
+  int rc = plan_analyse_mm(p->mm, st, CAP, LMAX, SEG, m, nnz, row_ptr);
   if (rc) return rc;
+  const TileAnalysis& tv = p->mm.tiles;
+  const int4* segs = p->mm.segs;
+  const int* n_seg = p->mm.n_seg;
   constexpr int W = VecOf<S>::W;
   const int lanes_needed = vec ? (k + W - 1) / W : k;
   int KTL = 1;
@@ -942,7 +1003,7 @@ static int launch_mm_tile(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m,
   if (rc) return rc;
   // long rows: segments of <= SEG entries, one CTA each
   const int grid = sm_count() * 4;
-  spmm_seg_prescale_kernel<S><<<grid, 256, 0, st>>>(tv.segs, tv.n_seg, k, beta, Y, ldy);
+  spmm_seg_prescale_kernel<S><<<grid, 256, 0, st>>>(segs, n_seg, k, beta, Y, ldy);
   B200SP_LAUNCH_CHECK();
   *name = vec ? "tile_vec" : "tile";
   if (vec) {
@@ -951,7 +1012,7 @@ static int launch_mm_tile(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m,
       *name = "tile_vec+seg_vec";
 #define B200SP_SEGV(L)                                                                                               \
   case L:                                                                                                            \
-    spmm_seg_vec_kernel<S, L><<<grid, 256, 0, st>>>(tv.segs, tv.n_seg, k, col_idx, vals, X, ldx, Y, ldy, alpha, beta); \
+    spmm_seg_vec_kernel<S, L><<<grid, 256, 0, st>>>(segs, n_seg, k, col_idx, vals, X, ldx, Y, ldy, alpha, beta); \
     break;
       switch (KTL) {
         B200SP_SEGV(1) B200SP_SEGV(2) B200SP_SEGV(4) B200SP_SEGV(8) B200SP_SEGV(16) B200SP_SEGV(32)
@@ -965,7 +1026,7 @@ static int launch_mm_tile(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m,
   while (KT < k && KT < 32) KT <<= 1;
 #define B200SP_SEG(K)                                                                                              \
   case K:                                                                                                          \
-    spmm_seg_kernel<S, K><<<grid, 256, 0, st>>>(tv.segs, tv.n_seg, k, col_idx, vals, X, ldx, Y, ldy, alpha, beta); \
+    spmm_seg_kernel<S, K><<<grid, 256, 0, st>>>(segs, n_seg, k, col_idx, vals, X, ldx, Y, ldy, alpha, beta); \
     break;
   switch (KT) {
     B200SP_SEG(1) B200SP_SEG(2) B200SP_SEG(4) B200SP_SEG(8) B200SP_SEG(16) B200SP_SEG(32)
@@ -978,7 +1039,7 @@ static int launch_mm_tile(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m,
 // ---------------------------------------------------------------------------
 // Item kernel (default for row-major X and Y with a plan; B200SP_SPMM_KERNEL=items): the gather-bound formulation.
 // On power-law matrices the tile kernel's row groups of one warp run loops of very different lengths and wait for
-// the longest; here the unit of work is an ITEM -- a run of <= LMAX consecutive entries of one row (spmm_items.h) --
+// the longest; here the unit of work is an ITEM -- a run of <= LMAX consecutive entries of one row (MMItems, spmv_plan.h) --
 // and the items are sorted by length, longest first.  A group of KTL lanes (VW adjacent columns each, one 16-byte
 // load of the X row segment per lane and entry) owns one item, so the 32/KTL groups of a warp run loops of equal
 // length with 4 independent gathers in flight per lane, nothing waits, and the long items are scheduled first.
@@ -1057,14 +1118,10 @@ __global__ void __launch_bounds__(256) mmi_fill_kernel(int m, const int* __restr
   }
 }
 
-static int plan_analyse_items(b200sp_spmv_plan* p, cudaStream_t st, int lmax, int m, int64_t nnz, const int* row_ptr, MMItems** out) {
-  MMItems* mi = plan_mm_items(p);
-  *out = mi;
-  if (mi->items && mi->key_row_ptr == row_ptr && mi->key_m == m && mi->key_nnz == nnz && mi->key_lmax == lmax) return B200SP_OK;
-  void* old[] = {mi->items, mi->multi, mi->partial};
-  for (void* q : old)
-    if (q) cudaFreeAsync(q, st);
-  *mi = MMItems();
+static int plan_analyse_items(MMItems* mi, cudaStream_t st, int lmax, int m, int64_t nnz, const int* row_ptr) {
+  const PlanKey key{row_ptr, nullptr, m, -1, nnz, lmax};
+  if (mi->key == key) return B200SP_OK;
+  mi->release(st);
   DevTmp tmp(st);
   int *hist, *counters;
   B200SP_CUDA_TRY(tmp.alloc(&hist, lmax + 1));
@@ -1090,16 +1147,13 @@ static int plan_analyse_items(b200sp_spmv_plan* p, cudaStream_t st, int lmax, in
   mi->n_multi_long = h_cnt[4];
   mi->n_partial = h_cnt[1];
   mi->lmax = lmax;
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&mi->items, sizeof(int4) * (size_t)std::max(mi->n_items, 1), st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&mi->multi, sizeof(int4) * (size_t)std::max(mi->n_multi, 1), st));
+  B200SP_CUDA_TRY(mi->items.alloc((size_t)std::max(mi->n_items, 1), st));
+  B200SP_CUDA_TRY(mi->multi.alloc((size_t)std::max(mi->n_multi, 1), st));
   B200SP_CUDA_TRY(cudaMemcpyAsync(hist, h_cur, sizeof(int) * (size_t)(lmax + 1), cudaMemcpyHostToDevice, st));
   mmi_fill_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, lmax, hist, counters, mi->items, mi->multi, mi->n_multi);
   B200SP_LAUNCH_CHECK();
   B200SP_CUDA_TRY(cudaStreamSynchronize(st));  // h_cur is pageable host memory: consumed before it goes out of scope
-  mi->key_row_ptr = row_ptr;
-  mi->key_m = m;
-  mi->key_nnz = nnz;
-  mi->key_lmax = lmax;
+  mi->key = key;
   return B200SP_OK;
 }
 
@@ -1380,17 +1434,10 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
     const int v = atoi(e);
     if (v >= 16 && v <= MMI_MAXL) LMAX = v;
   }
-  MMItems* mi;
-  int rc = plan_analyse_items(p, st, LMAX, m, nnz, row_ptr, &mi);
+  MMItems* mi = &p->mm.items;
+  int rc = plan_analyse_items(mi, st, LMAX, m, nnz, row_ptr);
   if (rc) return rc;
-  const size_t need = sizeof(A) * (size_t)mi->n_partial * (size_t)k;
-  if (need > mi->partial_bytes) {
-    if (mi->partial) cudaFreeAsync(mi->partial, st);
-    mi->partial = nullptr;
-    mi->partial_bytes = 0;
-    B200SP_CUDA_TRY(cudaMallocAsync(&mi->partial, need, st));
-    mi->partial_bytes = need;
-  }
+  B200SP_CUDA_TRY(mi->partial.grow(sizeof(A) * (size_t)mi->n_partial * (size_t)k, st));
   constexpr int W = VecOf<S>::W;
   const int lanes_needed = vec ? (k + W - 1) / W : k;
   int KTL = 1;
@@ -1406,13 +1453,13 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   case L:                                                                                                                  \
     if (coop == 8)                                                                                                         \
       spmm_item_coop_kernel<S, V, L, 8><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,    \
-                                                              (A*)mi->partial, alpha, beta);                               \
+                                                              mi->partial.as<A>(), alpha, beta);                               \
     else if (coop == 4)                                                                                                    \
       spmm_item_coop_kernel<S, V, L, 4><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,    \
-                                                              (A*)mi->partial, alpha, beta);                               \
+                                                              mi->partial.as<A>(), alpha, beta);                               \
     else                                                                                                                   \
       spmm_item_kernel<S, V, L><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,            \
-                                                      (A*)mi->partial, alpha, beta);                                       \
+                                                      mi->partial.as<A>(), alpha, beta);                                       \
     break;
     if (vec) {
       switch (KTL) { B200SP_MMI(W, 1) B200SP_MMI(W, 2) B200SP_MMI(W, 4) B200SP_MMI(W, 8) B200SP_MMI(W, 16) B200SP_MMI(W, 32) }
@@ -1425,12 +1472,12 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   const int n_short = mi->n_multi - mi->n_multi_long;
   if (n_short > 0) {
     const int g = (int)std::min<int64_t>(((int64_t)n_short + 7) / 8, (int64_t)sm_count() * 16);  // a warp per row
-    spmm_item_reduce_kernel<S><<<std::max(g, 1), 256, 0, st>>>(n_short, mi->multi, k, (const A*)mi->partial, Y, ldy, alpha, beta);
+    spmm_item_reduce_kernel<S><<<std::max(g, 1), 256, 0, st>>>(n_short, mi->multi, k, mi->partial.as<const A>(), Y, ldy, alpha, beta);
     B200SP_LAUNCH_CHECK();
   }
   if (mi->n_multi_long > 0) {
     const int g = std::min(mi->n_multi_long, sm_count() * 8);  // a CTA per row
-    spmm_item_reduce_long_kernel<S><<<g, 256, 0, st>>>(mi->n_multi_long, mi->multi + n_short, k, (const A*)mi->partial, Y, ldy, alpha, beta);
+    spmm_item_reduce_long_kernel<S><<<g, 256, 0, st>>>(mi->n_multi_long, mi->multi + n_short, k, mi->partial.as<const A>(), Y, ldy, alpha, beta);
     B200SP_LAUNCH_CHECK();
   }
   return B200SP_OK;
@@ -1491,7 +1538,7 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
     const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
     spmm_transpose_kernel<S><<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, Y, yr, yc, alpha);
     B200SP_LAUNCH_CHECK();
-    plan_set_last_kernel(p, "spmm_transpose");
+    set_last_kernel(p, "spmm_transpose");
     return B200SP_OK;
   }
   const bool split = use_split_kernel(p);
@@ -1500,7 +1547,7 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
     if (choice == 4) {
       constexpr int W = VecOf<S>::W;
       const bool vec = (k % W == 0) && (ldx % W == 0) && (ldy % W == 0) && ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0;
-      plan_set_last_kernel(p, vec ? "spmm_items_vec" : "spmm_items");
+      set_last_kernel(p, vec ? "spmm_items_vec" : "spmm_items");
       return launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
     }
     const char* name = "rowmajor";
@@ -1517,30 +1564,30 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
     if (rc) return rc;
     char label[48];
     snprintf(label, sizeof(label), "spmm_%s", name);
-    plan_set_last_kernel(p, label);
+    set_last_kernel(p, label);
     return B200SP_OK;
   }
   // LayoutLeft operands: with a plan and k >= 4, relayout to row-major scratch and use the row-major kernel
   if (p && k >= 4) {
-    void *xt = nullptr, *yt = nullptr;
-    const size_t xtb = xrm ? 0 : sizeof(S) * (size_t)xrows * k;
-    const size_t ytb = yrm ? 0 : sizeof(S) * (size_t)yrows * k;
-    int rc = plan_mv_scratch(p, st, xtb, ytb, &xt, &yt);
-    if (rc) return rc;
+    B200SP_CUDA_TRY(p->mm.xt.grow(xrm ? 0 : sizeof(S) * (size_t)xrows * k, st));
+    B200SP_CUDA_TRY(p->mm.yt.grow(yrm ? 0 : sizeof(S) * (size_t)yrows * k, st));
+    S* xt = p->mm.xt.as<S>();
+    S* yt = p->mm.yt.as<S>();
+    int rc;
     const int tb = 256;
     auto rl_grid = [](int64_t rows) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>((rows + 127) / 128, (int64_t)sm_count() * 16)); };
     const S* Xr = X;
     int64_t ldxr = ldx;
     if (!xrm) {
-      relayout_kernel<S, true><<<rl_grid(xrows), tb, 0, st>>>(xrows, k, (S*)xt, X, nullptr, xr, xc);
+      relayout_kernel<S, true><<<rl_grid(xrows), tb, 0, st>>>(xrows, k, xt, X, nullptr, xr, xc);
       B200SP_LAUNCH_CHECK();
-      Xr = (const S*)xt;
+      Xr = xt;
       ldxr = k;
     }
     S* Yr = Y;
     int64_t ldyr = ldy;
     if (!yrm) {
-      Yr = (S*)yt;
+      Yr = yt;
       ldyr = k;
       if (beta != S(0)) {
         relayout_kernel<S, true><<<rl_grid(yrows), tb, 0, st>>>(yrows, k, Yr, Y, nullptr, yr, yc);
@@ -1568,13 +1615,13 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
     }
     char label[48];
     snprintf(label, sizeof(label), "spmm_relayout+%s", name);
-    plan_set_last_kernel(p, label);
+    set_last_kernel(p, label);
     return B200SP_OK;
   }
   const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
   spmm_general_kernel<S><<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, Y, yr, yc, alpha, beta);
   B200SP_LAUNCH_CHECK();
-  plan_set_last_kernel(p, "spmm_general");
+  set_last_kernel(p, "spmm_general");
   return B200SP_OK;
 }
 
@@ -1612,9 +1659,8 @@ static int spmm_impl_f16(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m,
     float* acc = nullptr;
     const size_t acc_bytes = sizeof(float) * (size_t)yrows * (size_t)k;
     if (p) {
-      void *unused = nullptr, *yt = nullptr;
-      if (int rc = plan_mv_scratch(p, st, 0, acc_bytes, &unused, &yt)) return rc;
-      acc = (float*)yt;
+      B200SP_CUDA_TRY(p->mm.yt.grow(acc_bytes, st));
+      acc = p->mm.yt.as<float>();
     } else {
       B200SP_CUDA_TRY(tmp.alloc(&acc, (size_t)yrows * (size_t)k));
     }
@@ -1624,33 +1670,33 @@ static int spmm_impl_f16(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m,
     B200SP_LAUNCH_CHECK();
     spmm_acc_epilogue_kernel<<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, acc, alpha, beta, Y, yr, yc);
     B200SP_LAUNCH_CHECK();
-    plan_set_last_kernel(p, "spmm_transpose");
+    set_last_kernel(p, "spmm_transpose");
     return B200SP_OK;
   }
   constexpr int W = VecOf<S>::W;
   if (p && xrm && yrm) {
     const bool vec = (k % W == 0) && (ldx % W == 0) && (ldy % W == 0) && ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0;
-    plan_set_last_kernel(p, vec ? "spmm_items_vec" : "spmm_items");
+    set_last_kernel(p, vec ? "spmm_items_vec" : "spmm_items");
     return launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
   }
   if (p && k >= 4) {  // LayoutLeft operands: row-major copies in the plan's scratch, as for fp32
-    void *xt = nullptr, *yt = nullptr;
-    const size_t xtb = xrm ? 0 : sizeof(S) * (size_t)xrows * k;
-    const size_t ytb = yrm ? 0 : sizeof(S) * (size_t)yrows * k;
-    if (int rc = plan_mv_scratch(p, st, xtb, ytb, &xt, &yt)) return rc;
+    B200SP_CUDA_TRY(p->mm.xt.grow(xrm ? 0 : sizeof(S) * (size_t)xrows * k, st));
+    B200SP_CUDA_TRY(p->mm.yt.grow(yrm ? 0 : sizeof(S) * (size_t)yrows * k, st));
+    S* xt = p->mm.xt.as<S>();
+    S* yt = p->mm.yt.as<S>();
     auto rl_grid = [](int64_t rows) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>((rows + 127) / 128, (int64_t)sm_count() * 16)); };
     const S* Xr = X;
     int64_t ldxr = ldx;
     if (!xrm) {
-      relayout_kernel<S, true><<<rl_grid(xrows), 256, 0, st>>>(xrows, k, (S*)xt, X, nullptr, xr, xc);
+      relayout_kernel<S, true><<<rl_grid(xrows), 256, 0, st>>>(xrows, k, xt, X, nullptr, xr, xc);
       B200SP_LAUNCH_CHECK();
-      Xr = (const S*)xt;
+      Xr = xt;
       ldxr = k;
     }
     S* Yr = Y;
     int64_t ldyr = ldy;
     if (!yrm) {
-      Yr = (S*)yt;
+      Yr = yt;
       ldyr = k;
       if (beta != 0.0f) {
         relayout_kernel<S, true><<<rl_grid(yrows), 256, 0, st>>>(yrows, k, Yr, Y, nullptr, yr, yc);
@@ -1663,13 +1709,13 @@ static int spmm_impl_f16(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m,
       relayout_kernel<S, false><<<rl_grid(yrows), 256, 0, st>>>(yrows, k, Yr, nullptr, Y, yr, yc);
       B200SP_LAUNCH_CHECK();
     }
-    plan_set_last_kernel(p, "spmm_relayout+items");
+    set_last_kernel(p, "spmm_relayout+items");
     return B200SP_OK;
   }
   const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
   spmm_general_kernel<S><<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, Y, yr, yc, alpha, beta);
   B200SP_LAUNCH_CHECK();
-  plan_set_last_kernel(p, "spmm_general");
+  set_last_kernel(p, "spmm_general");
   return B200SP_OK;
 }
 

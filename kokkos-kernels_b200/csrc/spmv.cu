@@ -23,8 +23,7 @@
 //                       inputs): sub-warp per row straight from global memory.
 //   spmv_transpose_kernel  T/H modes: y pre-scaled, atomicAdd scatter.
 #include "common.cuh"
-#include "tile_ring.cuh"
-#include "spmm_items.h"
+#include "spmv_plan.h"
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
@@ -115,12 +114,6 @@ __device__ __forceinline__ S subwarp_sum(S v) {
   for (int o = LPR / 2; o > 0; o >>= 1) v += shfl_xor(v, o);
   return v;
 }
-
-// extra destinations of y: peer GPUs' x buffers (fused all-gather over NVLink, DESIGN.md section 6)
-struct YExtra {
-  void* p[7];
-  int n;
-};
 
 // ex.n > 0: every value is also stored to ex.n further destinations (P2P mappings of the peers' buffers, or one NVSwitch
 // multicast mapping).  ex.n < 0 ("forward", one destination ex.p[0]) is seen by the forwarding form of the tiled kernel only,
@@ -365,14 +358,13 @@ __global__ void find_long_rows_kernel(int m, const int* __restrict__ row_ptr, in
 // The tiles and long rows of the tile kernels (spmv_tile_kernel, spmm_tile_kernel, the BSR ones of bsr.cu with blocks for
 // entries) for a stage of cap entries and a row limit of lmax.  *out owns what it allocated, also on an error.
 int tile_analyse(cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int cap, int lmax, TileAnalysis* out) {
-  *out = TileAnalysis();
   out->LMAX = lmax;
   out->T = cap - lmax - 8;
   out->n_tiles = (int)(nnz / out->T) + 1;
   out->long_cap = (int)(nnz / (lmax + 1)) + 1;  // every long row holds more than lmax entries
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&out->tiles, sizeof(int4) * (size_t)out->n_tiles, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&out->long_rows, sizeof(int) * (size_t)out->long_cap, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&out->n_long, sizeof(int), st));
+  B200SP_CUDA_TRY(out->tiles.alloc((size_t)out->n_tiles, st));
+  B200SP_CUDA_TRY(out->long_rows.alloc((size_t)out->long_cap, st));
+  B200SP_CUDA_TRY(out->n_long.alloc(1, st));
   B200SP_CUDA_TRY(cudaMemsetAsync(out->n_long, 0, sizeof(int), st));
   build_tiles_kernel<<<(out->n_tiles + 255) / 256, 256, 0, st>>>(m, row_ptr, out->n_tiles, out->T, cap, out->tiles);
   B200SP_LAUNCH_CHECK();
@@ -545,10 +537,6 @@ __global__ void pattern_assign_kernel(int m, const int* __restrict__ row_ptr, co
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ int64_t dmin64(int64_t a, int64_t b) { return a < b ? a : b; }
 __device__ __forceinline__ int64_t dmax64(int64_t a, int64_t b) { return a > b ? a : b; }
-
-// which columns the tiled kernel reads: col_idx, the plan's 16-bit deltas + anchors (section 3.5), or its pattern starts +
-// anchors + dictionary (section 3.6)
-enum TileCols { COLS_I32 = 0, COLS_DELTA = 1, COLS_PAT = 2 };
 
 // The pattern form's layout, for every configuration (DESIGN.md sections 3.6 and 7): stages of PAT_CAP entries with PAT_RCAP
 // row slots, two CTAs of 16 consumer warps per SM in f64.  The form streams no per-entry columns, so a stage holds only values
@@ -955,205 +943,30 @@ __global__ void __launch_bounds__(128, 16) peer_push_sm_kernel(const double* __r
 
 using namespace b200sp;
 
-struct b200sp_spmv_plan {
-  int algo = B200SP_SPMV_DEFAULT;
-  // tuning overrides (-1 = auto)
-  int cfg = -1, lpr = -1, ctas_per_sm = -1;
-  // cache key of the analysed matrix
-  const int* key_row_ptr = nullptr;
-  int key_m = -1, key_n = -1;
-  int64_t key_nnz = -1;
-  int key_cfg = -1;
-  // analysis products (device)
-  int4* tiles = nullptr;
-  int n_tiles = 0;
-  int T = 0, LMAX = 0;
-  int* long_rows = nullptr;
-  int* n_long = nullptr;       // device counter
-  int* n_long_host = nullptr;  // pinned mirror, valid once n_long_event completed
-  cudaEvent_t n_long_event = nullptr;
-  bool n_long_known = false;
-  int long_cap = 0;
-  // 16-bit column form of the tiled kernel (build_idx16_kernel, DESIGN.md section 3.5), keyed on col_idx on top of the
-  // analysis key and released with the analysis.  Calls use it once the flag, fetched without a host synchronisation like
-  // n_long, says that the matrix qualifies (idx16_state 1); until then, and for a matrix that does not, the 32-bit columns.
-  // The pattern form (pattern_*_kernel, section 3.6) is built in the same call and its verdict comes with the same event;
-  // once it is chosen the deltas are released.
-  uint16_t* idx16_d = nullptr;     // nnz deltas, padded to a multiple of 8 entries
-  int* idx16_anchor = nullptr;     // m anchors, padded to a multiple of 4 rows
-  uint16_t* pat_pid = nullptr;     // m pattern starts, padded to a multiple of 8 rows
-  int* pat_dict = nullptr;         // DCAP offsets + the used length
-  int4* pat_tiles = nullptr;       // the pattern form's tiles (PAT_TILE_CAP entries, the cfg's LMAX), built with its verdict
-  int pat_n_tiles = 0;
-  int* idx16_bad = nullptr;        // device flags: [0] deltas, [1] patterns
-  int* idx16_bad_host = nullptr;   // pinned mirror, valid once idx16_event completed
-  cudaEvent_t idx16_event = nullptr;
-  const int* idx16_key_ci = nullptr;  // col_idx the state below belongs to
-  int idx16_state = 0;                // -1: verdict pending, else the TileCols of the matrix
-  int cols_launch = COLS_I32;         // the current call's tiled launch takes this form
-  // host-vector staging (b200sp_spmv_hostvec_*)
-  void* dx = nullptr;
-  void* dy = nullptr;
-  size_t dx_bytes = 0, dy_bytes = 0;
-  // rank-2 scratch (spmm.cu)
-  void* xt = nullptr;
-  void* yt = nullptr;
-  size_t xt_bytes = 0, yt_bytes = 0;
-  // nnz-chunk -> row table of the split SpMM kernel
-  int* chunk_row = nullptr;
-  int n_chunks = 0, chunk_q = 0;
-  const int* chunk_key = nullptr;
-  int chunk_m = -1;
-  int64_t chunk_nnz = -1;
-  // adaptive row splitting of the long rows (B200SP_SPMV_LONGROWS=seg): segments, per-row (first segment, count), partial sums
-  int4* r1_segs = nullptr;
-  int* r1_n_seg = nullptr;
-  int2* r1_row_seg = nullptr;
-  void* r1_partial = nullptr;
-  int r1_seg_cap = 0;
-  bool r1_built = false;
-  // rank-2 tile kernel (spmm.cu): its own tile analysis (smaller row limit) + segment list of the long rows
-  int4* mm_tiles = nullptr;
-  int mm_n_tiles = 0, mm_T = 0, mm_LMAX = 0, mm_cap = 0;
-  int* mm_long_rows = nullptr;
-  int* mm_n_long = nullptr;
-  int4* mm_segs = nullptr;
-  int* mm_n_seg = nullptr;
-  int mm_seg_cap = 0;
-  const int* mm_key_row_ptr = nullptr;
-  int mm_key_m = -1, mm_key_cap = -1, mm_key_lmax = -1;
-  int64_t mm_key_nnz = -1;
-  // rank-2 item kernel (spmm.cu, spmm_items.h): length-sorted work items
-  b200sp::MMItems mmi;
-  // cached transpose (B200SP_SPMV_OPT_CACHE_TRANSPOSE): structure of A^T + source entry of each of its entries,
-  // values re-gathered on every call (they may have changed in place), and a plan of its own for A^T
-  bool cache_transpose = false;
-  int *t_rp = nullptr, *t_ci = nullptr, *t_src = nullptr;
-  void* t_vals = nullptr;
-  size_t t_vals_bytes = 0;
-  const int *t_key_rp = nullptr, *t_key_ci = nullptr;
-  int t_key_m = -1, t_key_n = -1;
-  int64_t t_key_nnz = -1;
-  b200sp_spmv_plan* tplan = nullptr;
-  char last_kernel[160] = "none";
-  b200sp::YExtra extra = {{nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, 0};
-  // self-tuning between the tiled and the row-vector kernel (same bits, different speed by matrix):
-  // call 0 tile, call 1 tile timed, call 2 vector timed, then the faster one (DESIGN.md section 3.3)
-  int at_calls = 0, at_choice = -1;
-  cudaEvent_t at_ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  float at_tile_ms = 0.f, at_vec_ms = 0.f;
-  // tile sub-range of the next tiled launch (host-vector pipeline computes y piece by piece); hi < 0 = all
-  int range_lo = 0, range_hi = -1;
-  // host-vector pipeline (b200sp_spmv_hostvec_*): double-buffered device x / y, copy streams, events
-  struct HostPipe {
-    bool init = false;
-    cudaStream_t sH = nullptr, sD = nullptr;
-    void* dx[2] = {nullptr, nullptr};
-    void* dy[2] = {nullptr, nullptr};
-    size_t xb = 0, yb = 0;
-    cudaEvent_t ev_x[2], ev_c[2], ev_done[2], ev_chunk[8];
-    unsigned long long call = 0;
-    int nc = 0;
-    int tile_b[9];
-    int row_b[9];
-    const int* key = nullptr;
-    int key_cfg = -1, key_m = -1;
-    int64_t key_nnz = -1;
-    const void* key_tiles = nullptr;  // the tile table the piece bounds were cut from
-    bool defer = false;  // B200SP_SPMV_OPT_HOSTVEC_DEFER: `stream` does not wait for a call's download before the next call computes
-    int last_b = -1;     // buffer of the latest call whose download `stream` has not been made to wait for
-  } pipe;
-};
-
 namespace b200sp {
 
-static void plan_release_idx16_arrays(b200sp_spmv_plan* p, cudaStream_t st) {
-  void* ptrs[] = {p->idx16_d, p->idx16_anchor, p->pat_pid, p->pat_dict, p->idx16_bad};
-  for (void* q : ptrs)
-    if (q) cudaFreeAsync(q, st);
-  p->idx16_d = nullptr;
-  p->idx16_anchor = nullptr;
-  p->pat_pid = nullptr;
-  p->pat_dict = nullptr;
-  p->idx16_bad = nullptr;
-  if (p->pat_tiles) cudaFreeAsync(p->pat_tiles, st);
-  p->pat_tiles = nullptr;
-  p->pat_n_tiles = 0;
+// what plan_analyse builds and b200sp_spmv_plan_invalidate drops: the tiles, the column forms and the long-row segments
+static void plan_reset_analysis(b200sp_spmv_plan* p, cudaStream_t st) {
+  p->r1.reset(st);
+  p->cols.reset(st);
+  p->segs.release(st);
 }
-
-static void plan_release_analysis(b200sp_spmv_plan* p, cudaStream_t st) {
-  plan_release_idx16_arrays(p, st);
-  p->idx16_key_ci = nullptr;
-  p->idx16_state = 0;
-  if (p->tiles) cudaFreeAsync(p->tiles, st);
-  if (p->long_rows) cudaFreeAsync(p->long_rows, st);
-  if (p->n_long) cudaFreeAsync(p->n_long, st);
-  if (p->r1_segs) cudaFreeAsync(p->r1_segs, st);
-  if (p->r1_n_seg) cudaFreeAsync(p->r1_n_seg, st);
-  if (p->r1_row_seg) cudaFreeAsync(p->r1_row_seg, st);
-  if (p->r1_partial) cudaFreeAsync(p->r1_partial, st);
-  p->r1_segs = nullptr;
-  p->r1_n_seg = nullptr;
-  p->r1_row_seg = nullptr;
-  p->r1_partial = nullptr;
-  p->r1_built = false;
-  p->tiles = nullptr;
-  p->long_rows = nullptr;
-  p->n_long = nullptr;
-  p->n_tiles = 0;
-  p->n_long_known = false;
-  p->key_row_ptr = nullptr;
-}
-
-static void plan_release_mm(b200sp_spmv_plan* p, cudaStream_t st) {
-  void* ptrs[] = {p->mm_tiles, p->mm_long_rows, p->mm_n_long, p->mm_segs, p->mm_n_seg};
-  for (void* q : ptrs)
-    if (q) cudaFreeAsync(q, st);
-  p->mm_tiles = nullptr;
-  p->mm_long_rows = nullptr;
-  p->mm_n_long = nullptr;
-  p->mm_segs = nullptr;
-  p->mm_n_seg = nullptr;
-  p->mm_key_row_ptr = nullptr;
-  void* iptrs[] = {p->mmi.items, p->mmi.multi, p->mmi.partial};
-  for (void* q : iptrs)
-    if (q) cudaFreeAsync(q, st);
-  p->mmi = b200sp::MMItems();
-}
-
-b200sp::MMItems* plan_mm_items(b200sp_spmv_plan* p) { return &p->mmi; }
 
 template <typename S>
 static int plan_analyse(b200sp_spmv_plan* p, cudaStream_t st, int cfg, int m, int n, int64_t nnz,
                         const int* row_ptr) {
-  if (p->key_row_ptr == row_ptr && p->key_m == m && p->key_n == n && p->key_nnz == nnz &&
-      p->key_cfg == cfg && p->long_rows)
-    return B200SP_OK;
-  plan_release_analysis(p, st);
+  const PlanKey key{row_ptr, nullptr, m, n, nnz, cfg};
+  if (p->r1.key == key) return B200SP_OK;
+  plan_reset_analysis(p, st);
   const TileCfg c = kCfgs[cfg];
   TileAnalysis a;
   const int rc = tile_analyse(st, m, nnz, row_ptr, c.cap, c.cap / 4, &a);
-  p->tiles = a.tiles;
-  p->n_tiles = a.n_tiles;
-  p->T = a.T;
-  p->LMAX = a.LMAX;
-  p->long_rows = a.long_rows;
-  p->n_long = a.n_long;
-  p->long_cap = a.long_cap;
+  p->r1.a = std::move(a);
+  p->r1.cut = ++p->cuts;
   if (rc != B200SP_OK) return rc;
-  if (!p->n_long_host) B200SP_CUDA_TRY(cudaMallocHost((void**)&p->n_long_host, sizeof(int)));
-  if (!p->n_long_event) B200SP_CUDA_TRY(cudaEventCreateWithFlags(&p->n_long_event, cudaEventDisableTiming));
-  *p->n_long_host = -1;
-  B200SP_CUDA_TRY(cudaMemcpyAsync(p->n_long_host, p->n_long, sizeof(int), cudaMemcpyDeviceToHost, st));
-  B200SP_CUDA_TRY(cudaEventRecord(p->n_long_event, st));
-  p->n_long_known = false;
-  p->key_row_ptr = row_ptr;
-  p->key_m = m;
-  p->key_n = n;
-  p->key_nnz = nnz;
-  p->key_cfg = cfg;
-  p->at_calls = 0;
-  p->at_choice = -1;
+  if (int rc2 = p->r1.n_long.fetch(p->r1.a.n_long, 1, st)) return rc2;
+  p->r1.key = key;
+  p->at.reset();
   return B200SP_OK;
 }
 
@@ -1163,38 +976,34 @@ static int plan_analyse(b200sp_spmv_plan* p, cudaStream_t st, int cfg, int m, in
 // matrix qualifies for both.  A matrix that qualifies for neither, or whose streams do not fit in device memory, keeps the
 // 32-bit columns: the call does not fail.  B200SP_SPMV_PATTERN=0 at the build leaves out the pattern analysis.
 static int plan_idx16(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, const int* col_idx) {
+  SpmvCols& c = p->cols;
+  const int LMAX = p->r1.a.LMAX;
   // the deltas of a pattern-form matrix go on the call after the one that learnt the verdict: a call never frees the streams
   // it has built, so what a handle holds after its first call does not depend on how soon the verdict arrived
-  if (p->idx16_state == COLS_PAT && p->idx16_d) {
-    cudaFreeAsync(p->idx16_d, st);
-    p->idx16_d = nullptr;
-  }
-  if (p->idx16_key_ci != col_idx) {
-    plan_release_idx16_arrays(p, st);
-    p->idx16_key_ci = col_idx;
-    p->idx16_state = COLS_I32;
+  if (c.state == COLS_PAT) c.d.release(st);
+  if (c.key_ci != col_idx) {
+    c.release_streams(st);
+    c.key_ci = col_idx;
+    c.state = COLS_I32;
     const char* pe = getenv("B200SP_SPMV_PATTERN");
     const bool pat = !(pe && pe[0] == '0');
     const size_t nd = ((size_t)nnz + 7) & ~(size_t)7, na = ((size_t)m + 3) & ~(size_t)3, np = ((size_t)m + 7) & ~(size_t)7;
     // hash table, slot representatives, slot starts, slot lengths, row slots: freed once the pattern passes are issued
     const size_t scratch = sizeof(unsigned long long) * PAT_SLOTS + sizeof(int) * (3 * (size_t)PAT_SLOTS + (size_t)m);
     unsigned long long* table = nullptr;
-    if (cudaMallocAsync((void**)&p->idx16_d, sizeof(uint16_t) * nd, st) != cudaSuccess ||
-        cudaMallocAsync((void**)&p->idx16_anchor, sizeof(int) * na, st) != cudaSuccess ||
-        cudaMallocAsync((void**)&p->idx16_bad, 2 * sizeof(int), st) != cudaSuccess ||
-        (pat && (cudaMallocAsync((void**)&p->pat_pid, sizeof(uint16_t) * np, st) != cudaSuccess ||
-                 cudaMallocAsync((void**)&p->pat_dict, sizeof(int) * (DCAP + 1), st) != cudaSuccess ||
+    if (c.d.alloc(nd, st) != cudaSuccess || c.anchor.alloc(na, st) != cudaSuccess || c.bad.alloc(2, st) != cudaSuccess ||
+        (pat && (c.pid.alloc(np, st) != cudaSuccess || c.dict.alloc(DCAP + 1, st) != cudaSuccess ||
                  cudaMallocAsync((void**)&table, scratch, st) != cudaSuccess))) {
       (void)cudaGetLastError();  // not an error of the call: it runs on the 32-bit columns
       if (table) cudaFreeAsync(table, st);
-      plan_release_idx16_arrays(p, st);
+      c.release_streams(st);
       return B200SP_OK;
     }
-    B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_d + nnz, 0, sizeof(uint16_t) * (nd - (size_t)nnz), st));
-    B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_anchor + m, 0, sizeof(int) * (na - (size_t)m), st));
-    B200SP_CUDA_TRY(cudaMemsetAsync(p->idx16_bad, 0, 2 * sizeof(int), st));
+    B200SP_CUDA_TRY(cudaMemsetAsync(c.d + nnz, 0, sizeof(uint16_t) * (nd - (size_t)nnz), st));
+    B200SP_CUDA_TRY(cudaMemsetAsync(c.anchor + m, 0, sizeof(int) * (na - (size_t)m), st));
+    B200SP_CUDA_TRY(cudaMemsetAsync(c.bad, 0, 2 * sizeof(int), st));
     const int blocks = (int)std::max<int64_t>(1, std::min<int64_t>(((int64_t)m + 31) / 32, (int64_t)sm_count() * 16));
-    build_idx16_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, p->LMAX, p->idx16_d, p->idx16_anchor, p->idx16_bad);
+    build_idx16_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, LMAX, c.d, c.anchor, c.bad);
     B200SP_LAUNCH_CHECK();
     if (pat) {
       int* rep = reinterpret_cast<int*>(table + PAT_SLOTS);
@@ -1202,186 +1011,73 @@ static int plan_idx16(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, 
       int* slot_len = slot_start + PAT_SLOTS;
       int* row_slot = slot_len + PAT_SLOTS;
       B200SP_CUDA_TRY(cudaMemsetAsync(table, 0, sizeof(unsigned long long) * PAT_SLOTS, st));
-      B200SP_CUDA_TRY(cudaMemsetAsync(p->pat_pid + m, 0, sizeof(uint16_t) * (np - (size_t)m), st));
-      pattern_hash_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, p->LMAX, table, rep, row_slot, p->idx16_bad + 1);
+      B200SP_CUDA_TRY(cudaMemsetAsync(c.pid + m, 0, sizeof(uint16_t) * (np - (size_t)m), st));
+      pattern_hash_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, LMAX, table, rep, row_slot, c.bad + 1);
       B200SP_LAUNCH_CHECK();
-      pattern_dict_kernel<<<1, 256, 0, st>>>(row_ptr, col_idx, table, rep, slot_start, slot_len, p->pat_dict, p->idx16_bad + 1);
+      pattern_dict_kernel<<<1, 256, 0, st>>>(row_ptr, col_idx, table, rep, slot_start, slot_len, c.dict, c.bad + 1);
       B200SP_LAUNCH_CHECK();
-      pattern_assign_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, p->LMAX, row_slot, slot_start, slot_len, p->pat_dict,
-                                                    p->pat_pid, p->idx16_bad + 1);
+      pattern_assign_kernel<<<blocks, 256, 0, st>>>(m, row_ptr, col_idx, LMAX, row_slot, slot_start, slot_len, c.dict, c.pid,
+                                                    c.bad + 1);
       B200SP_LAUNCH_CHECK();
       cudaFreeAsync(table, st);
     }
-    if (!p->idx16_bad_host) B200SP_CUDA_TRY(cudaMallocHost((void**)&p->idx16_bad_host, 2 * sizeof(int)));
-    if (!p->idx16_event) B200SP_CUDA_TRY(cudaEventCreateWithFlags(&p->idx16_event, cudaEventDisableTiming));
-    B200SP_CUDA_TRY(cudaMemcpyAsync(p->idx16_bad_host, p->idx16_bad, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    B200SP_CUDA_TRY(cudaEventRecord(p->idx16_event, st));
-    p->idx16_state = -1;
+    if (int rc = c.verdict.fetch(c.bad, 2, st)) return rc;
+    c.state = -1;
   }
-  if (p->idx16_state < 0 && cudaEventQuery(p->idx16_event) == cudaSuccess) {
-    const int* bad = p->idx16_bad_host;
-    p->idx16_state = (p->pat_pid && bad[1] == 0) ? COLS_PAT : bad[0] == 0 ? COLS_DELTA : COLS_I32;
-    if (p->idx16_state == COLS_PAT) {
+  if (c.state < 0 && c.verdict.ready()) {
+    const int* bad = c.verdict.h;
+    c.state = (c.pid && bad[1] == 0) ? COLS_PAT : bad[0] == 0 ? COLS_DELTA : COLS_I32;
+    if (c.state == COLS_PAT) {
       // the pattern form's own tiles, for its larger stages, ahead of its first launch; its long rows are the cfg's (same
-      // LMAX), so the analysis's copy of them is dropped.  A table that cannot be built leaves the matrix on the deltas.
+      // LMAX), so the cut's copy of them is dropped.  A table that cannot be built leaves the matrix on the deltas.
       TileAnalysis a;
-      const int rc = tile_analyse(st, m, nnz, row_ptr, PAT_TILE_CAP, p->LMAX, &a);
-      if (a.long_rows) cudaFreeAsync(a.long_rows, st);
-      if (a.n_long) cudaFreeAsync(a.n_long, st);
-      p->pat_tiles = a.tiles;
-      p->pat_n_tiles = a.n_tiles;
+      const int rc = tile_analyse(st, m, nnz, row_ptr, PAT_TILE_CAP, LMAX, &a);
+      a.release_long_rows(st);
+      c.pat = std::move(a);
+      c.pat_cut = ++p->cuts;
       if (rc != B200SP_OK) {
         (void)cudaGetLastError();
-        if (a.tiles) cudaFreeAsync(a.tiles, st);
-        p->pat_tiles = nullptr;
-        p->pat_n_tiles = 0;
-        p->idx16_state = COLS_DELTA;
+        c.pat.release(st);
+        c.state = COLS_DELTA;
       }
     }
-    if (p->idx16_state == COLS_I32) plan_release_idx16_arrays(p, st);  // the key stays: not built again for this matrix
-    if (p->idx16_state == COLS_DELTA) {
-      if (p->pat_pid) cudaFreeAsync(p->pat_pid, st);
-      if (p->pat_dict) cudaFreeAsync(p->pat_dict, st);
-      p->pat_pid = nullptr;
-      p->pat_dict = nullptr;
+    if (c.state == COLS_I32) c.release_streams(st);  // the key stays: not built again for this matrix
+    if (c.state == COLS_DELTA) {
+      c.pid.release(st);
+      c.dict.release(st);
     }
   }
   return B200SP_OK;
 }
 
-// The column form of the next tiled launch (p->cols_launch), and so its tile table (plan_tiles).
+// The column form of the next tiled launch (p->cols.launch), and so its tile table (plan_tiles).
 // B200SP_SPMV_IDX16=0: the 32-bit columns (A/B comparisons; the 16-bit streams are not built for this call).
-static int plan_cols(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, const int* col_idx) {
+static int plan_cols(b200sp_spmv_plan* p, cudaStream_t st, int cfg, int m, int64_t nnz, const int* row_ptr, const int* col_idx) {
   const char* i16 = getenv("B200SP_SPMV_IDX16");
-  p->cols_launch = COLS_I32;
+  p->cols.launch = COLS_I32;
   if (!(i16 && i16[0] == '0')) {
     const int rc = plan_idx16(p, st, m, nnz, row_ptr, col_idx);
     if (rc) return rc;
-    if (p->idx16_state > 0) p->cols_launch = p->idx16_state;
+    if (p->cols.state > 0) p->cols.launch = p->cols.state;
   }
   // one tile table at a time: the pattern form's while it runs, else the cfg's, cut again when a call goes back to them
-  if (p->cols_launch == COLS_PAT) {
-    if (p->tiles) cudaFreeAsync(p->tiles, st);
-    p->tiles = nullptr;
-    p->n_tiles = 0;
-  } else if (!p->tiles) {
-    TileAnalysis a;
-    const int rc = tile_analyse(st, m, nnz, row_ptr, kCfgs[p->key_cfg].cap, p->LMAX, &a);
-    if (a.long_rows) cudaFreeAsync(a.long_rows, st);
-    if (a.n_long) cudaFreeAsync(a.n_long, st);
-    p->tiles = a.tiles;
-    p->n_tiles = a.n_tiles;
+  TileAnalysis& a = p->r1.a;
+  if (p->cols.launch == COLS_PAT) {
+    a.tiles.release(st);
+    a.n_tiles = 0;
+  } else if (!a.tiles) {
+    TileAnalysis cut;
+    const int rc = tile_analyse(st, m, nnz, row_ptr, kCfgs[cfg].cap, a.LMAX, &cut);
+    cut.release_long_rows(st);  // the analysis keeps the list its segments were built from
+    a.tiles = std::move(cut.tiles);
+    a.n_tiles = cut.n_tiles;
+    p->r1.cut = ++p->cuts;
     if (rc != B200SP_OK) return rc;
   }
   return B200SP_OK;
 }
 
-static const int4* plan_tiles(const b200sp_spmv_plan* p, int* n_tiles) {
-  const bool pat = p->cols_launch == COLS_PAT;
-  *n_tiles = pat ? p->pat_n_tiles : p->n_tiles;
-  return pat ? p->pat_tiles : p->tiles;
-}
-
-// rank-2 scratch + bookkeeping used by spmm.cu
-int plan_mv_scratch(b200sp_spmv_plan* p, cudaStream_t st, size_t xt_bytes, size_t yt_bytes, void** xt, void** yt) {
-  if (xt_bytes > p->xt_bytes) {
-    if (p->xt) cudaFreeAsync(p->xt, st);
-    p->xt = nullptr;
-    p->xt_bytes = 0;
-    B200SP_CUDA_TRY(cudaMallocAsync(&p->xt, xt_bytes, st));
-    p->xt_bytes = xt_bytes;
-  }
-  if (yt_bytes > p->yt_bytes) {
-    if (p->yt) cudaFreeAsync(p->yt, st);
-    p->yt = nullptr;
-    p->yt_bytes = 0;
-    B200SP_CUDA_TRY(cudaMallocAsync(&p->yt, yt_bytes, st));
-    p->yt_bytes = yt_bytes;
-  }
-  *xt = p->xt;
-  *yt = p->yt;
-  return B200SP_OK;
-}
-__global__ void build_chunk_rows_kernel(int m, const int* __restrict__ row_ptr, int n_chunks, int Q,
-                                        int* __restrict__ chunk_row);
-int plan_chunk_rows(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int Q, int** chunk_row,
-                    int* n_chunks) {
-  if (!(p->chunk_row && p->chunk_key == row_ptr && p->chunk_m == m && p->chunk_nnz == nnz && p->chunk_q == Q)) {
-    if (p->chunk_row) cudaFreeAsync(p->chunk_row, st);
-    p->chunk_row = nullptr;
-    p->n_chunks = (int)((nnz + Q - 1) / Q);
-    if (p->n_chunks < 1) p->n_chunks = 1;
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->chunk_row, sizeof(int) * (size_t)p->n_chunks, st));
-    build_chunk_rows_kernel<<<(p->n_chunks + 255) / 256, 256, 0, st>>>(m, row_ptr, p->n_chunks, Q, p->chunk_row);
-    B200SP_LAUNCH_CHECK();
-    p->chunk_key = row_ptr;
-    p->chunk_m = m;
-    p->chunk_nnz = nnz;
-    p->chunk_q = Q;
-  }
-  *chunk_row = p->chunk_row;
-  *n_chunks = p->n_chunks;
-  return B200SP_OK;
-}
-// Segments of the rows the rank-2 tile kernel leaves out (longer than LMAX): {row, first entry, end entry,
-// flags}; flags bit 0 = the row has several segments (its pieces are combined with atomics), bit 1 = first
-// segment of its row.  One thread per long row.
-__global__ void build_segments_kernel(const int* __restrict__ long_rows, const int* __restrict__ n_long,
-                                      const int* __restrict__ row_ptr, int SEG, int4* __restrict__ segs,
-                                      int* __restrict__ n_seg) {
-  const int nl = *n_long;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += gridDim.x * blockDim.x) {
-    const int r = long_rows[i];
-    const int s = row_ptr[r], e = row_ptr[r + 1];
-    const int nseg = (e - s + SEG - 1) / SEG;
-    const int base = atomicAdd(n_seg, nseg);
-    for (int q = 0; q < nseg; ++q)
-      segs[base + q] = make_int4(r, s + q * SEG, min(e, s + (q + 1) * SEG), (nseg > 1 ? 1 : 0) | (q == 0 ? 2 : 0));
-  }
-}
-
-// Tile analysis of the rank-2 tile kernel (spmm.cu): same descriptors as the rank-1 kernel's, with its own
-// stage capacity and row limit; cached per matrix in the plan; stream-ordered, no host synchronisation.
-int plan_analyse_mm(b200sp_spmv_plan* p, cudaStream_t st, int cap, int lmax, int seg, int m, int64_t nnz, const int* row_ptr,
-                    MMTileView* out) {
-  if (!(p->mm_tiles && p->mm_key_row_ptr == row_ptr && p->mm_key_m == m && p->mm_key_nnz == nnz && p->mm_key_cap == cap &&
-        p->mm_key_lmax == lmax)) {
-    plan_release_mm(p, st);
-    p->mm_cap = cap;
-    TileAnalysis a;
-    const int rc = tile_analyse(st, m, nnz, row_ptr, cap, lmax, &a);
-    p->mm_tiles = a.tiles;
-    p->mm_n_tiles = a.n_tiles;
-    p->mm_T = a.T;
-    p->mm_LMAX = a.LMAX;
-    p->mm_long_rows = a.long_rows;
-    p->mm_n_long = a.n_long;
-    if (rc != B200SP_OK) return rc;
-    p->mm_seg_cap = (int)(nnz / seg) + a.long_cap + 1;
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->mm_segs, sizeof(int4) * (size_t)p->mm_seg_cap, st));
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->mm_n_seg, sizeof(int), st));
-    B200SP_CUDA_TRY(cudaMemsetAsync(p->mm_n_seg, 0, sizeof(int), st));
-    build_segments_kernel<<<std::max(1, std::min((a.long_cap + 255) / 256, sm_count() * 4)), 256, 0, st>>>(
-        p->mm_long_rows, p->mm_n_long, row_ptr, seg, p->mm_segs, p->mm_n_seg);
-    B200SP_LAUNCH_CHECK();
-    p->mm_key_row_ptr = row_ptr;
-    p->mm_key_m = m;
-    p->mm_key_nnz = nnz;
-    p->mm_key_cap = cap;
-    p->mm_key_lmax = lmax;
-  }
-  out->tiles = p->mm_tiles;
-  out->n_tiles = p->mm_n_tiles;
-  out->LMAX = p->mm_LMAX;
-  out->segs = p->mm_segs;
-  out->n_seg = p->mm_n_seg;
-  out->seg_cap = p->mm_seg_cap;
-  return B200SP_OK;
-}
-
-void plan_set_last_kernel(b200sp_spmv_plan* p, const char* s) {
-  if (p) snprintf(p->last_kernel, sizeof(p->last_kernel), "%s", s);
-}
+static const TileAnalysis& plan_tiles(const b200sp_spmv_plan* p) { return p->cols.launch == COLS_PAT ? p->cols.pat : p->r1.a; }
 
 int spmv_lanes_per_row(int64_t m, int64_t nnz);
 static int pick_lpr(int m, int64_t nnz) { return spmv_lanes_per_row(m, nnz); }
@@ -1404,11 +1100,11 @@ static int launch_tile_form(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t
   constexpr int KSTAGES = PAT ? PAT_STAGES : STAGES, KCAP = PAT ? PAT_CAP : CAP;
   using Smem = TileSmem<S, KCAP, KSTAGES, COLS>;
   auto kern = spmv_tile_kernel<S, LPR, NW, KSTAGES, KCAP, UNR, COLS, false>;
-  const uint16_t* c16 = PAT ? p->pat_pid : p->idx16_d;
-  const int* anchor = p->idx16_anchor;
-  const int* dict = p->pat_dict;
-  int n_tiles = 0;
-  const int4* tiles = plan_tiles(p, &n_tiles);
+  const uint16_t* c16 = PAT ? p->cols.pid : p->cols.d;
+  const int* anchor = p->cols.anchor;
+  const int* dict = p->cols.dict;
+  const int n_tiles = plan_tiles(p).n_tiles;
+  const int4* tiles = plan_tiles(p).tiles;
   const size_t smem = sizeof(Smem) + tile_smem_extra<COLS>() + 128;
   static KernelSetup ks;
   int occ_dev = 1;
@@ -1427,13 +1123,13 @@ static int launch_tile_form(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t
       static KernelSetup ksf;
       int occ_f = 1;
       if (int rc = kernel_setup(ksf, kf, (NW + 1) * 32, smem, &occ_f)) return rc;
-      kf<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals, x,
+      kf<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->r1.a.LMAX, tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals, x,
                                             y, alpha, beta, p->extra);
       launched = true;
     }
   }
   if (!launched)
-    kern<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->LMAX, tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals, x,
+    kern<<<grid, (NW + 1) * 32, smem, st>>>(m, nnz, hi - lo, p->r1.a.LMAX, tiles + lo, row_ptr, col_idx, c16, anchor, dict, vals, x,
                                             y, alpha, beta, direct_extra(p->extra));
   B200SP_LAUNCH_CHECK();
   // the pattern form is a sub-form of the 16-bit column data (pattern starts + anchors): IDX=u16, and COLS names the source
@@ -1448,9 +1144,9 @@ static int launch_tile_form(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t
 template <typename S, int LPR, int NW, int STAGES, int CAP, int UNR = 8>
 static int launch_tile(b200sp_spmv_plan* p, cudaStream_t st, int m, int64_t nnz, const int* row_ptr,
                        const int* col_idx, const S* vals, const S* x, S* y, S alpha, S beta) {
-  if (p->cols_launch == COLS_PAT)
+  if (p->cols.launch == COLS_PAT)
     return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, COLS_PAT>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
-  if (p->cols_launch == COLS_DELTA)
+  if (p->cols.launch == COLS_DELTA)
     return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, COLS_DELTA>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
   return launch_tile_form<S, LPR, NW, STAGES, CAP, UNR, COLS_I32>(p, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta);
 }
@@ -1509,16 +1205,6 @@ int transpose_structure(cudaStream_t st, int m, int n, int64_t nnz, const int* r
 template <typename S>
 int gather_values(cudaStream_t st, int64_t nnz, const int* t_src, const S* v, S* tv);
 
-static void plan_release_transpose(b200sp_spmv_plan* p, cudaStream_t st) {
-  void* ptrs[] = {p->t_rp, p->t_ci, p->t_src, p->t_vals};
-  for (void* q : ptrs)
-    if (q) cudaFreeAsync(q, st);
-  p->t_rp = p->t_ci = p->t_src = nullptr;
-  p->t_vals = nullptr;
-  p->t_vals_bytes = 0;
-  p->t_key_rp = nullptr;
-}
-
 template <typename S>
 static int spmv_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int n, int64_t nnz, S alpha,
                      const int* row_ptr, const int* col_idx, const S* vals, const S* x, S beta, S* y);
@@ -1529,39 +1215,29 @@ static int spmv_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
 template <typename S>
 static int spmv_cached_transpose(b200sp_spmv_plan* p, cudaStream_t st, int m, int n, int64_t nnz, S alpha,
                                  const int* row_ptr, const int* col_idx, const S* vals, const S* x, S beta, S* y) {
-  if (!(p->t_rp && p->t_key_rp == row_ptr && p->t_key_ci == col_idx && p->t_key_m == m && p->t_key_n == n &&
-        p->t_key_nnz == nnz)) {
-    plan_release_transpose(p, st);
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->t_rp, sizeof(int) * ((size_t)n + 1), st));
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->t_ci, sizeof(int) * (size_t)nnz, st));
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->t_src, sizeof(int) * (size_t)nnz, st));
-    int rc = transpose_structure(st, m, n, nnz, row_ptr, col_idx, p->t_rp, p->t_ci, p->t_src);
+  SpmvTranspose& t = p->t;
+  const PlanKey key{row_ptr, col_idx, m, n, nnz};
+  if (t.key != key) {
+    t.key = PlanKey();
+    B200SP_CUDA_TRY(t.rp.alloc((size_t)n + 1, st));
+    B200SP_CUDA_TRY(t.ci.alloc((size_t)nnz, st));
+    B200SP_CUDA_TRY(t.src.alloc((size_t)nnz, st));
+    int rc = transpose_structure(st, m, n, nnz, row_ptr, col_idx, t.rp, t.ci, t.src);
     if (rc) return rc;
-    p->t_key_rp = row_ptr;
-    p->t_key_ci = col_idx;
-    p->t_key_m = m;
-    p->t_key_n = n;
-    p->t_key_nnz = nnz;
-    if (!p->tplan) {
-      rc = b200sp_spmv_plan_create(&p->tplan, p->algo);
+    t.key = key;
+    if (!t.plan) {
+      rc = b200sp_spmv_plan_create(&t.plan, p->algo);
       if (rc) return rc;
-      p->tplan->cfg = p->cfg;
-      p->tplan->ctas_per_sm = p->ctas_per_sm;
+      t.plan->cfg = p->cfg;
+      t.plan->ctas_per_sm = p->ctas_per_sm;
     }
   }
-  const size_t need = sizeof(S) * (size_t)nnz;
-  if (need > p->t_vals_bytes) {
-    if (p->t_vals) cudaFreeAsync(p->t_vals, st);
-    p->t_vals = nullptr;
-    p->t_vals_bytes = 0;
-    B200SP_CUDA_TRY(cudaMallocAsync(&p->t_vals, need, st));
-    p->t_vals_bytes = need;
-  }
-  int rc = gather_values<S>(st, nnz, p->t_src, vals, (S*)p->t_vals);
+  B200SP_CUDA_TRY(t.vals.grow(sizeof(S) * (size_t)nnz, st));
+  int rc = gather_values<S>(st, nnz, t.src, vals, t.vals.as<S>());
   if (rc) return rc;
-  rc = spmv_impl<S>(p->tplan, st, 'N', n, m, nnz, alpha, p->t_rp, p->t_ci, (const S*)p->t_vals, x, beta, y);
+  rc = spmv_impl<S>(t.plan, st, 'N', n, m, nnz, alpha, t.rp, t.ci, t.vals.as<S>(), x, beta, y);
   if (rc) return rc;
-  snprintf(p->last_kernel, sizeof(p->last_kernel), "cached_transpose+%.70s", p->tplan->last_kernel);
+  snprintf(p->last_kernel, sizeof(p->last_kernel), "cached_transpose+%.70s", t.plan->last_kernel);
   return B200SP_OK;
 }
 
@@ -1622,7 +1298,7 @@ static int spmv_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   if (rc) return rc;
   // a piece of the host-vector pipeline runs the form its call settled on, with the tiles its bounds were cut from
   if (p->range_hi < 0) {
-    rc = plan_cols(p, st, m, nnz, row_ptr, col_idx);
+    rc = plan_cols(p, st, cfg, m, nnz, row_ptr, col_idx);
     if (rc) return rc;
   }
   const int lpr = p->lpr > 0 ? p->lpr : lpr_auto;
@@ -1631,24 +1307,24 @@ static int spmv_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   int phase = -1;  // 1: time the tiled kernel, 2: time the vector kernel
   bool use_vec = false;
   if (autotune) {
-    if (p->at_choice < 0 && p->at_calls >= 3 && cudaEventQuery(p->at_ev[1]) == cudaSuccess &&
-        cudaEventQuery(p->at_ev[3]) == cudaSuccess) {
-      if (cudaEventElapsedTime(&p->at_tile_ms, p->at_ev[0], p->at_ev[1]) == cudaSuccess &&
-          cudaEventElapsedTime(&p->at_vec_ms, p->at_ev[2], p->at_ev[3]) == cudaSuccess)
-        p->at_choice = (p->at_vec_ms < 0.9f * p->at_tile_ms) ? 1 : 0;
+    SpmvTuning& at = p->at;
+    if (at.choice < 0 && at.calls >= 3 && cudaEventQuery(at.ev[1]) == cudaSuccess && cudaEventQuery(at.ev[3]) == cudaSuccess) {
+      if (cudaEventElapsedTime(&at.tile_ms, at.ev[0], at.ev[1]) == cudaSuccess &&
+          cudaEventElapsedTime(&at.vec_ms, at.ev[2], at.ev[3]) == cudaSuccess)
+        at.choice = (at.vec_ms < 0.9f * at.tile_ms) ? 1 : 0;
     }
-    if (p->at_calls == 1 || p->at_calls == 2) {
-      phase = p->at_calls;
+    if (at.calls == 1 || at.calls == 2) {
+      phase = at.calls;
       for (int i = 0; i < 4; ++i)
-        if (!p->at_ev[i]) B200SP_CUDA_TRY(cudaEventCreate(&p->at_ev[i]));
+        if (!at.ev[i]) B200SP_CUDA_TRY(cudaEventCreate(&at.ev[i]));
     }
-    p->at_calls++;
-    use_vec = phase == 2 || (phase < 0 && p->at_choice == 1);
-    if (phase > 0) B200SP_CUDA_TRY(cudaEventRecord(p->at_ev[phase == 1 ? 0 : 2], st));
+    at.calls++;
+    use_vec = phase == 2 || (phase < 0 && at.choice == 1);
+    if (phase > 0) B200SP_CUDA_TRY(cudaEventRecord(at.ev[phase == 1 ? 0 : 2], st));
   }
   if (use_vec) {
     // same split as the tiled kernel: rows beyond LMAX go to the long-row kernel below, so the choice never changes a bit
-    rc = launch_vector<S>(p, st, lpr, m, row_ptr, col_idx, vals, x, y, alpha, beta, p->LMAX);
+    rc = launch_vector<S>(p, st, lpr, m, row_ptr, col_idx, vals, x, y, alpha, beta, p->r1.a.LMAX);
   } else {
     switch (lpr) {
       case 2: rc = launch_tile_cfg<S, 2>(p, cfg, st, m, nnz, row_ptr, col_idx, vals, x, y, alpha, beta); break;
@@ -1661,37 +1337,40 @@ static int spmv_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   }
   if (rc) return rc;
   // long rows: skip the launch once the (asynchronously fetched) count is known to be 0
-  if (!p->n_long_known && cudaEventQuery(p->n_long_event) == cudaSuccess) p->n_long_known = true;
-  if (!(p->n_long_known && *p->n_long_host == 0) && (p->range_hi < 0 || p->range_lo == 0)) {
+  SpmvTiles& r1 = p->r1;
+  if (!r1.n_long_known && r1.n_long.ready()) r1.n_long_known = true;
+  if (!(r1.n_long_known && *r1.n_long.h == 0) && (p->range_hi < 0 || p->range_lo == 0)) {
     const char* lr = getenv("B200SP_SPMV_LONGROWS");
     if (lr && lr[0] == 's') {
       constexpr int SEG = 4096;
-      if (!p->r1_built) {
-        p->r1_seg_cap = (int)(nnz / SEG) + p->long_cap + 1;
-        B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->r1_segs, sizeof(int4) * (size_t)p->r1_seg_cap, st));
-        B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->r1_n_seg, sizeof(int), st));
-        B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->r1_row_seg, sizeof(int2) * (size_t)p->long_cap, st));
-        B200SP_CUDA_TRY(cudaMallocAsync(&p->r1_partial, sizeof(double) * (size_t)p->r1_seg_cap, st));
-        B200SP_CUDA_TRY(cudaMemsetAsync(p->r1_n_seg, 0, sizeof(int), st));
-        build_row_segments_kernel<<<std::max(1, std::min((p->long_cap + 255) / 256, sm_count() * 4)), 256, 0, st>>>(
-            p->long_rows, p->n_long, row_ptr, SEG, p->r1_segs, p->r1_n_seg, p->r1_row_seg);
+      SpmvSegs& g = p->segs;
+      const int long_cap = r1.a.long_cap;
+      if (!g.built) {
+        g.cap = (int)(nnz / SEG) + long_cap + 1;
+        B200SP_CUDA_TRY(g.segs.alloc((size_t)g.cap, st));
+        B200SP_CUDA_TRY(g.n_seg.alloc(1, st));
+        B200SP_CUDA_TRY(g.row_seg.alloc((size_t)long_cap, st));
+        B200SP_CUDA_TRY(g.partial.alloc(sizeof(double) * (size_t)g.cap, st));
+        B200SP_CUDA_TRY(cudaMemsetAsync(g.n_seg, 0, sizeof(int), st));
+        build_row_segments_kernel<<<std::max(1, std::min((long_cap + 255) / 256, sm_count() * 4)), 256, 0, st>>>(
+            r1.a.long_rows, r1.a.n_long, row_ptr, SEG, g.segs, g.n_seg, g.row_seg);
         B200SP_LAUNCH_CHECK();
-        p->r1_built = true;
+        g.built = true;
       }
-      spmv_seg_partial_kernel<S><<<sm_count() * 4, 256, 0, st>>>(p->r1_segs, p->r1_n_seg, col_idx, vals, x, (S*)p->r1_partial);
+      spmv_seg_partial_kernel<S><<<sm_count() * 4, 256, 0, st>>>(g.segs, g.n_seg, col_idx, vals, x, g.partial.as<S>());
       B200SP_LAUNCH_CHECK();
-      spmv_seg_combine_kernel<S><<<std::max(1, std::min((p->long_cap + 255) / 256, sm_count())), 256, 0, st>>>(
-          p->long_rows, p->n_long, p->r1_row_seg, (const S*)p->r1_partial, y, alpha, beta, direct_extra(p->extra));
+      spmv_seg_combine_kernel<S><<<std::max(1, std::min((long_cap + 255) / 256, sm_count())), 256, 0, st>>>(
+          r1.a.long_rows, r1.a.n_long, g.row_seg, g.partial.as<const S>(), y, alpha, beta, direct_extra(p->extra));
       B200SP_LAUNCH_CHECK();
       snprintf(p->last_kernel + strlen(p->last_kernel), sizeof(p->last_kernel) - strlen(p->last_kernel), "+seg");
     } else {
-      int blocks = p->n_long_known ? std::min(*p->n_long_host, sm_count() * 4) : sm_count() * 2;
-      spmv_longrow_kernel<S><<<blocks, 256, 0, st>>>(p->long_rows, p->n_long, row_ptr, col_idx, vals, x, y, alpha, beta,
+      int blocks = r1.n_long_known ? std::min(*r1.n_long.h, sm_count() * 4) : sm_count() * 2;
+      spmv_longrow_kernel<S><<<blocks, 256, 0, st>>>(r1.a.long_rows, r1.a.n_long, row_ptr, col_idx, vals, x, y, alpha, beta,
                                                      direct_extra(p->extra));
       B200SP_LAUNCH_CHECK();
     }
   }
-  if (phase > 0) B200SP_CUDA_TRY(cudaEventRecord(p->at_ev[phase == 1 ? 1 : 3], st));
+  if (phase > 0) B200SP_CUDA_TRY(cudaEventRecord(p->at.ev[phase == 1 ? 1 : 3], st));
   return B200SP_OK;
 }
 
@@ -1730,42 +1409,15 @@ int b200sp_spmv_plan_create(b200sp_spmv_plan** plan, int algo) {
 int b200sp_spmv_plan_destroy(b200sp_spmv_plan* p, void* stream) {
   if (!p) return B200SP_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  plan_release_analysis(p, st);
-  plan_release_mm(p, st);
-  plan_release_transpose(p, st);
-  if (p->tplan) b200sp_spmv_plan_destroy(p->tplan, stream);
-  p->tplan = nullptr;
-  if (p->dx) cudaFreeAsync(p->dx, st);
-  if (p->dy) cudaFreeAsync(p->dy, st);
-  if (p->xt) cudaFreeAsync(p->xt, st);
-  if (p->yt) cudaFreeAsync(p->yt, st);
-  if (p->chunk_row) cudaFreeAsync(p->chunk_row, st);
-  for (int i = 0; i < 4; ++i)
-    if (p->at_ev[i]) cudaEventDestroy(p->at_ev[i]);
-  if (p->pipe.init) {
-    cudaStreamSynchronize(p->pipe.sH);
-    cudaStreamSynchronize(p->pipe.sD);
-    for (int b = 0; b < 2; ++b) {
-      if (p->pipe.dx[b]) cudaFree(p->pipe.dx[b]);
-      if (p->pipe.dy[b]) cudaFree(p->pipe.dy[b]);
-      cudaEventDestroy(p->pipe.ev_x[b]);
-      cudaEventDestroy(p->pipe.ev_c[b]);
-      cudaEventDestroy(p->pipe.ev_done[b]);
-    }
-    for (int c = 0; c < 8; ++c) cudaEventDestroy(p->pipe.ev_chunk[c]);
-    cudaStreamDestroy(p->pipe.sH);
-    cudaStreamDestroy(p->pipe.sD);
-  }
-  if (p->n_long_event) {
-    cudaEventSynchronize(p->n_long_event);  // the pinned mirror must not be written after it is freed
-    cudaEventDestroy(p->n_long_event);
-  }
-  if (p->n_long_host) cudaFreeHost(p->n_long_host);
-  if (p->idx16_event) {
-    cudaEventSynchronize(p->idx16_event);
-    cudaEventDestroy(p->idx16_event);
-  }
-  if (p->idx16_bad_host) cudaFreeHost(p->idx16_bad_host);
+  p->r1.release(st);
+  p->cols.release(st);
+  p->segs.release(st);
+  p->mm.release(st);
+  p->t.release(st);
+  p->at.release();
+  p->dx.release(st);
+  p->dy.release(st);
+  p->pipe.release();
   delete p;
   return B200SP_OK;
 }
@@ -1791,17 +1443,12 @@ int b200sp_spmv_plan_invalidate(b200sp_spmv_plan* p, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   // everything derived from the STRUCTURE of the matrix the plan last saw: tiles, long rows, 16-bit column stream, rank-2
   // tiles / segments / items, chunk table, cached transpose, host-vector piece bounds, self-tuning state.  Buffers that only depend on sizes stay.
-  plan_release_analysis(p, st);
-  plan_release_mm(p, st);
-  if (p->chunk_row) cudaFreeAsync(p->chunk_row, st);
-  p->chunk_row = nullptr;
-  p->chunk_key = nullptr;
-  p->n_chunks = 0;
-  p->t_key_rp = p->t_key_ci = nullptr;
-  p->pipe.key = nullptr;
-  p->at_calls = 0;
-  p->at_choice = -1;
-  if (p->tplan) return b200sp_spmv_plan_invalidate(p->tplan, stream);
+  plan_reset_analysis(p, st);
+  p->mm.reset(st);
+  p->t.key = PlanKey();
+  p->pipe.key = PlanKey();
+  p->at.reset();
+  if (p->t.plan) return b200sp_spmv_plan_invalidate(p->t.plan, stream);
   return B200SP_OK;
 }
 
@@ -1952,22 +1599,12 @@ int b200sp_peer_push(void* stream, const void* src, int64_t bytes, int n_dst, vo
 static int hostvec_simple(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int n, int64_t nnz, double alpha,
                           const int* row_ptr, const int* col_idx, const double* vals, const double* x_host,
                           double beta, double* y_host, size_t xb, size_t yb) {
-  if (xb > p->dx_bytes) {
-    if (p->dx) cudaFreeAsync(p->dx, st);
-    p->dx = nullptr;
-    B200SP_CUDA_TRY(cudaMallocAsync(&p->dx, xb, st));
-    p->dx_bytes = xb;
-  }
-  if (yb > p->dy_bytes) {
-    if (p->dy) cudaFreeAsync(p->dy, st);
-    p->dy = nullptr;
-    B200SP_CUDA_TRY(cudaMallocAsync(&p->dy, yb, st));
-    p->dy_bytes = yb;
-  }
+  B200SP_CUDA_TRY(p->dx.grow(xb, st));
+  B200SP_CUDA_TRY(p->dy.grow(yb, st));
   if (xb) B200SP_CUDA_TRY(cudaMemcpyAsync(p->dx, x_host, xb, cudaMemcpyHostToDevice, st));
   if (beta != 0.0 && yb) B200SP_CUDA_TRY(cudaMemcpyAsync(p->dy, y_host, yb, cudaMemcpyHostToDevice, st));
-  int rc = spmv_impl<double>(p, st, mode, m, n, nnz, alpha, row_ptr, col_idx, vals, (const double*)p->dx, beta,
-                             (double*)p->dy);
+  int rc = spmv_impl<double>(p, st, mode, m, n, nnz, alpha, row_ptr, col_idx, vals, p->dx.as<const double>(), beta,
+                             p->dy.as<double>());
   if (rc) return rc;
   if (yb) B200SP_CUDA_TRY(cudaMemcpyAsync(y_host, p->dy, yb, cudaMemcpyDeviceToHost, st));
   return B200SP_OK;
@@ -2017,11 +1654,15 @@ int b200sp_spmv_hostvec_f64_i32(b200sp_spmv_plan* p, void* stream, char mode, in
   int rc = plan_analyse<double>(p, st, cfg, m, n, nnz, row_ptr);
   if (rc) return rc;
   // the column form is settled once per call, so that every piece launches on the table the bounds come from
-  rc = plan_cols(p, st, m, nnz, row_ptr, col_idx);
+  rc = plan_cols(p, st, cfg, m, nnz, row_ptr, col_idx);
   if (rc) return rc;
-  int n_tiles = 0;
-  const int4* tiles = plan_tiles(p, &n_tiles);
-  if (q.key != row_ptr || q.key_cfg != cfg || q.key_m != m || q.key_nnz != nnz || q.key_tiles != (const void*)tiles) {
+  const int n_tiles = plan_tiles(p).n_tiles;
+  const int4* tiles = plan_tiles(p).tiles;
+  // keyed on the cut that made the table this call launches on, not on its address: a new table may come back at the address
+  // of the one the bounds were cut from, and the plan may hold both tables
+  const uint64_t cut = p->cols.launch == COLS_PAT ? p->cols.pat_cut : p->r1.cut;
+  const PlanKey key{row_ptr, nullptr, m, -1, nnz, cfg, (int64_t)cut};
+  if (q.key != key) {
     q.nc = 4;  // pieces of y that go down while the next piece is computed (B200SP_HOSTVEC_PIECES: 1..8, tuning)
     if (const char* e = getenv("B200SP_HOSTVEC_PIECES")) {
       const int v = atoi(e);
@@ -2036,11 +1677,7 @@ int b200sp_spmv_hostvec_f64_i32(b200sp_spmv_plan* p, void* stream, char mode, in
     for (int c = 0; c < q.nc; ++c) q.row_b[c] = d[c].x;  // first row of the first tile of piece c
     q.row_b[q.nc] = m;
     q.row_b[0] = 0;
-    q.key = row_ptr;
-    q.key_cfg = cfg;
-    q.key_m = m;
-    q.key_nnz = nnz;
-    q.key_tiles = (const void*)tiles;
+    q.key = key;
   }
   const int b = (int)(q.call & 1ull);
   if (q.defer && q.call >= 2) {

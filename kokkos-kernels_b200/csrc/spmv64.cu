@@ -26,15 +26,11 @@
 struct b200sp_spmv64_plan {
   int algo = 0;
   int64_t window_nnz = b200sp::kDefaultWindow;
-  // key of the analysed matrix
-  const void* key_rp = nullptr;
-  const void* key_ci = nullptr;
-  int64_t key_m = -1, key_n = -1, key_nnz = -1;
-  int key_bits = 0;
+  b200sp::PlanKey key;  // of the analysed matrix
   // analysis products: windows based on multiples of 4 entries (16-byte aligned bulk copies), one plan per window
   b200sp::RowWindows cut;
   std::vector<b200sp_spmv_plan*> plans;
-  int* col32 = nullptr;  // device: narrowed columns (64-bit input only)
+  b200sp::DevArray<int> col32;  // narrowed columns (64-bit input only)
   char last_kernel[128] = "none";
 };
 
@@ -46,16 +42,14 @@ void release(b200sp_spmv64_plan* p, cudaStream_t st) {
   for (b200sp_spmv_plan* pl : p->plans) b200sp_spmv_plan_destroy(pl, (void*)st);
   p->plans.clear();
   p->cut.release(st);
-  if (p->col32) cudaFreeAsync(p->col32, st);
-  p->col32 = nullptr;
-  p->key_rp = nullptr;
+  p->col32.release(st);
+  p->key = PlanKey();
 }
 
 int analyse(b200sp_spmv64_plan* p, cudaStream_t st, int64_t m, int64_t n, int64_t nnz, const int64_t* row_ptr,
             const void* col_idx, int col_bits) {
-  if (p->key_rp == row_ptr && p->key_ci == col_idx && p->key_m == m && p->key_n == n && p->key_nnz == nnz &&
-      p->key_bits == col_bits)
-    return B200SP_OK;
+  const PlanKey key{row_ptr, col_idx, m, n, nnz, col_bits};
+  if (p->key == key) return B200SP_OK;
   release(p, st);
   int64_t row = 0;
   int rc = cut_windows(st, m, row_ptr, nullptr, p->window_nnz, 4, &p->cut, &row);
@@ -74,7 +68,7 @@ int analyse(b200sp_spmv64_plan* p, cudaStream_t st, int64_t m, int64_t n, int64_
     int bad = 0;
     B200SP_CUDA_TRY(tmp.alloc(&d_bad, 1));
     B200SP_CUDA_TRY(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
-    B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->col32, sizeof(int) * (size_t)std::max<int64_t>(nnz, 1), st));
+    B200SP_CUDA_TRY(p->col32.alloc((size_t)std::max<int64_t>(nnz, 1), st));
     win64_narrow_kernel<<<grid_for(nnz, 256, 16), 256, 0, st>>>(nnz, (const int64_t*)col_idx, p->col32, d_bad);
     B200SP_LAUNCH_CHECK();
     B200SP_CUDA_TRY(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -92,12 +86,7 @@ int analyse(b200sp_spmv64_plan* p, cudaStream_t st, int64_t m, int64_t n, int64_
     // on where the windows fall, and equals the 32-bit entry points' on a matrix both can take
     if ((rc = b200sp_spmv_plan_tune(pl, -1, spmv_lanes_per_row(m, nnz), -1))) return rc;
   }
-  p->key_rp = row_ptr;
-  p->key_ci = col_idx;
-  p->key_m = m;
-  p->key_n = n;
-  p->key_nnz = nnz;
-  p->key_bits = col_bits;
+  p->key = key;
   return B200SP_OK;
 }
 
@@ -203,7 +192,7 @@ int b200sp_spmv64_plan_set_window(b200sp_spmv64_plan* p, int64_t max_entries) {
   B200SP_REQUIRE(p != nullptr, "spmv64_plan_set_window: null plan");
   if (int rc = b200sp::check_window_limit("spmv64_plan_set_window", max_entries)) return rc;
   p->window_nnz = max_entries;
-  p->key_rp = nullptr;  // next call analyses again
+  p->key = b200sp::PlanKey();  // next call analyses again
   return B200SP_OK;
 }
 

@@ -37,10 +37,10 @@ struct b200sp_sptrsv_plan {
   bool symbolic = false;
   const int *key_rp = nullptr, *key_ci = nullptr;
   int n_levels = 0;
-  int4* level_rows = nullptr;     // rows grouped by level (device): (row, first entry, end of the row, -)
+  b200sp::DevArray<int4> level_rows;  // rows grouped by level (device): (row, first entry, end of the row, -)
   int group = 8;                  // lanes per row of the solve kernels
   int* level_ptr_host = nullptr;  // n_levels + 1 offsets (host)
-  int* level_ptr_dev = nullptr;   // the same on the device (the chain kernel walks it)
+  b200sp::DevArray<int> level_ptr_dev;  // the same on the device (the chain kernel walks it)
   struct Segment {
     int l0, l1;  // levels [l0, l1): one launch per level, or one single-CTA launch for the whole run when `chain`
     bool chain;
@@ -213,10 +213,8 @@ void tr_launch_solve(const b200sp_sptrsv_plan* p, cudaStream_t st, int n, const 
 }
 
 void tr_release(b200sp_sptrsv_plan* p, cudaStream_t st) {
-  if (p->level_rows) cudaFreeAsync(p->level_rows, st);
-  p->level_rows = nullptr;
-  if (p->level_ptr_dev) cudaFreeAsync(p->level_ptr_dev, st);
-  p->level_ptr_dev = nullptr;
+  p->level_rows.release(st);
+  p->level_ptr_dev.release(st);
   delete[] p->level_ptr_host;
   p->level_ptr_host = nullptr;
   p->segments.clear();
@@ -309,10 +307,10 @@ int sptrsv_symbolic_impl(b200sp_sptrsv_plan* p, cudaStream_t st, int n, const in
   for (int l = 0; l < levels; ++l) p->level_ptr_host[l + 1] = p->level_ptr_host[l] + hc[l];
   delete[] hc;
   B200SP_CUDA_TRY(cudaMemcpyAsync(cursor, p->level_ptr_host, sizeof(int) * (size_t)(levels + 1), cudaMemcpyHostToDevice, st));
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->level_rows, sizeof(int4) * (size_t)n, st));
+  B200SP_CUDA_TRY(p->level_rows.alloc((size_t)n, st));
   tr_place_kernel<<<grid_for(n), 256, 0, st>>>(n, rp, lv[cur], cursor, p->level_rows);
   B200SP_LAUNCH_CHECK();
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&p->level_ptr_dev, sizeof(int) * (size_t)(levels + 1), st));
+  B200SP_CUDA_TRY(p->level_ptr_dev.alloc((size_t)(levels + 1), st));
   B200SP_CUDA_TRY(cudaMemcpyAsync(p->level_ptr_dev, p->level_ptr_host, sizeof(int) * (size_t)(levels + 1), cudaMemcpyHostToDevice, st));
   B200SP_CUDA_TRY(cudaStreamSynchronize(st));  // level_ptr_host was the source of asynchronous copies; tmp is released below
   // launch plan: runs of two or more consecutive small levels become one single-CTA launch

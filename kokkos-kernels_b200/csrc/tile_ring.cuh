@@ -201,22 +201,22 @@ __device__ __forceinline__ bool tile_row_bounds(const Ring& sm, int stage, const
 // than lmax are listed for the caller's long-row kernel.  Stream-ordered, no host synchronisation.
 // ---------------------------------------------------------------------------------------------------------------------
 struct TileAnalysis {
-  int4* tiles = nullptr;  // {r0, r1, s, e} per tile
+  DevArray<int4> tiles;  // {r0, r1, s, e} per tile
   int n_tiles = 0, T = 0, LMAX = 0;
-  int* long_rows = nullptr;  // long_cap entries, *n_long of them used
-  int* n_long = nullptr;
+  DevArray<int> long_rows;  // long_cap entries, *n_long of them used
+  DevArray<int> n_long;
   int long_cap = 0;
+  void release_long_rows(cudaStream_t st) {
+    long_rows.release(st);
+    n_long.release(st);
+  }
+  void release(cudaStream_t st) {
+    tiles.release(st);
+    release_long_rows(st);
+    n_tiles = 0;
+  }
 };
+// *out is empty on entry
 int tile_analyse(cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int cap, int lmax, TileAnalysis* out);
-
-// what plan_analyse_mm (spmv.cu) hands to the rank-2 tile kernel (spmm.cu)
-struct MMTileView {
-  const int4* tiles;  // {r0, r1, s, e} per tile
-  int n_tiles;
-  int LMAX;           // rows longer than this are left to the segment kernel
-  const int4* segs;   // {row, e0, e1, flags} (flags bit 0: row has several segments, bit 1: first segment)
-  const int* n_seg;   // device counter
-  int seg_cap;
-};
 
 }  // namespace b200sp

@@ -29,11 +29,10 @@ struct RowWindow {
 
 struct RowWindows {
   std::vector<RowWindow> win;
-  int* rel = nullptr;    // device: relative row maps of all windows
+  DevArray<int> rel;     // relative row maps of all windows
   int64_t rel_size = 0;  // ints in rel
   void release(cudaStream_t st) {
-    if (rel) cudaFreeAsync(rel, st);
-    rel = nullptr;
+    rel.release(st);
     rel_size = 0;
     win.clear();
   }
@@ -146,8 +145,8 @@ int cut_windows(cudaStream_t st, int64_t m, const int64_t* rp, const int64_t* P,
     w.rel_off = total;
     total += ((int64_t)(w.r1 - w.r0) + 1 + align - 1) & ~(int64_t)(align - 1);
   }
-  int* rel = nullptr;
-  B200SP_CUDA_TRY(cudaMallocAsync((void**)&rel, sizeof(int) * (size_t)std::max<int64_t>(total, 1), st));
+  DevArray<int> rel;
+  B200SP_CUDA_TRY(rel.alloc((size_t)std::max<int64_t>(total, 1), st));
   const int rc = [&]() -> int {
     for (const RowWindow& w : win) {
       const int64_t count = (int64_t)(w.r1 - w.r0) + 1;
@@ -157,11 +156,11 @@ int cut_windows(cudaStream_t st, int64_t m, const int64_t* rp, const int64_t* P,
     return B200SP_OK;
   }();
   if (rc) {
-    cudaFreeAsync(rel, st);
+    rel.release(st);
     return rc;
   }
   out->win = std::move(win);
-  out->rel = rel;
+  out->rel = std::move(rel);
   out->rel_size = total;
   return B200SP_OK;
 }

@@ -164,3 +164,94 @@ def test_stateless_entry_points_and_pipelines(emu, oracle):
         K.test_hostvec_pipeline_logic(emu, oracle, 4)
     with balanced(emu, "multi-GPU kernels in one process"):
         K.test_multi_gpu_kernels_single_process(emu, oracle)
+
+
+def hostvec(emu, p, mode, m, n, rp, ci, v, x, y, alpha, beta):
+    E.ok(emu.b200sp_spmv_hostvec_f64_i32(p.h, None, mode.encode(), m, n, len(ci), alpha, E.ptr(rp), E.ptr(ci), E.ptr(v), E.ptr(x), beta,
+                                         E.ptr(y)))
+
+
+def test_spmv_plan_parts_give_everything_back(emu):
+    """each part of the SpMV plan that no bracket above reaches: long-row segments, the pattern form's tile table and the cfg's
+    cut again, the rank-2 tile and split kernels, the simple host-vector path, and every part built again after invalidate"""
+    from test_emulated_kernels import env
+    import pattern_cases as PC
+
+    m, n = 9000, 7000
+    rp64, ci, v = random_crs(m, n, 9.0, seed=3, long_rows=3)
+    rp = rp64.astype(np.int32)
+    rng = np.random.default_rng(4)
+    x, xt = rng.random(n), rng.random(m)
+    with balanced(emu, "long-row segments (B200SP_SPMV_LONGROWS=seg)"), env(B200SP_SPMV_LONGROWS="seg"):
+        p = E.SpmvPlan()
+        y = np.zeros(m)
+        for _ in range(4):
+            E.spmv(p, "N", m, n, rp, ci, v, x, y, 1.0, 0.0)
+            assert p.kernel().endswith("+seg"), p.kernel()
+        p.close()
+    with balanced(emu, "pattern tile table -> cfg tile table -> pattern tile table on one plan"):
+        A = PC.lap_case("dof2")
+        ya = np.zeros(len(A[0]) - 1)
+        p = E.SpmvPlan()
+        for idx16 in (None, "0", None):
+            with env(B200SP_SPMV_IDX16=idx16, B200SP_NO_AUTOTUNE=1):
+                E.spmv(p, "N", len(A[0]) - 1, A[3], A[0], A[1], A[2], np.ones(A[3]), ya, 1.0, 0.0)
+            assert ("COLS=pat" in p.kernel()) == (idx16 is None), p.kernel()
+        p.close()
+    with balanced(emu, "rank-2 tile and split kernels (segments, chunk table)"):
+        p = E.SpmvPlan()
+        for kern in ("tile", "tilev", "split"):
+            with env(B200SP_SPMM_KERNEL=kern):
+                Y = np.zeros((m, 8))
+                E.spmm(p, "N", m, n, rp, ci, v, np.asarray(rng.random((n, 8))), Y, 1.0, 0.0)
+                assert p.kernel().startswith("spmm_" + kern[:4]), p.kernel()
+        p.close()
+    with balanced(emu, "simple host-vector path (staging vectors)"):
+        p = E.SpmvPlan()
+        for mode, xv, ylen in (("N", x, m), ("T", xt, n), ("N", x, m)):
+            hostvec(emu, p, mode, m, n, rp, ci, v, xv, np.zeros(ylen), 1.0, 0.0)
+        p.close()
+    with balanced(emu, "invalidate, then every part built again"):
+        p = E.SpmvPlan()
+        E.ok(emu.b200sp_spmv_plan_set_option(p.h, 1, 1))
+        for _ in range(2):
+            with env(B200SP_SPMV_LONGROWS="seg"):
+                for _ in range(4):
+                    E.spmv(p, "N", m, n, rp, ci, v, x, np.zeros(m), 1.0, 0.0)
+            E.spmv(p, "T", m, n, rp, ci, v, xt, np.zeros(n), 1.0, 0.0)
+            for order in "CF":
+                E.spmm(p, "N", m, n, rp, ci, v, np.asarray(rng.random((n, 5)), order=order), np.zeros((m, 5), order=order), 1.0, 0.0)
+            for kern in ("tile", "split"):
+                with env(B200SP_SPMM_KERNEL=kern):
+                    E.spmm(p, "N", m, n, rp, ci, v, rng.random((n, 8)), np.zeros((m, 8)), 1.0, 0.0)
+            hostvec(emu, p, "N", m, n, rp, ci, v, x, np.zeros(m), 1.0, 0.0)
+            E.ok(emu.b200sp_spmv_plan_invalidate(p.h, None))
+        p.close()
+
+
+def test_hostvec_pipeline_follows_col_idx(emu):
+    """one plan, one structure, three col_idx arrays: the pattern form, a copy of it at another address, and columns that only
+    qualify for the deltas; and a call on the 32-bit columns between two pattern calls, after which the plan holds both tile
+    tables.  The piece bounds follow the table each call launches on."""
+    from test_emulated_kernels import env
+    import pattern_cases as PC
+
+    rp, ci, v, ncols = PC.lap27(36, 36, 36, 2)
+    m = len(rp) - 1
+    assert len(ci) >= (1 << 22)  # the pipeline
+    assert PC.expected_cols((rp, ci, v, ncols), 512) == "pat"
+    ci_delta = PC.random_rows(rp, ncols)
+    assert PC.expected_cols((rp, ci_delta, v, ncols), 512) == "delta"
+    x = np.random.default_rng(5).uniform(-1, 1, ncols)
+    with balanced(emu, "host-vector pipeline over changing col_idx"):
+        p = E.SpmvPlan()
+        for cols, idx16 in ((ci, None), (ci, None), (ci, "0"), (ci, None), (ci.copy(), None), (ci_delta, None), (ci, None)):
+            y = np.full(m, np.nan)
+            with env(B200SP_SPMV_IDX16=idx16):
+                hostvec(emu, p, "N", m, ncols, rp, cols, v, x, y, 1.0, 0.0)
+            ref = E.SpmvPlan()
+            yr = np.full(m, np.nan)
+            E.spmv(ref, "N", m, ncols, rp, cols, v, x, yr, 1.0, 0.0)
+            ref.close()
+            assert np.array_equal(y, yr), idx16
+        p.close()

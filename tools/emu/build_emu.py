@@ -20,7 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, "kokkos-kernels_b200", "csrc")
 OUT = os.path.join(HERE, "_build")
 SOURCES = ["spmv.cu", "spmv64.cu", "spmm.cu", "spgemm.cu", "spgemm64.cu", "bspgemm.cu", "crs_utils.cu", "bsr.cu", "cg.cu", "gmres.cu", "gs.cu", "gs2.cu", "sptrsv.cu", "crs_io.cpp"]
-HEADERS = ["common.cuh", "scan.cuh", "tile_ring.cuh", "spgemm_esc.cuh", "bspgemm.cuh", "spmm_items.h", "windows64.cuh"]
+HEADERS = ["common.cuh", "scan.cuh", "tile_ring.cuh", "spgemm_esc.cuh", "bspgemm.cuh", "spmv_plan.h", "windows64.cuh"]
 
 
 def _match_back_angle(text, end):
