@@ -263,9 +263,10 @@ int b200sp_spgemm_numeric_f32_i32(b200sp_spgemm_plan* plan, void* stream, int m,
 
 /* spgemm_jacobi (sparse/src/KokkosSparse_spgemm_jacobi.hpp:25-190; native kernels
  * sparse/impl/KokkosSparse_spgemm_jacobi_{sparseacc,denseacc,seq}_impl.hpp): C = (I - omega * diag(dinv) * A) * B
- * = B - omega*dinv_i*(A*B)_i row by row, on the structure spgemm_symbolic computed for A*B with the same plan (A is
- * square and holds its diagonal, so that row i of B lies inside the pattern of row i of A*B -- the reference's
- * kernels assume the same; rows that violate it are completed without writing past their extent).  dinv has m
+ * = B - omega*dinv_i*(A*B)_i row by row, on the structure spgemm_symbolic computed for A*B with the same plan.  A is
+ * square; when it holds its diagonal, row i of B lies inside the pattern of row i of A*B.  A row of A without its
+ * diagonal gives C restricted to the pattern of A*B: the entries of row i of B outside that pattern are dropped, and a
+ * row whose pattern is empty stays empty (the reference's kernels assume the diagonal and write past the row).  dinv has m
  * entries (the reference passes an m x 1 view).  C rows come out sorted.  B200SP_ERR_STATE without a prior
  * symbolic.  Asynchronous on `stream`. */
 int b200sp_spgemm_jacobi_f64_i32(b200sp_spgemm_plan* plan, void* stream, int m, int n, int k,
@@ -337,6 +338,13 @@ int b200sp_spgemm_numeric_f32_i64(b200sp_spgemm_plan* plan, void* stream, int m,
  * default); smaller limits only make sense for tests.  _windows: the windows of the last 64-bit symbolic (0 for none). */
 int b200sp_spgemm_plan_set_window(b200sp_spgemm_plan* plan, int64_t max_entries);
 int b200sp_spgemm_plan_windows(const b200sp_spgemm_plan* plan);
+/* Rows per kernel path of the last symbolic and the last numeric or jacobi call on this plan, summed over the windows of a
+ * product with 64-bit offsets, written to counts[0 .. n-1] (counters past the 13th are 0): [0..3] the expand / sort /
+ * compress bins, [4] the symbolic hash bin, [5] the symbolic bitmap, [6..10] the numeric hash bins of the last numeric or
+ * jacobi call, [11] its fallback rows too long for shared memory, [12] its rows handed to the fallback at run time (hash
+ * table overflow, or a jacobi row whose row of B leaves the pattern).  Counters 6..12 are 0 before the first numeric call.
+ * Synchronises the device. */
+int b200sp_spgemm_plan_paths(const b200sp_spgemm_plan* plan, int64_t* counts, int n);
 
 /* ---- CrsMatrix utilities either side of the hot path (SURVEY.md section 8f) ----------------- */
 /* sort_crs_matrix / sort_crs_graph (sparse/src/KokkosSparse_SortCrs.hpp:43-120,209-270): every row

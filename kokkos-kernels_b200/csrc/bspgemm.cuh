@@ -16,6 +16,8 @@ void bsp_state_free(BspState* s, cudaStream_t st);
 struct Spgemm64State;
 bool spgemm64_holds_product(const Spgemm64State* s);  // a 64-bit symbolic completed on the plan
 void spgemm64_state_free(Spgemm64State* s, cudaStream_t st);
+int spgemm64_window_count(const Spgemm64State* s);                          // windows of the last 64-bit symbolic
+const b200sp_spgemm_plan* spgemm64_window_plan(const Spgemm64State* s, int w);  // the 32-bit plan of window w
 
 struct SpgemmPlanView {
   bool symbolic_done;

@@ -666,7 +666,8 @@ __global__ void __launch_bounds__(G <= 32 ? 256 : G)
   }
   gsync();
   const int cmin = work ? cmin_arr[i] : 0;
-  const long long span = work ? ((long long)cmax_arr[i] - cmin + 1) : 1;
+  const int cmax = work ? cmax_arr[i] : 0;
+  const long long span = work ? ((long long)cmax - cmin + 1) : 1;
   const bool dense = span <= KSLOTS;
   const unsigned long long mult = dense ? 0ull : (((unsigned long long)KSLOTS << 32) / (unsigned long long)span);
   const int a0 = work ? rpA[i] : 0, a1 = work ? rpA[i + 1] : 0;
@@ -684,6 +685,12 @@ __global__ void __launch_bounds__(G <= 32 ? 256 : G)
     if (PCAP > 0 && staged) {
       pcol[id] = c;
       pval[id] = v;
+    }
+    if (JAC && (c < cmin || c > cmax)) {
+      // a column of row i of B outside the span of A*B's row (A without its diagonal): it has no slot in the table; the
+      // row goes to the fallback kernel, which drops such columns
+      sm_flag[g] = 1;
+      return;
     }
     int h = slot_of(c);
     while (true) {
@@ -815,9 +822,11 @@ __global__ void __launch_bounds__(G <= 32 ? 256 : G)
     for (int q = tg; q < nz; q += G) vC[cbase + q] = vals[q];
 }
 
-// spgemm_jacobi rows that do not fit shared memory (or overflowed): num_fallback_kernel with row i of B
-// inserted first and A's values scaled by -omega*dinv[i] (kept separate from the validated fallback kernel
-// until it has had its own GPU run)
+// spgemm_jacobi rows that do not fit shared memory, overflowed, or whose row i of B brought columns outside the symbolic
+// pattern: num_fallback_kernel with A's values scaled by -omega*dinv[i], then row i of B added where its column is in the
+// pattern.  The products go in first: their distinct columns ARE the symbolic pattern, so at most nz keys enter a table of
+// at least 2*nz slots and every probe ends.  Row i of B only looks its columns up and drops the ones it does not find: for
+// an A without its diagonal the row is C restricted to the pattern of A*B.
 template <typename S>
 __global__ void __launch_bounds__(256)
     num_fallback_jacobi_kernel(const int* __restrict__ fb_rows, const int* __restrict__ fb_count, int log2slots,
@@ -846,9 +855,9 @@ __global__ void __launch_bounds__(256)
     const S mult = -omega * dinv[i];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int a0 = rpA[i], a1 = rpA[i + 1];
-    for (int ja = a0 - 1 + warp; ja < a1; ja += 8) {  // index a0 - 1: row i of B itself, weight 1
-      const int ca = ja < a0 ? i : ciA[ja];
-      const S va = ja < a0 ? S(1) : vA[ja] * mult;
+    for (int ja = a0 + warp; ja < a1; ja += 8) {
+      const int ca = ciA[ja];
+      const S va = vA[ja] * mult;
       for (int jb = rpB[ca] + lane; jb < rpB[ca + 1]; jb += 32) {
         const int c = ciB[jb];
         const S v = vB[jb] * va;
@@ -866,11 +875,20 @@ __global__ void __launch_bounds__(256)
       }
     }
     __syncthreads();
+    // row i of B, weight 1: lookups only (the table holds at most nz keys, so an absent column meets an empty slot)
+    for (int jb = rpB[i] + threadIdx.x; jb < rpB[i + 1]; jb += 256) {
+      const int c = ciB[jb];
+      size_t h = hash_mul(c, lg);
+      int kcur;
+      while ((kcur = keys[h]) != c && kcur != EMPTY) h = (h + 1) & (tsz - 1);
+      if (kcur == c) atomicAdd(&vals[h], vB[jb]);
+    }
+    __syncthreads();
     for (size_t s = threadIdx.x; s < tsz; s += 256) {
       const int key = keys[s];
       if (key != EMPTY) {
         const int p = atomicAdd(&cursor, 1);
-        if (p < nz) {  // more distinct columns than the symbolic pattern holds = precondition violated: drop, do not corrupt
+        if (p < nz) {  // a structure other than the symbolic phase's: drop, do not write past the row
           ciC[cbase + p] = key;
           vC[cbase + p] = vals[s];
         }
@@ -1001,6 +1019,8 @@ static constexpr int kFbCtas = 16;
 static const int kEscThr[] = {256, 1024, 4096, 8192};
 static constexpr int kEscBins = 4;
 static constexpr int kEscCap = 8192;
+// b200sp_spgemm_plan_paths: ESC bins, symbolic hash bin, bitmap, numeric hash bins, static and overflowed fallback rows
+static constexpr int kSpgemmPaths = kEscBins + 2 + kNumBins + 1;
 
 struct b200sp_spgemm_plan {
   bool symbolic_done = false;
@@ -1020,6 +1040,7 @@ struct b200sp_spgemm_plan {
   bool all_built = false;
   const int* cur_rows = nullptr;  // the grouping the hash-kernel launchers read (num_rows or all_rows)
   const int* cur_off = nullptr;
+  const int* last_off = nullptr;  // the grouping of the last numeric / jacobi call (num_off or all_off), for plan_paths
   b200sp::DevArray<int> esc_key;   // per row: max(products, 2 nnz(A_i))
   b200sp::DevArray<int> esc_rows;  // rows grouped by ESC bin
   int esc_off[kEscBins + 3] = {0};
@@ -1042,6 +1063,7 @@ static void spgemm_release(b200sp_spgemm_plan* p, cudaStream_t st) {
   p->all_built = false;
   p->cur_rows = nullptr;
   p->cur_off = nullptr;
+  p->last_off = nullptr;
   bsp_state_free(p->bsp, st);
   p->bsp = nullptr;
   p->symbolic_done = false;
@@ -1229,6 +1251,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
     set_error("spgemm_numeric: dimensions (%d,%d,%d) differ from symbolic (%d,%d,%d)", m, n, k, p->m, p->n, p->k);
     return B200SP_ERR_STATE;
   }
+  p->last_off = nullptr;
   if (m == 0 || p->c_nnz == 0) return B200SP_OK;
   B200SP_REQUIRE(rpA && ciA && vA && rpB && ciB && vB && rpC && ciC && vC, "spgemm_numeric: null pointer argument");
   // fallback scratch for values (type-dependent; keys were sized in symbolic)
@@ -1259,6 +1282,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
     if (rc) return rc;
     if ((rc = launch_esc_num<S, 512, 8, 12, 2>(st, p, 2, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
     if ((rc = launch_esc_num<S, 1024, 8, 13, 1>(st, p, 3, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
+    p->last_off = p->num_off;
     if (p->esc_off[kEscBins] < m) {
       p->cur_rows = p->num_rows;
       p->cur_off = p->num_off;
@@ -1277,6 +1301,7 @@ static int numeric_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, in
   if ((rc = ensure_all_bins(p, st, rpC))) return rc;
   p->cur_rows = p->all_rows;
   p->cur_off = p->all_off;
+  p->last_off = p->all_off;
   if (variant == 6) {  // variant 5 + occupancy words from 16-byte key loads and a scan that keeps every warp busy
 #define NUM6(B, G, KS, PAD, VCAP)                                                                                 \
   if ((rc = launch_num2<S, G, KS, PAD, VCAP, 0, true, false, true>(st, p, B, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC))) return rc;
@@ -1365,6 +1390,7 @@ static int jacobi_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int
     return B200SP_ERR_STATE;
   }
   B200SP_REQUIRE(m == n, "spgemm_jacobi: C = (I - omega D^-1 A) B needs a square A (m = %d, n = %d)", m, n);
+  p->last_off = nullptr;
   if (m == 0 || p->c_nnz == 0) return B200SP_OK;
   B200SP_REQUIRE(rpA && ciA && vA && rpB && ciB && vB && rpC && ciC && vC && dinv, "spgemm_jacobi: null pointer argument");
   const size_t need = sizeof(S) * (size_t)kFbCtas * ((size_t)1 << p->fb_log2);
@@ -1374,6 +1400,7 @@ static int jacobi_impl(b200sp_spgemm_plan* p, cudaStream_t st, int m, int n, int
   if ((rc = ensure_all_bins(p, st, rpC))) return rc;
   p->cur_rows = p->all_rows;
   p->cur_off = p->all_off;
+  p->last_off = p->all_off;
 #define NUMJ(B, G, KS, PAD, VCAP)                                                                                       \
   if ((rc = launch_num2<S, G, KS, PAD, VCAP, 0, false, true>(st, p, B, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC, omega, \
                                                             dinv)))                                                     \
@@ -1437,6 +1464,7 @@ int b200sp_spgemm_symbolic_i32(b200sp_spgemm_plan* p, void* stream, int m, int n
   p->rpA = rpA; p->ciA = ciA; p->rpB = rpB; p->ciB = ciB;
   p->c_nnz = 0; p->c_max = 0; p->fb_static = 0;
   for (int b = 0; b <= kNumBins; ++b) p->num_off[b] = 0;
+  for (int b = 0; b < kEscBins + 3; ++b) p->esc_off[b] = 0;
 
   // degenerate shapes: zero row_ptr, c_nnz = 0 (symbolic_spec.hpp:101-107, numeric_tpl_spec_decl.hpp:55-68)
   int64_t nnzA = 0, nnzB = 0;
@@ -1672,6 +1700,28 @@ int b200sp_spgemm_numeric_f32_i32(b200sp_spgemm_plan* plan, void* stream, int m,
                                   const int* ciA, const float* vA, const int* rpB, const int* ciB, const float* vB,
                                   const int* rpC, int* ciC, float* vC) {
   return numeric_impl<float>(plan, (cudaStream_t)stream, m, n, k, rpA, ciA, vA, rpB, ciB, vB, rpC, ciC, vC);
+}
+
+int b200sp_spgemm_plan_paths(const b200sp_spgemm_plan* plan, int64_t* counts, int n) {
+  B200SP_REQUIRE(plan != nullptr && (counts != nullptr || n <= 0), "spgemm_plan_paths: null argument");
+  int64_t c[kSpgemmPaths] = {0};
+  // a product with 64-bit offsets: the sum over the plans of its windows
+  const bool wide = spgemm64_holds_product(plan->s64);
+  const int nplans = wide ? spgemm64_window_count(plan->s64) : 1;
+  for (int w = 0; w < nplans; ++w) {
+    const b200sp_spgemm_plan* p = wide ? spgemm64_window_plan(plan->s64, w) : plan;
+    if (!p->symbolic_done) continue;
+    for (int b = 0; b < kEscBins + 2; ++b) c[b] += p->esc_off[b + 1] - p->esc_off[b];
+    if (!p->last_off) continue;
+    for (int b = 0; b < kNumBins; ++b) c[kEscBins + 2 + b] += p->last_off[b + 1] - p->last_off[b];
+    // the run-time overflows: rows the shared-memory kernels appended to the fallback list after the static ones
+    int fb = p->fb_static;
+    B200SP_CUDA_TRY(cudaDeviceSynchronize());
+    B200SP_CUDA_TRY(cudaMemcpy(&fb, p->fb_count.ptr, sizeof(int), cudaMemcpyDeviceToHost));
+    c[kSpgemmPaths - 1] += fb - p->fb_static;
+  }
+  for (int i = 0; i < n; ++i) counts[i] = i < kSpgemmPaths ? c[i] : 0;
+  return B200SP_OK;
 }
 
 }  // extern "C"

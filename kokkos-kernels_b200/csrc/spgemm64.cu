@@ -230,6 +230,10 @@ int numeric64(b200sp_spgemm_plan* p, void* stream, int m, int n, int k, const in
 
 bool spgemm64_holds_product(const Spgemm64State* s) { return s && s->done; }
 
+int spgemm64_window_count(const Spgemm64State* s) { return s ? (int)s->plans.size() : 0; }
+
+const b200sp_spgemm_plan* spgemm64_window_plan(const Spgemm64State* s, int w) { return s->plans[(size_t)w]; }
+
 void spgemm64_state_free(Spgemm64State* s, cudaStream_t st) {
   if (!s) return;
   release_windows(s, st);

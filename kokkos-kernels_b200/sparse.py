@@ -762,6 +762,17 @@ class SPGEMMHandle:
         """Windows of the last symbolic on 64-bit offsets (0 otherwise)."""
         return _lib.sparse().b200sp_spgemm_plan_windows(self._plan)
 
+    PATHS = ("esc0", "esc1", "esc2", "esc3", "sym_hash", "sym_bitmap", "hash0", "hash1", "hash2", "hash3", "hash4",
+             "fallback", "overflow")
+
+    def paths(self):
+        """Rows per kernel path of the last symbolic and numeric (or jacobi) call, as a dict keyed by PATHS: the expand /
+        sort / compress bins, the symbolic hash bin and bitmap, the numeric hash bins, the fallback rows too long for
+        shared memory and the rows handed to the fallback at run time.  Synchronises the device."""
+        counts = (C.c_int64 * len(self.PATHS))()
+        check(_lib.sparse().b200sp_spgemm_plan_paths(self._plan, counts, len(self.PATHS)))
+        return dict(zip(self.PATHS, counts))
+
     def __del__(self):
         try:
             if self._plan:
@@ -938,7 +949,8 @@ def spgemm_numeric(kh, A, Amode, B, Bmode, Cm):
 def spgemm_jacobi(kh, A, Amode, B, Bmode, Cm, omega, dinv):
     """KokkosSparse::Experimental::spgemm_jacobi (sparse/src/KokkosSparse_spgemm_jacobi.hpp:25-190):
     C = (I - omega * diag(dinv) * A) * B on the structure spgemm_symbolic(kh, A, B) produced; dinv has one entry
-    per row (the reference passes an m x 1 view)."""
+    per row (the reference passes an m x 1 view).  A row of A without its diagonal gives C restricted to the pattern of
+    A*B: the entries of row i of B outside it are dropped, and a row whose pattern is empty stays empty."""
     if Amode or Bmode:
         raise B200SparseError("KokkosSparse::spgemm_jacobi: transposing A or B is not supported")
     if any(t.dtype == torch.int64 for t in (A.row_map, B.row_map, Cm.row_map)):

@@ -169,6 +169,18 @@ def spgemm(A, B, m, n, k, dtype):
         ok(L.b200sp_spgemm_plan_destroy(h, None))
 
 
+PATHS = ("esc0", "esc1", "esc2", "esc3", "sym_hash", "sym_bitmap", "hash0", "hash1", "hash2", "hash3", "hash4", "fallback",
+         "overflow")
+
+
+def spgemm_paths(h):
+    """b200sp_spgemm_plan_paths of a plan handle (c_void_p) as a dict keyed by PATHS (kokkos_kernels_b200.sparse's
+    SPGEMMHandle.PATHS)."""
+    counts = (C.c_int64 * len(PATHS))()
+    ok(lib().b200sp_spgemm_plan_paths(h, counts, len(PATHS)))
+    return dict(zip(PATHS, counts))
+
+
 class BsrPlan:
     def __init__(self):
         self.h = C.c_void_p()

@@ -210,3 +210,143 @@ def assert_within(got, exact, bound, what):
         r, c = (int(t) for t in np.argwhere(bad)[0])
         raise AssertionError(f"{what}: {int(bad.sum())} entries off; first at row {r}, column {c}: got {got[r, c]!r}, "
                              f"exact {exact[r, c]!r}, error {float(err[r, c]):.3e}, bound {float(bound[r, c]):.3e}")
+
+
+# ---- SpGEMM: C = A*B and spgemm_jacobi's C = B - omega*diag(dinv)*A*B ----------------------------------------------------
+def product_rows(A, B):
+    """Products per row of A*B (int64)."""
+    rpA, ciA = np.asarray(A[0], dtype=np.int64), np.asarray(A[1], dtype=np.int64)
+    lenB = np.diff(np.asarray(B[0], dtype=np.int64))
+    per_entry = lenB[ciA]
+    cum = np.concatenate([[0], np.cumsum(per_entry)])
+    return cum[rpA[1:]] - cum[rpA[:-1]]
+
+
+def _spgemm_parts(A, B, omega=None, dinv=None):
+    """Structure of A*B with, per entry, the wide sum, the number n_ij of products that land on it and the sum of their
+    magnitudes (float64).  With omega / dinv: the sums are of -omega*dinv_i*a_ik*b_kj plus b_ij where (i, j) is in the
+    pattern of A*B, and the magnitudes include |b_ij|.  Rows are expanded in blocks of at most _CHUNK products, each block
+    sorted by (row, column); nothing of size k is allocated."""
+    rpA, ciA, vA = (np.asarray(x) for x in A)
+    rpB, ciB, vB = (np.asarray(x) for x in B)
+    dtype = vA.dtype
+    dt = wide(dtype)
+    m = len(rpA) - 1
+    rpA64, rpB64 = rpA.astype(np.int64), rpB.astype(np.int64)
+    lenB = np.diff(rpB64)
+    per_entry = lenB[ciA.astype(np.int64)]
+    cumE = np.concatenate([[0], np.cumsum(per_entry)])  # products before entry e of A
+    prow = cumE[rpA64]  # products before row i
+    ncol = int(ciB.max()) + 1 if len(ciB) else 1
+    jac = omega is not None
+    if jac:
+        wrow = -(dt(np.asarray(omega, dtype=dtype)) * np.asarray(dinv, dtype=dtype).astype(dt))  # -omega*dinv_i, wide
+    out_len = np.zeros(m, dtype=np.int64)
+    cols, vals, cnts, scales = [], [], [], []
+    r0 = 0
+    while r0 < m:
+        r1 = int(np.searchsorted(prow, prow[r0] + _CHUNK, side="right")) - 1
+        r1 = min(max(r1, r0 + 1), m)
+        e0, e1 = int(rpA64[r0]), int(rpA64[r1])
+        cnt = per_entry[e0:e1]
+        P = int(cnt.sum())
+        ent = np.repeat(np.arange(e0, e1, dtype=np.int64), cnt)  # entry of A of each product
+        within = np.arange(P, dtype=np.int64) - np.repeat(cumE[e0:e1] - cumE[e0], cnt)
+        bidx = rpB64[ciA[ent].astype(np.int64)] + within
+        arow = np.repeat(np.arange(r0, r1, dtype=np.int64), np.diff(rpA64[r0:r1 + 1]))
+        row = np.repeat(arow - r0, cnt)
+        col = ciB[bidx].astype(np.int64)
+        a = vA[ent].astype(dt)
+        if jac:
+            a = wrow[row + r0] * a
+        term = a * vB[bidx].astype(dt)
+        mag = np.abs(term.astype(np.float64))
+        key = row * ncol + col
+        order = np.argsort(key, kind="stable")
+        key, term, mag = key[order], term[order], mag[order]
+        first = np.flatnonzero(np.concatenate([[True], key[1:] != key[:-1]])) if P else np.zeros(0, np.int64)
+        ukey = key[first]
+        s = np.add.reduceat(term, first) if P else np.zeros(0, dt)
+        sc = np.add.reduceat(mag, first) if P else np.zeros(0)
+        n = np.diff(np.concatenate([first, [P]]))
+        urow, ucol = ukey // ncol, ukey % ncol
+        if jac:  # row i of B, weight 1, where its column is in the pattern
+            b0, b1 = int(rpB64[min(r0, len(rpB64) - 1)]), int(rpB64[min(r1, len(rpB64) - 1)])
+            brow = np.repeat(np.arange(r0, min(r1, len(rpB64) - 1), dtype=np.int64), lenB[r0:r1]) - r0
+            bkey = brow * ncol + ciB[b0:b1].astype(np.int64)
+            pos = np.searchsorted(ukey, bkey)
+            hit = pos < len(ukey)
+            hit[hit] = ukey[pos[hit]] == bkey[hit]
+            s[pos[hit]] += vB[b0:b1][hit].astype(dt)  # columns are distinct within a row of B
+            sc[pos[hit]] += np.abs(vB[b0:b1][hit].astype(np.float64))
+        out_len[r0:r1] = np.bincount(urow, minlength=r1 - r0)
+        cols.append(ucol.astype(np.int32))
+        vals.append(s.astype(dt))
+        cnts.append(n)
+        scales.append(sc)
+        r0 = r1
+    rp = np.concatenate([[0], np.cumsum(out_len)])
+    assert rp[-1] < 2**31
+    cat = lambda xs, t: np.concatenate(xs) if xs else np.zeros(0, t)
+    return rp.astype(np.int32), cat(cols, np.int32), cat(vals, dt), cat(cnts, np.int64), cat(scales, np.float64)
+
+
+def spgemm_exact(A, B):
+    """C = A*B for A = (row_map, entries, values), B likewise: (row_map, entries, values) with sorted rows, the values in the
+    wide format of A's dtype.  Every product (i, c, a*b) is expanded, sorted by (row, column) and reduced; an entry whose
+    products cancel to 0 stays in the structure, as in the library's symbolic phase."""
+    rp, ci, v, _, _ = _spgemm_parts(A, B)
+    return rp, ci, v
+
+
+def spgemm_bound(A, B):
+    """Per entry of spgemm_exact: gamma(n_ij + 2, u) * S_ij + gamma(n_ij + 1, u_w) * S_ij, S_ij = sum |a_ik b_kj| over the
+    n_ij products that land on (i, j) (not the row's maximum), u the unit roundoff of the data and u_w that of the wide
+    format.
+
+    Derivation (as spmm_bound's).  Each product b_kj*a_ik is rounded once.  However the kernel groups the additions -- a
+    sorted run added left to right, a shared-memory atomicAdd per product onto a zero slot, a global hash slot -- they form
+    a tree over the n_ij products, plus at most one addition onto the initial +0 (exact, but counted), so each product
+    passes through at most n_ij rounded additions: n_ij + 1 roundings in all, a factor (1 + theta), |theta| <=
+    gamma(n_ij + 1).  One spare rounding gives n_ij + 2.  The wide reference rounds each product at most once (fp64 data in
+    long double) and its sorted sum has n_ij - 1 additions: gamma_w(n_ij + 1) covers it, so the bound holds against the
+    reference and not only against the exact product.  Underflow is not modelled."""
+    _, _, _, n, S = _spgemm_parts(A, B)
+    return _spgemm_factor(A[2].dtype, n, 2, 1) * S
+
+
+def _spgemm_factor(dtype, n, extra, extra_w):
+    n = n.astype(np.float64)
+    return gamma(n + extra, unit_roundoff(dtype)) + gamma(n + extra_w, unit_roundoff(wide(dtype)))
+
+
+def spgemm_ref(A, B):
+    """(row_map, entries, exact values, bound) in one expansion."""
+    rp, ci, v, n, S = _spgemm_parts(A, B)
+    return rp, ci, v, _spgemm_factor(A[2].dtype, n, 2, 1) * S
+
+
+def jacobi_exact(A, B, omega, dinv):
+    """spgemm_jacobi's C = B - omega*diag(dinv)*A*B on the pattern of A*B (the library's symbolic structure): entry (i, j)
+    is b_ij (0 where B has no entry) - omega*dinv_i*sum_k a_ik b_kj.  omega and dinv are rounded to the data type first, as
+    the library receives them.  Where A lacks its diagonal, entries of row i of B outside the pattern are dropped."""
+    rp, ci, v, _, _ = _spgemm_parts(A, B, omega, dinv)
+    return rp, ci, v
+
+
+def jacobi_bound(A, B, omega, dinv):
+    """Per entry of jacobi_exact: gamma(n_ij + 4, u) * S_ij + gamma(n_ij + 4, u_w) * S_ij, S_ij = |b_ij| + sum |omega dinv_i
+    a_ik b_kj| over the n_ij products of A*B on (i, j).
+
+    Each product carries three roundings -- mult = -omega*dinv[i], a*mult, b*(a*mult) -- and b_ij none (weight 1); the
+    n_ij + 1 terms meet in a tree of at most n_ij rounded additions (plus the exact one onto +0), so every term is within
+    gamma(n_ij + 3) relatively; one spare rounding gives n_ij + 4.  The wide reference rounds each product at most three
+    times and adds n_ij times: gamma_w(n_ij + 4) covers it."""
+    _, _, _, n, S = _spgemm_parts(A, B, omega, dinv)
+    return _spgemm_factor(A[2].dtype, n, 4, 4) * S
+
+
+def jacobi_ref(A, B, omega, dinv):
+    """(row_map, entries, exact values, bound) in one expansion."""
+    rp, ci, v, n, S = _spgemm_parts(A, B, omega, dinv)
+    return rp, ci, v, _spgemm_factor(A[2].dtype, n, 4, 4) * S

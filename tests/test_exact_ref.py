@@ -228,3 +228,156 @@ def test_assert_within_special_values():
     for bad in ([[np.nan, np.inf, np.nan]], [[1.0, -np.inf, np.nan]], [[1.0, np.inf, 0.0]], [[np.inf, np.inf, np.nan]]):
         with pytest.raises(AssertionError, match="row 0"):
             R.assert_within(np.array(bad), exact, bound, "special")
+
+
+# ---- SpGEMM and spgemm_jacobi ---------------------------------------------------------------------------------------------
+def _spgemm_pair(rng, dtype, square=False, cancel=True):
+    """A (m x n) and B (n x k) with distinct sorted columns per row, mixed-sign values; a few pairs of equal B rows that A
+    weights +a and -a (entries that cancel exactly)."""
+    m, n, k = (int(rng.integers(5, 40)),) * 3 if square else tuple(int(x) for x in rng.integers(5, 40, 3))
+    if square:
+        n = k = m
+
+    def rows(nr, nc, lo, hi):
+        cols = [np.sort(rng.choice(nc, min(nc, int(rng.integers(lo, hi))), replace=False)) for _ in range(nr)]
+        rp = np.concatenate([[0], np.cumsum([len(c) for c in cols])]).astype(np.int32)
+        ci = np.concatenate(cols).astype(np.int32) if cols else np.zeros(0, np.int32)
+        return rp, ci, spmm_cases._values(rng, len(ci), dtype)
+
+    A = rows(m, n, 0, 9)
+    B = rows(n, k, 0, 9)
+    if square:  # the whole diagonal
+        cols = [np.union1d(A[1][A[0][i]:A[0][i + 1]], [i]) for i in range(m)]
+        rp = np.concatenate([[0], np.cumsum([len(c) for c in cols])]).astype(np.int32)
+        A = (rp, np.concatenate(cols).astype(np.int32), spmm_cases._values(rng, int(rp[-1]), dtype))
+    if cancel and n >= 2:  # B row 1 = B row 0; every row of A holding both weights them +a, -a
+        rpB, ciB, vB = B
+        r0 = (ciB[rpB[0]:rpB[1]], vB[rpB[0]:rpB[1]])
+        cols = [r0[0] if j == 1 else ciB[rpB[j]:rpB[j + 1]] for j in range(n)]
+        vals = [r0[1] if j == 1 else vB[rpB[j]:rpB[j + 1]] for j in range(n)]
+        B = (np.concatenate([[0], np.cumsum([len(c) for c in cols])]).astype(np.int32), np.concatenate(cols).astype(np.int32),
+             np.concatenate(vals).astype(dtype))
+        rpA, ciA, vA = A
+        vA = vA.copy()
+        for i in range(m):
+            seg = slice(rpA[i], rpA[i + 1])
+            c = ciA[seg]
+            if 0 in c and 1 in c:
+                vA[seg][np.flatnonzero(c == 1)[0]] = -vA[seg][np.flatnonzero(c == 0)[0]]
+        A = (rpA, ciA, vA)
+    return A, B, m, n, k
+
+
+def _kernel_like(A, B, dtype, rng, omega=None, dinv=None, mutate=None):
+    """C in the data's own precision the way a kernel may compute it: every product rounded, each entry's products added
+    in a random order from +0.  mutate(i, j, terms) may change one entry's list of (kind, value) terms."""
+    rp, ci, _ = R.spgemm_exact(A, B)
+    out = np.zeros(len(ci), dtype=dtype)
+    rpA, ciA, vA = A
+    rpB, ciB, vB = B
+    for i in range(len(rpA) - 1):
+        terms = {}
+        mult = None if omega is None else dtype(-dtype(omega) * dinv[i])
+        for e in range(rpA[i], rpA[i + 1]):
+            a = vA[e] if mult is None else dtype(vA[e] * mult)
+            for f in range(rpB[ciA[e]], rpB[ciA[e] + 1]):
+                terms.setdefault(int(ciB[f]), []).append(("p", dtype(vB[f] * a)))
+        if omega is not None:
+            for f in range(rpB[i], rpB[i + 1]):
+                if int(ciB[f]) in terms:
+                    terms[int(ciB[f])].append(("b", vB[f]))
+        for q in range(rp[i], rp[i + 1]):
+            t = terms[int(ci[q])]
+            if mutate is not None:
+                t = mutate(i, int(ci[q]), list(t))
+            acc = dtype(0)
+            for j in rng.permutation(len(t)):
+                acc = dtype(acc + t[j][1])
+            out[q] = acc
+    return out
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+def test_spgemm_exact_structure_and_values(oracle, dtype):
+    """Structure equal to the oracle's SpGEMM and spgemm_jacobi; fp32 values equal scipy's float64 product of the same data
+    (every fp32 product is exact in float64)."""
+    import scipy.sparse as ss
+
+    rng = np.random.default_rng(31)
+    for it in range(40):
+        square = it % 2 == 1
+        A, B, m, n, k = _spgemm_pair(rng, dtype, square)
+        rp, ci, v = R.spgemm_exact(A, B)
+        assert v.dtype == R.wide(dtype)
+        exp = oracle.spgemm(*A, *B, k)
+        assert np.array_equal(exp[0], rp) and np.array_equal(exp[1], ci)
+        if dtype == np.float32:
+            sA = ss.csr_matrix((A[2].astype(np.float64), A[1], A[0]), shape=(m, n))
+            sB = ss.csr_matrix((B[2].astype(np.float64), B[1], B[0]), shape=(n, k))
+            S, M = (sA @ sB).toarray(), (abs(sA) @ abs(sB)).toarray()  # scipy's float64 sums, and their scale
+            D = np.zeros((m, k))
+            D[np.repeat(np.arange(m), np.diff(rp)), ci] = v
+            assert (np.abs(D - S) <= 1e-14 * M).all()
+        if square:
+            dinv = spmm_cases._values(rng, m, dtype)
+            rpj, cij, vj = R.jacobi_exact(A, B, 0.7, dinv)
+            expj = oracle.spgemm_jacobi(*A, *B, k, dtype(0.7), dinv)
+            assert np.array_equal(expj[0], rpj) and np.array_equal(expj[1], cij)
+
+
+def test_spgemm_exact_keeps_cancelled_entries():
+    rng = np.random.default_rng(4)
+    A = (np.array([0, 2], np.int32), np.array([0, 1], np.int32), np.array([1.5, -1.5]))
+    v = spmm_cases._values(rng, 3, np.float64)
+    B = (np.array([0, 3, 6], np.int32), np.array([2, 5, 9, 2, 5, 9], np.int32), np.concatenate([v, v]))
+    rp, ci, val = R.spgemm_exact(A, B)
+    assert list(rp) == [0, 3] and list(ci) == [2, 5, 9] and not val.any()
+    assert (R.spgemm_bound(A, B) > 0).all()
+
+
+@pytest.mark.parametrize("dtype", DTYPES)
+@pytest.mark.parametrize("jacobi", [False, True])
+def test_spgemm_bound_holds_and_catches(dtype, jacobi):
+    """A kernel-like computation (rounded products, random addition order) stays within the bound; the same with one
+    product dropped, one product added twice, one product's sign flipped, or (jacobi) dinv[0] read for every row is
+    caught."""
+    rng = np.random.default_rng(17 + jacobi)
+    caught = dict(drop=0, twice=0, sign=0, dinv0=0)
+    for _ in range(25):
+        A, B, m, n, k = _spgemm_pair(rng, dtype, square=jacobi)
+        omega, dinv = (0.7, spmm_cases._values(rng, m, dtype)) if jacobi else (None, None)
+        if jacobi:
+            rp, ci, ex, bound = R.jacobi_ref(A, B, omega, dinv)
+        else:
+            rp, ci, ex, bound = R.spgemm_ref(A, B)
+        for _ in range(2):  # re-summed in other orders: within the bound
+            R.assert_within(_kernel_like(A, B, dtype, rng, omega, dinv), ex, bound, "kernel-like")
+        # the entry with the largest product relative to its scale: a single product there exceeds the bound
+        target = {}
+
+        def pick(i, j, t):
+            big = max(range(len(t)), key=lambda x: abs(float(t[x][1])))
+            if t[big][0] == "p":
+                target.setdefault((i, j), (big, abs(float(t[big][1]))))
+            return t
+
+        _kernel_like(A, B, dtype, rng, omega, dinv, pick)
+        q_of = {(i, int(c)): q for i in range(m) for q, c in zip(range(rp[i], rp[i + 1]), ci[rp[i]:rp[i + 1]])}
+        cand = [(ij, b) for ij, (b, mag) in target.items() if mag > 8 * bound[q_of[ij]]]
+        if not cand:
+            continue
+        (ti, tj), big = cand[0]
+        muts = {"drop": lambda t: t[:big] + t[big + 1:], "twice": lambda t: t + [t[big]],
+                "sign": lambda t: t[:big] + [("p", -t[big][1])] + t[big + 1:]}
+        for kind, f in muts.items():
+            bad = _kernel_like(A, B, dtype, rng, omega, dinv, lambda i, j, t: f(t) if (i, j) == (ti, tj) else t)
+            with pytest.raises(AssertionError, match=f"row {q_of[(ti, tj)]}, "):
+                R.assert_within(bad, ex, bound, kind)
+            caught[kind] += 1
+        if jacobi and m > 1 and not np.all(dinv == dinv[0]):
+            bad = _kernel_like(A, B, dtype, rng, omega, np.full(m, dinv[0], dtype))
+            with pytest.raises(AssertionError):
+                R.assert_within(bad, ex, bound, "dinv[0]")
+            caught["dinv0"] += 1
+    assert min(caught["drop"], caught["twice"], caught["sign"]) >= 10, caught
+    assert not jacobi or caught["dinv0"] >= 10, caught
