@@ -513,6 +513,10 @@ int b200sp_gs_get_coloring(const b200sp_gs_plan* plan, int* num_colors, const in
 /* The same copied to host arrays of n, num_colors + 1 and n entries (NULL: skipped); synchronises `stream`. */
 int b200sp_gs_copy_coloring(const b200sp_gs_plan* plan, void* stream, int* colors_host, int* color_ptr_host,
                             int* color_rows_host);
+/* Label of the set kernel the plan's last apply launched, with its launch count: "gs_set<f64,LPR=8>x12" ("none" before
+ * the first apply).  Lanes per row follow the average row length (B200SP_GS_LPR=2|4|8|16|32 at symbolic forces them).
+ * Static storage owned by the plan (tests). */
+const char* b200sp_gs_last_kernel(const b200sp_gs_plan* plan);
 
 /* ---- Two-stage Gauss-Seidel (SURVEY.md 8f rank 4: the Gauss-Seidel that is a loop of SpMVs) -------------------------
  * gauss_seidel_symbolic / numeric / apply with a handle created as GS_TWOSTAGE and inner Jacobi-Richardson sweeps

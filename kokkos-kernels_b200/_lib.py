@@ -117,6 +117,7 @@ SPARSE_API = {
     "b200sp_gs_apply_f32_i32": (i32, [vp, vp, i32, vp, vp, vp, vp, vp, i32, f32, i32, i32]),
     "b200sp_gs_copy_coloring": (i32, [vp, vp, vp, vp, vp]),
     "b200sp_gs_get_coloring": (i32, [vp, C.POINTER(i32), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]),
+    "b200sp_gs_last_kernel": (C.c_char_p, [vp]),
     "b200sp_pcg_solve_f64_i32": (i32, [vp, vp, vp, i32, i64, vp, vp, vp, vp, vp, i32, f64, i32, C.POINTER(i32), C.POINTER(f64)]),
     "b200sp_pcg_solve_gs2_f64_i32": (i32, [vp, vp, vp, i32, i64, vp, vp, vp, vp, vp, i32, f64, i32, C.POINTER(i32), C.POINTER(f64)]),
     "b200sp_cg_solve_f64_i32": (i32, [vp, vp, i32, i64, vp, vp, vp, vp, vp, i32, f64, i32, C.POINTER(i32), C.POINTER(f64)]),

@@ -19,6 +19,7 @@
 //     nonsymmetric matrix is coloured on the union of its pattern and its transpose's (is_graph_symmetric = 0).
 //   * same arithmetic per row as the reference, dot product split over the row's lanes and summed by shuffles.
 #include <algorithm>
+#include <cstdio>
 #include <cstdlib>
 #include <vector>
 
@@ -217,6 +218,7 @@ struct b200sp_gs_plan {
   int dinv_bytes_per = 0;
   bool symbolic_done = false, numeric_done = false;
   int lpr = 4;
+  char last_kernel[64] = "none";  // the set kernel of the last apply and its launch count (tests)
 };
 
 namespace b200sp {
@@ -277,6 +279,7 @@ int gs_apply_impl(b200sp_gs_plan* p, cudaStream_t st, int n, const int* rp, cons
   if (init_zero_x)  // all of x, ghost entries included, as the reference's zero_vector(num_cols, ...) does (gauss_seidel_impl.hpp:1426-1428)
     B200SP_CUDA_TRY(cudaMemsetAsync(x, 0, sizeof(S) * (size_t)std::max(n, p->ncols), st));
   const S* dinv = p->dinv.as<const S>();
+  int launches = 0;
   for (int s = 0; s < sweeps; ++s) {
     for (int backward = 0; backward < 2; ++backward) {
       if (!backward && direction == 2) continue;
@@ -296,9 +299,11 @@ int gs_apply_impl(b200sp_gs_plan* p, cudaStream_t st, int n, const int* rp, cons
           default: gs_set_kernel<S, 32><<<blocks, 256, 0, st>>>(p->color_rows + b, count, rp, ci, v, dinv, y, x, omega); break;
         }
         B200SP_LAUNCH_CHECK();
+        ++launches;
       }
     }
   }
+  snprintf(p->last_kernel, sizeof(p->last_kernel), "gs_set<%s,LPR=%d>x%d", sizeof(S) == 8 ? "f64" : "f32", p->lpr, launches);
   return B200SP_OK;
 }
 
@@ -439,6 +444,11 @@ int b200sp_gs_symbolic_nc_i32(b200sp_gs_plan* p, void* stream, int n, int ncols,
   B200SP_CUDA_TRY(cudaStreamSynchronize(st));
   const double avg = (double)nnz / (double)n;
   p->lpr = avg <= 8.0 ? 2 : avg <= 96.0 ? 4 : avg <= 384.0 ? 8 : avg <= 1536.0 ? 16 : 32;
+  if (const char* f = getenv("B200SP_GS_LPR")) {  // lanes per row forced (tests): 2, 4, 8, 16 or 32
+    const int l = atoi(f);
+    B200SP_REQUIRE(l == 2 || l == 4 || l == 8 || l == 16 || l == 32, "gauss_seidel_symbolic: B200SP_GS_LPR must be 2, 4, 8, 16 or 32 (got %s)", f);
+    p->lpr = l;
+  }
   p->symbolic_done = true;
   return B200SP_OK;
 }
@@ -457,6 +467,8 @@ int b200sp_gs_apply_f32_i32(b200sp_gs_plan* p, void* stream, int n, const int* r
                             const float* y, int init_zero_x, float omega, int sweeps, int direction) {
   return gs_apply_impl<float>(p, (cudaStream_t)stream, n, row_ptr, col_idx, vals, x, y, init_zero_x, omega, sweeps, direction);
 }
+
+const char* b200sp_gs_last_kernel(const b200sp_gs_plan* p) { return p ? p->last_kernel : "none"; }
 
 // colouring produced by symbolic (tests, and callers that want to reuse it): device pointers owned by the plan
 int b200sp_gs_get_coloring(const b200sp_gs_plan* p, int* num_colors, const int** colors, const int** color_ptr, const int** color_rows) {

@@ -506,6 +506,10 @@ class GaussSeidelHandle:
                                                     C.c_void_p(crows.ctypes.data)))
         return colors, cptr, crows
 
+    def last_kernel(self):
+        """Set kernel of the last apply and its launch count, e.g. "gs_set<f64,LPR=8>x12"."""
+        return _lib.sparse().b200sp_gs_last_kernel(self._plan).decode()
+
     def __del__(self):
         try:
             if self._plan:

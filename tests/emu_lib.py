@@ -311,6 +311,9 @@ class GsPlan:
         arr = lambda p, cnt: np.ctypeslib.as_array((C.c_int * cnt).from_address(p.value)).copy() if cnt else np.zeros(0, np.int32)
         return nc.value, arr(pc, n), arr(pp, nc.value + 1), arr(pr, n)
 
+    def kernel(self):
+        return lib().b200sp_gs_last_kernel(self.h).decode()
+
 
 def pcg_solve(plan, gs_plan, rp, ci, v, b, x, maximum_iteration, tolerance, check_every=0):
     it, nr = C.c_int(), C.c_double()

@@ -350,3 +350,328 @@ def jacobi_ref(A, B, omega, dinv):
     """(row_map, entries, exact values, bound) in one expansion."""
     rp, ci, v, n, S = _spgemm_parts(A, B, omega, dinv)
     return rp, ci, v, _spgemm_factor(A[2].dtype, n, 4, 4) * S
+
+
+# ---- Gauss-Seidel: one point sweep (gs.cu), and the two-stage / classic forms (gs2.cu, sptrsv.cu) --------------------------
+def _rows_of(rp):
+    rp = np.asarray(rp, dtype=np.int64)
+    return np.repeat(np.arange(len(rp) - 1, dtype=np.int64), np.diff(rp))
+
+
+def _segment_max(starts, vals, empty):
+    """out[r] = max of vals over the entries of row r (int64); `empty` for rows without entries."""
+    nrows = len(starts) - 1
+    out = np.full(nrows, empty, dtype=np.int64)
+    nz = np.flatnonzero(np.diff(starts) > 0)
+    if len(nz):
+        out[nz] = np.maximum.reduceat(np.asarray(vals, dtype=np.int64), np.asarray(starts, dtype=np.int64)[nz])
+    return out
+
+
+def _row_sums(starts, w, xe, dt):
+    """sum over the entries e of row r of w[e] * xe[e] in dt (xe already gathered per entry)."""
+    return _segment_sums(np.asarray(starts, dtype=np.int64), np.arange(len(w), dtype=np.int64), w, np.asarray(xe)[:, None], dt)[:, 0]
+
+
+def _gs_sweep_parts(rp, ci, v, colors, x_old, x_new, y, omega, direction):
+    dtype = v.dtype
+    dt = wide(dtype)
+    rp = np.asarray(rp, dtype=np.int64)
+    ci = np.asarray(ci, dtype=np.int64)
+    n = len(rp) - 1
+    row = _rows_of(rp)
+    colors = np.asarray(colors, dtype=np.int64)
+    assert direction in (1, 2), "one forward (1) or one backward (2) sweep"
+    sq = ci < n
+    cc = np.full(len(ci), -1, dtype=np.int64)
+    cc[sq] = colors[ci[sq]]
+    diag = ci == row
+    # forward: columns of an earlier colour were swept before row i and hold their new value; backward: the mirror image.
+    # The diagonal and the ghost columns read x_old.
+    newer = (cc < colors[row]) if direction == 1 else (cc > colors[row])
+    newer &= sq & ~diag
+    x_old = np.asarray(x_old)
+    xe = np.where(newer, np.asarray(x_new)[ci], x_old[ci])
+    dpiece = np.where(diag, v, 0).astype(dtype)
+    same_sign = np.ones(n, dtype=bool)
+    if diag.any():
+        pos = np.bincount(row[diag & (v > 0)], minlength=n)
+        neg = np.bincount(row[diag & (v < 0)], minlength=n)
+        same_sign = (pos == 0) | (neg == 0)
+    assert same_sign.all(), "a row's diagonal pieces must share a sign (their sum then has a relative error bound)"
+    ndiag = np.bincount(row[diag], minlength=n)
+    assert (ndiag > 0).all(), "every row needs a diagonal entry"
+    d = _row_sums(rp, dpiece, np.ones(len(ci)), dt)
+    s = _row_sums(rp, v, xe, dt)
+    om = dt(np.asarray(omega, dtype=dtype))
+    exact = x_old[:n].astype(dt) + om * (np.asarray(y).astype(dt) - s) / d
+    mag = _row_sums(rp, np.abs(v).astype(np.float64), np.abs(xe.astype(np.float64)), np.float64)
+    scale = np.abs(x_old[:n].astype(np.float64)) + abs(float(om)) / np.abs(d.astype(np.float64)) * (np.abs(np.asarray(y, np.float64)) + mag)
+    steps = np.diff(rp).astype(np.float64) + 4 + ndiag
+    bound = (gamma(steps, unit_roundoff(dtype)) + gamma(steps, unit_roundoff(dt))) * scale
+    return exact, bound
+
+
+def gs_sweep_exact(rp, ci, v, colors, x_old, x_new, y, omega, direction):
+    """Rows 0 .. n-1 of one point Gauss-Seidel sweep, each computed from the kernel's own neighbour values: row i of colour
+    c reads x_new_j where colour(j) < c (forward, direction 1) or colour(j) > c (backward, direction 2), x_old_j otherwise,
+    and x_old on its diagonal and ghost columns (j >= n).  Value x_old_i + omega * (y_i - sum_j a_ij x*_j) / d_i with d_i
+    the exact sum of the row's diagonal entries, in the wide format; omega is first rounded to v's dtype.  A local check:
+    the error of one row does not travel along the colour chain into the next one's reference."""
+    return _gs_sweep_parts(rp, ci, v, colors, x_old, x_new, y, omega, direction)[0]
+
+
+def gs_sweep_bound(rp, ci, v, colors, x_old, x_new, y, omega, direction):
+    """Per row of gs_sweep_exact: gamma(len_i + 4 + ndiag_i) * (|x_old_i| + |omega| / |d_i| * (|y_i| + sum_j |a_ij x*_j|)),
+    plus the same with the wide format's unit roundoff.
+
+    The kernel rounds each product a_ij x*_j once (or fuses it) and adds the len_i products in some tree (at most len_i
+    levels with the subtraction from y_i), multiplies by omega and by its inverse diagonal, and adds x_old_i: every term
+    passes through at most len_i + 3 roundings there.  The inverse diagonal is 1/d̂_i with d̂_i the rounded sum of ndiag_i
+    pieces of one sign: ndiag_i - 1 roundings, and one more for the division, counted as a rounding rather than reproduced,
+    so the bound holds whether or not the division is IEEE and with or without FMA contraction.  Total len_i + 4 + ndiag_i
+    - 1, one spare.  The wide reference does the same operations in its own format."""
+    return _gs_sweep_parts(rp, ci, v, colors, x_old, x_new, y, omega, direction)[1]
+
+
+_gamma_n = gamma  # the two-stage functions take a parameter named gamma
+
+
+class _Tracked:
+    """A vector of the two-stage evaluator: its value in the wide format (or the data's own, for a plain run), its magnitude
+    -- the same expression evaluated on |inputs| with every subtraction an addition -- and per entry the depth, the most
+    rounding steps on any path from an input to it.  For a straight-line program of additions, multiplications and
+    divisions by inputs, the computed value differs from the exact one by at most gamma(depth) * magnitude (Higham, lemma
+    3.1 and the bookkeeping of section 3.4, applied per monomial)."""
+
+    def __init__(self, val, mag, dep):
+        self.val, self.mag, self.dep = val, mag, np.asarray(dep, dtype=np.int64)
+
+    def copy(self):
+        return _Tracked(self.val.copy(), self.mag.copy(), self.dep.copy())
+
+
+class _Gs2Program:
+    def __init__(self, rp, ci, v, dinv, dt):
+        self.dtype = v.dtype
+        self.dt = dt
+        self.rp = np.asarray(rp, dtype=np.int64)
+        self.ci = np.asarray(ci, dtype=np.int64)
+        self.v = v
+        self.n = n = len(self.rp) - 1
+        row = self.row = _rows_of(self.rp)
+        diag = self.ci == row
+        idx = np.flatnonzero(diag)
+        r = row[idx]
+        assert len(np.unique(r)) == n, "every row needs a diagonal entry"
+        last = np.r_[r[1:] != r[:-1], True]  # numeric keeps the last diagonal entry of a row
+        a_d = np.zeros(n, dtype=self.dtype)
+        a_d[r[last]] = v[idx[last]]
+        self.Da = a_d
+        if dinv is None:  # D = 1/a_ii: one rounding
+            self.D = (dt(1) / a_d.astype(dt)), np.abs(1.0 / a_d.astype(np.float64)), 1
+        else:
+            dinv = np.asarray(dinv, dtype=self.dtype)
+            self.D = dinv.astype(dt), np.abs(dinv.astype(np.float64)), 0
+        self.given = dinv is not None
+        lower, upper, ghost = self.ci < row, (self.ci > row) & (self.ci < n), self.ci >= n
+        self.parts = {"A": np.ones(len(self.ci), dtype=bool), "L": lower, "U": upper, "La": lower | ghost, "Ua": upper | ghost}
+
+    def _sub(self, mask):
+        starts = np.zeros(self.n + 1, dtype=np.int64)
+        np.cumsum(np.bincount(self.row[mask], minlength=self.n), out=starts[1:])
+        return starts, self.ci[mask], self.v[mask], self.row[mask]
+
+    def matvec(self, part, alpha, x, y0, scaled=False):
+        """y0 + alpha * M x, M the part of A (scaled: rows times D, the values numeric stores for L and U)."""
+        starts, c, w, r = self._sub(self.parts[part])
+        dt = self.dt
+        ww, wm, wdep = w.astype(dt), np.abs(w.astype(np.float64)), 0
+        if scaled:
+            Dv, Dm, Dd = self.D
+            ww, wm, wdep = ww * Dv[r], wm * Dm[r], Dd + 1
+        al = dt(np.asarray(alpha, dtype=self.dtype))
+        with np.errstate(invalid="ignore"):
+            val = y0.val + al * _row_sums(starts, ww, x.val[c], dt)
+        mag = y0.mag + abs(float(al)) * _row_sums(starts, wm, x.mag[c], np.float64)
+        dep = np.maximum(y0.dep, _segment_max(starts, x.dep[c] + wdep, 0)) + np.diff(starts) + 4
+        return _Tracked(val, mag, dep)
+
+    def dscale(self, r):  # D .* r
+        Dv, Dm, Dd = self.D
+        return _Tracked(Dv * r.val, Dm * r.mag, r.dep + Dd + 1)
+
+    def scal(self, g, x):
+        gw = self.dt(np.asarray(g, dtype=self.dtype))
+        return _Tracked(gw * x.val, abs(float(gw)) * x.mag, x.dep + 1)
+
+    def damp(self, g, z, r):  # g z + (1 - g) r, with 1 - g rounded once
+        gw = self.dt(np.asarray(g, dtype=self.dtype))
+        hw = self.dt(1) - gw
+        return _Tracked(gw * z.val + hw * r.val, abs(float(gw)) * z.mag + abs(float(hw)) * r.mag,
+                        np.maximum(z.dep + 2, r.dep + 3))
+
+    def diag_term(self, om2, x, r):  # r + om2 * (Da .* x)
+        ow = self.dt(om2)
+        return _Tracked(r.val + ow * self.Da.astype(self.dt) * x.val[:self.n],
+                        r.mag + abs(float(ow)) * np.abs(self.Da.astype(np.float64)) * x.mag[:self.n],
+                        np.maximum(r.dep, x.dep[:self.n] + 2) + 1)
+
+    def update(self, x, z, omega, overwrite):
+        ow = self.dt(np.asarray(omega, dtype=self.dtype))
+        y = x.copy()
+        n = self.n
+        if overwrite:
+            y.val[:n], y.mag[:n], y.dep[:n] = ow * z.val, abs(float(ow)) * z.mag, z.dep + 1
+        else:
+            y.val[:n] = x.val[:n] + ow * z.val
+            y.mag[:n] = x.mag[:n] + abs(float(ow)) * z.mag
+            y.dep[:n] = np.maximum(x.dep[:n], z.dep + 1) + 1
+        return y
+
+    def trsv(self, r, forward):
+        """(L + D)^{-1} r (forward) or (U + D)^{-1} r, D the diagonal entry or 1/dinv; rows in dependency levels."""
+        dt, n = self.dt, self.n
+        starts, c, w, rr = self._sub(self.parts["L" if forward else "U"])
+        lvl = np.zeros(n, dtype=np.int64)
+        while True:  # longest chain below each row
+            nl = _segment_max(starts, lvl[c] + 1, 0)
+            if np.array_equal(nl, lvl):
+                break
+            lvl = nl
+        if self.given:
+            inv, invm = self.D[0], self.D[1]
+        else:
+            inv, invm = dt(1) / self.Da.astype(dt), np.abs(1.0 / self.Da.astype(np.float64))
+        z = _Tracked(np.zeros(n, dtype=dt), np.zeros(n), np.zeros(n, dtype=np.int64))
+        for L in range(int(lvl.max()) + 1 if n else 0):
+            rows = np.flatnonzero(lvl == L)
+            lens = starts[rows + 1] - starts[rows]
+            sub = np.zeros(len(rows) + 1, dtype=np.int64)
+            np.cumsum(lens, out=sub[1:])
+            e = np.repeat(starts[rows] - sub[:-1], lens) + np.arange(int(sub[-1]), dtype=np.int64)
+            s = _segment_sums(sub, c[e], w[e], z.val[:, None], dt)[:, 0] if len(e) else np.zeros(len(rows), dt)
+            sm = _segment_sums(sub, c[e], np.abs(w[e]).astype(np.float64), z.mag[:, None], np.float64)[:, 0] if len(e) else 0.0
+            z.val[rows] = (r.val[rows] - s) * inv[rows]
+            z.mag[rows] = (r.mag[rows] + sm) * invm[rows]
+            z.dep[rows] = np.maximum(r.dep[rows], _segment_max(sub, z.dep[c[e]] + 1, 0) if len(e) else 0) + lens + 1 + int(self.given)
+        return z
+
+
+def _gs2_run(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact, inner, outer, gamma_, two_stage, dinv, dt,
+             variant=None):
+    dtype = v.dtype
+    P = _Gs2Program(rp, ci, v, dinv, dt)
+    n = P.n
+    one = dtype.type(1)
+    om = dtype.type(omega)
+    g = dtype.type(gamma_)
+    inp = lambda a: _Tracked(np.asarray(a).astype(dt), np.abs(np.asarray(a).astype(np.float64)), np.zeros(len(a), dtype=np.int64))
+    x = inp(np.zeros(ncols, dtype) if init_zero else np.asarray(x0)[:ncols])  # init_zero: all ncols entries, ghosts included
+    bt = inp(b)
+    sweeps = max(outer, num_iter) * (2 if direction == 0 else 1)
+    for sweep in range(sweeps):
+        forward = direction == 1 or (direction == 0 and sweep % 2 == 0)
+        R = bt.copy()
+        if sweep > 0 or not init_zero:
+            if compact:
+                R = P.matvec("Ua" if forward else "La", -1.0, x, R)
+                if om != one:
+                    with np.errstate(divide="ignore"):
+                        R = P.diag_term(one / om - one, x, R)  # the scalar as the host computes it in the data's type
+            else:
+                R = P.matvec("A", -1.0, x, R)
+        if not two_stage:
+            Z = P.trsv(R, forward)
+            x = P.update(x, Z, 1.0, compact)
+            continue
+        if inner == 0:
+            Z = P.dscale(R)
+            if g != one:
+                Z = P.scal(g, Z)
+        else:
+            T = P.dscale(R)
+            R = T.copy()
+            if g != one:
+                R = P.scal(g, R)
+            for ii in range(inner):
+                Z = P.matvec("L" if forward else "U", -om, R, T, scaled=True)
+                if g != one:
+                    Z = P.damp(g, Z, Z if variant == "damp_z" else R)
+                if ii + 1 < inner:
+                    R = Z
+        x = P.update(x, Z, om, compact and variant != "accumulate")
+    return x
+
+
+def gs2_exact(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact=False, inner_sweeps=1, outer_sweeps=1, gamma=1.0,
+              two_stage=True, inverse_diagonal=None):
+    """x (ncols entries) after b200sp_gs2_apply, in the wide format, for one right-hand side.
+
+    The algorithm as the reference's TwostageGaussSeidel::apply states it (sparse/impl/KokkosSparse_twostage_gauss_seidel_impl.hpp
+    :778-1035): NumSweeps = max(outer, numIter), doubled for symmetric (forward, backward, ...); init_zero zeroes all ncols
+    entries of x, ghosts included.  Per sweep R = b - A x (compact: b - Ua x or b - La x, plus (1/omega - 1) Da.*x when
+    omega != 1; skipped on the first sweep after init_zero).  Two-stage: Z = gamma D.*R without inner sweeps; otherwise T = D.*R,
+    R = gamma T, and per inner sweep Z = T - omega (DL or DU) R, Z = gamma Z + (1 - gamma) R when gamma != 1, R = Z before the
+    next; then x += omega Z (compact: x = omega Z).  Classic (two_stage = False, omega = 1): Z = (L + D)^{-1} R or (U + D)^{-1}
+    R, then x += Z (compact: x = Z).  D = 1 / a_ii, or the caller's inverse diagonal; a_ii is the row's (last) diagonal entry.
+    omega, gamma and the inverse diagonal are first rounded to v's dtype, and 1/omega - 1 is the data-type scalar the host
+    computes, as the library receives them."""
+    return _gs2_run(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact, inner_sweeps, outer_sweeps, gamma, two_stage,
+                    inverse_diagonal, wide(v.dtype)).val
+
+
+def gs2_bound(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact=False, inner_sweeps=1, outer_sweeps=1, gamma=1.0,
+              two_stage=True, inverse_diagonal=None):
+    """Per entry of gs2_exact: (gamma(depth_i, u) + gamma(depth_i, u_w)) * magnitude_i.
+
+    The evaluator carries, with every vector, the magnitude (the program on |A|, |x|, |b|, |D|, |omega|, |gamma|, |1 - gamma|
+    with subtraction replaced by addition) and per entry the rounding depth: a product with a row of len_i entries adds len_i
+    + 4 to the deepest input of that row, as spmm_bound counts it (entries of DL and DU carry the rounding of a_ij * d_i, and
+    of d_i = 1/a_ii); a diagonal scaling, a scaling by gamma or omega, and an update add one or two; a row of the triangular
+    substitution adds its off-diagonal count, the division, and the rounding of 1/dinv when the caller supplied dinv.  The
+    bound is rigorous for any evaluation order the kernels choose; the wide reference's own error is added over the same
+    depth.  Ghost entries keep their input (depth 0, bound 0): they must come back unchanged."""
+    x = _gs2_run(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact, inner_sweeps, outer_sweeps, gamma, two_stage,
+                 inverse_diagonal, wide(v.dtype))
+    d = x.dep.astype(np.float64)
+    return (_gamma_n(d, unit_roundoff(v.dtype)) + _gamma_n(d, unit_roundoff(wide(v.dtype)))) * x.mag
+
+
+def gs2_ref(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact=False, inner_sweeps=1, outer_sweeps=1, gamma=1.0,
+            two_stage=True, inverse_diagonal=None):
+    """(gs2_exact, gs2_bound) in one evaluation."""
+    x = _gs2_run(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact, inner_sweeps, outer_sweeps, gamma, two_stage,
+                 inverse_diagonal, wide(v.dtype))
+    d = x.dep.astype(np.float64)
+    return x.val, (_gamma_n(d, unit_roundoff(v.dtype)) + _gamma_n(d, unit_roundoff(wide(v.dtype)))) * x.mag
+
+
+
+def trsv_row_bound(rp, ci, v, b, z, forward, inverse_diagonal=None):
+    """Local check of one triangular substitution from the kernel's own solution z: per row, the exact (b_i - sum_j a_ij z_j) / d_i
+    over the lower (forward) or upper off-diagonal entries (ghost columns skipped) and the bound gamma(len_i + 2) *
+    (|b_i| + sum_j |a_ij z_j|) / |d_i|, len_i the row's full length: at most len_i - 1 products and subtractions, the
+    division, and the rounding of 1/dinv.  Returns (exact, bound) for rows 0 .. n-1."""
+    dtype = v.dtype
+    dt = wide(dtype)
+    rp = np.asarray(rp, dtype=np.int64)
+    ci = np.asarray(ci, dtype=np.int64)
+    n = len(rp) - 1
+    row = _rows_of(rp)
+    take = (ci < row) if forward else ((ci > row) & (ci < n))
+    w = np.where(take, v, 0).astype(dtype)
+    zz = np.asarray(z)
+    ze = np.where(take, zz[np.minimum(ci, n - 1)], 0).astype(dtype)
+    s = _row_sums(rp, w, ze, dt)
+    sm = _row_sums(rp, np.abs(w).astype(np.float64), np.abs(ze.astype(np.float64)), np.float64)
+    P = _Gs2Program(rp, ci, v, inverse_diagonal, dt)
+    if inverse_diagonal is not None:
+        inv, invm = P.D[0], P.D[1]
+    else:
+        inv, invm = dt(1) / P.Da.astype(dt), np.abs(1.0 / P.Da.astype(np.float64))
+    bb = np.asarray(b)
+    exact = (bb.astype(dt) - s) * inv
+    steps = np.diff(rp).astype(np.float64) + 2
+    bound = (gamma(steps, unit_roundoff(dtype)) + gamma(steps, unit_roundoff(dt))) * (np.abs(bb.astype(np.float64)) + sm) * invm
+    return exact, bound

@@ -8,6 +8,7 @@ import pytest
 import scipy.sparse as sps
 
 import emu_lib as E
+import exact_ref as R
 from gmres_cases import gmres_matrix
 
 
@@ -68,6 +69,11 @@ def test_reference_unit_test_and_oracle_parity(emu, oracle, symmetric, dtype):
         tol = 1e-12 if dtype == np.float64 else 2e-5
         assert np.max(np.abs(x.astype(np.float64) - xo.astype(np.float64))) <= tol * max(1.0, np.max(np.abs(xo)))
         assert np.linalg.norm(x.astype(np.float64) - xs.astype(np.float64)) < init  # EXPECT_LT(result_norm_res, initial_norm_res)
+        if direction:  # one more sweep from here, each row within its local bound
+            x2 = x.copy()
+            assert plan.apply(n, rp, ci, v, x2, y, False, 0.9, 1, direction) == 0
+            R.assert_within(x2, R.gs_sweep_exact(rp, ci, v, colors, x, x2, y, 0.9, direction),
+                            R.gs_sweep_bound(rp, ci, v, colors, x, x2, y, 0.9, direction), plan.kernel())
     # more sweeps from the current x (init_zero_x = false) keep converging
     before = np.linalg.norm(x.astype(np.float64) - xs.astype(np.float64))
     assert plan.apply(n, rp, ci, v, x, y, False, 0.9, 3, 0) == 0

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import emu_lib as E
+import exact_ref as R
 from test_oracle_gs2 import dd_matrix
 
 
@@ -45,6 +46,8 @@ def test_oracle_parity(emu, oracle, dtype, compact):
                     assert np.array_equal(x[n:], x0[n:])  # ghosts untouched
                 err = np.max(np.abs(x.astype(np.float64) - xo.astype(np.float64)))
                 assert err <= tol * 20 * max(1.0, np.max(np.abs(xo))), (inner, gamma, outer, direction, omega, init_zero, err)
+                ex, bnd = R.gs2_ref(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact, inner, outer, gamma)
+                R.assert_within(x, ex, bnd, str((inner, gamma, outer, direction, omega, init_zero)))
         plan.close()
 
 

@@ -381,3 +381,144 @@ def test_spgemm_bound_holds_and_catches(dtype, jacobi):
             caught["dinv0"] += 1
     assert min(caught["drop"], caught["twice"], caught["sign"]) >= 10, caught
     assert not jacobi or caught["dinv0"] >= 10, caught
+
+
+# ---- Gauss-Seidel -------------------------------------------------------------------------------------------------------
+def _greedy_coloring(c):
+    """A proper colouring of A + A^T (square part), natural order, as (colors, color_ptr, color_rows)."""
+    import gs_cases as G
+
+    P = G._pattern(c)
+    P = (P + P.T).tocsr()
+    n = c["n"]
+    col = np.full(n, -1)
+    for i in range(n):
+        used = set(col[P.indices[P.indptr[i]:P.indptr[i + 1]]].tolist())
+        k = 0
+        while k in used:
+            k += 1
+        col[i] = k
+    nc = col.max() + 1
+    cptr = np.zeros(nc + 1, np.int32)
+    np.cumsum(np.bincount(col, minlength=nc), out=cptr[1:])
+    return col, cptr, np.argsort(col, kind="stable").astype(np.int32)
+
+
+def _gs_case(dtype, cancel=False):
+    import gs_cases as G
+
+    c = G.nonsymmetric_case(0.1, ghosts=7)
+    v = c["v"].astype(dtype)
+    y, x0 = G.vectors(c, dtype, 1)
+    if cancel:  # y = A x0 on every third row: the residual of those rows cancels
+        n = c["n"]
+        Ax = np.zeros(n, dtype)
+        rows = np.repeat(np.arange(n), np.diff(c["rp"]))
+        np.add.at(Ax, rows, (v.astype(np.float64) * x0[c["ci"]]).astype(dtype))
+        y[::3] = Ax[::3]
+    return c, v, y, x0
+
+
+def _dinv(c, v):
+    n = c["n"]
+    rows = np.repeat(np.arange(n), np.diff(c["rp"]))
+    d = rows == c["ci"]
+    return (1.0 / np.bincount(rows[d], weights=v[d].astype(np.float64), minlength=n)).astype(v.dtype)
+
+
+@pytest.mark.parametrize("dtype", [np.float64, np.float32])
+@pytest.mark.parametrize("cancel", [False, True])
+def test_gs_sweep_bound_holds_for_the_oracle(oracle, dtype, cancel):
+    c, v, y, x0 = _gs_case(dtype, cancel)
+    colors, cptr, crows = _greedy_coloring(c)
+    for direction in (1, 2):
+        x = x0.copy()
+        oracle.gs_apply(c["rp"], c["ci"], v, cptr, crows, _dinv(c, v), y, x, False, dtype(0.9), 1, direction)
+        ex = R.gs_sweep_exact(c["rp"], c["ci"], v, colors, x0, x, y, 0.9, direction)
+        R.assert_within(x[:c["n"]], ex, R.gs_sweep_bound(c["rp"], c["ci"], v, colors, x0, x, y, 0.9, direction), f"direction {direction}")
+
+
+def test_gs_sweep_bound_rejects_a_dropped_entry_and_a_wrong_colour_order(oracle):
+    c, v, y, x0 = _gs_case(np.float64)
+    colors, cptr, crows = _greedy_coloring(c)
+    n, rp, ci = c["n"], c["rp"], c["ci"]
+    rows = np.repeat(np.arange(n), np.diff(rp))
+    ex_bd = lambda x, d: (R.gs_sweep_exact(rp, ci, v, colors, x0, x, y, 0.9, d), R.gs_sweep_bound(rp, ci, v, colors, x0, x, y, 0.9, d))
+    # a dropped entry: the largest off-diagonal term of a row
+    off = np.flatnonzero(rows != ci)
+    e = off[np.argmax(np.abs(v[off] * x0[ci[off]]))]
+    vd = v.copy()
+    vd[e] = 0
+    x = x0.copy()
+    oracle.gs_apply(rp, ci, vd, cptr, crows, _dinv(c, v), y, x, False, 0.9, 1, 1)
+    with pytest.raises(AssertionError):
+        R.assert_within(x[:n], *ex_bd(x, 1), "dropped entry")
+    # one row swept in the wrong colour order: moved behind every other set of a forward sweep
+    sq = (rows != ci) & (ci < n)
+    r = next(i for i in range(n) if np.any(sq[rp[i]:rp[i + 1]] & (colors[np.minimum(ci[rp[i]:rp[i + 1]], n - 1)] > colors[i])))
+    late = np.concatenate([crows[crows != r], [r]]).astype(np.int32)
+    lptr = np.concatenate([cptr, [n]]).astype(np.int32)
+    lptr[colors[r] + 1:len(cptr)] = cptr[colors[r] + 1:] - 1  # r's own set ends one row earlier, r alone in a last set
+    x = x0.copy()
+    oracle.gs_apply(rp, ci, v, lptr, late, _dinv(c, v), y, x, False, 0.9, 1, 1)
+    with pytest.raises(AssertionError, match=f"row {r},"):
+        R.assert_within(x[:n], *ex_bd(x, 1), "wrong colour order")
+
+
+GS2_OPTS = [dict(compact=False, inner=2, gamma=0.7, outer=1, omega=0.9, given=False, direction=0, init_zero=False, num_iter=2),
+            dict(compact=True, inner=3, gamma=1.0, outer=3, omega=0.9, given=True, direction=2, init_zero=True, num_iter=1),
+            dict(compact=True, inner=0, gamma=0.7, outer=1, omega=1.0, given=False, direction=1, init_zero=False, num_iter=1)]
+
+
+@pytest.mark.parametrize("dtype", [np.float64, np.float32])
+def test_gs2_bound_holds_for_the_oracle(oracle, dtype):
+    import gs_cases as G
+
+    c = G.gs2_case(0.1)
+    v = c["v"].astype(dtype)
+    b, x0 = G.vectors(c, dtype, 2)
+    b[::4] = 0  # rows whose update is pure cancellation of the current x
+    for g in GS2_OPTS:
+        dinv = G.given_dinv(c, dtype) if g["given"] else None
+        x = x0.copy()
+        oracle.gs2_apply(c["rp"], c["ci"], v, c["ncols"], x, b, g["init_zero"], dtype(g["omega"]), g["num_iter"], g["direction"], compact=g["compact"],
+                         inner_sweeps=g["inner"], outer_sweeps=g["outer"], gamma=dtype(g["gamma"]), inverse_diagonal=dinv)
+        ex, bd = R.gs2_ref(c["rp"], c["ci"], v, c["ncols"], x0, b, g["init_zero"], g["omega"], g["num_iter"], g["direction"], g["compact"], g["inner"],
+                           g["outer"], g["gamma"], True, dinv)
+        R.assert_within(x, ex, bd, str(g))
+    for given, compact, direction in ((False, False, 0), (True, True, 1), (True, False, 2)):
+        dinv = G.given_dinv(c, dtype) if given else None
+        x = x0.copy()
+        oracle.gs2_classic_apply(c["rp"], c["ci"], v, c["ncols"], x, b, False, 2, direction, compact=compact, inverse_diagonal=dinv)
+        ex, bd = R.gs2_ref(c["rp"], c["ci"], v, c["ncols"], x0, b, False, 1.0, 2, direction, compact, 0, 1, 1.0, False, dinv)
+        R.assert_within(x, ex, bd, f"classic {given} {compact} {direction}")
+        z = np.zeros(c["ncols"], dtype)
+        oracle.gs2_classic_apply(c["rp"], c["ci"], v, c["ncols"], z, b, True, 1, 1 + (direction == 2), compact=compact, inverse_diagonal=dinv)
+        ex, bd = R.trsv_row_bound(c["rp"], c["ci"], v, b, z[:c["n"]], direction != 2, dinv)
+        R.assert_within(z[:c["n"]], ex, bd, "classic local")
+
+
+def test_gs2_bound_rejects_wrong_programs(oracle):
+    """A dropped entry, (1 - gamma) * Z for (1 - gamma) * R, and x += omega Z where the compact form needs x = omega Z, each
+    computed in the data's own precision, fall outside the bound; the same program without the change stays inside."""
+    import gs_cases as G
+
+    c = G.gs2_case(0.1)
+    v = c["v"]
+    b, x0 = G.vectors(c, np.float64, 2)
+    args = (c["rp"], c["ci"], v, c["ncols"], x0, b)
+    plain = lambda variant, **k: R._gs2_run(*args, **k, dt=np.float64, variant=variant).val
+    opts = dict(init_zero=False, omega=0.9, num_iter=1, direction=1, compact=True, inner=2, outer=1, gamma_=0.7, two_stage=True, dinv=None)
+    ex, bd = R.gs2_ref(*args, False, 0.9, 1, 1, True, 2, 1, 0.7)
+    R.assert_within(plain(None, **opts), ex, bd, "plain run")
+    for variant in ("damp_z", "accumulate"):
+        with pytest.raises(AssertionError):
+            R.assert_within(plain(variant, **opts), ex, bd, variant)
+    rows = np.repeat(np.arange(c["n"]), np.diff(c["rp"]))
+    off = np.flatnonzero(rows != c["ci"])
+    vd = v.copy()
+    vd[off[len(off) // 2]] = 0
+    x = x0.copy()
+    oracle.gs2_apply(c["rp"], c["ci"], vd, c["ncols"], x, b, False, 0.9, 1, 1, compact=True, inner_sweeps=2, gamma=0.7)
+    with pytest.raises(AssertionError):
+        R.assert_within(x, ex, bd, "dropped entry")

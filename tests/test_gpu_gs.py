@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+import exact_ref as R
 from gmres_cases import gmres_matrix
 from test_emulated_gs import check_coloring, symmetrize
 from test_oracle_cg import spd_lap27
@@ -47,6 +48,13 @@ def test_gauss_seidel(cuda, oracle, symmetric, dtype):
         tol = 1e-12 if dtype == np.float64 else 2e-5
         assert np.max(np.abs(x.astype(np.float64) - xo.astype(np.float64))) <= tol * max(1.0, np.max(np.abs(xo)))
         assert np.linalg.norm(x.astype(np.float64) - xs.astype(np.float64)) < init
+        if direction:  # one more sweep from here, each row within its local bound
+            xd2 = xd.clone()
+            fn(kh, n, n, rpd, cid, vd, xd2, yd, False, True, 0.9, 1)
+            torch.cuda.synchronize()
+            x2 = xd2.cpu().numpy()
+            bound = R.gs_sweep_bound(rp, ci, v, colors, x, x2, y, 0.9, direction)
+            R.assert_within(x2, R.gs_sweep_exact(rp, ci, v, colors, x, x2, y, 0.9, direction), bound, kh.get_gs_handle().last_kernel())
     kh.destroy_gs_handle()
 
 
@@ -102,3 +110,10 @@ def test_gauss_seidel_ghost_columns(cuda, oracle):
         x = xd.cpu().numpy()
         xo = oracle.gs_apply(rp, ci, v, cptr, crows, dinv, b, x0.copy(), False, 0.9, 2, direction)
         assert np.array_equal(x[n:], x0[n:]) and np.max(np.abs(x - xo)) <= 1e-12
+        if direction:
+            xd2 = t(x)
+            fn(kh, n, ncols, rpd, cid, vd, xd2, t(b), False, True, 0.9, 1)
+            torch.cuda.synchronize()
+            x2 = xd2.cpu().numpy()
+            R.assert_within(x2[:n], R.gs_sweep_exact(rp, ci, v, colors, x, x2, b, 0.9, direction),
+                            R.gs_sweep_bound(rp, ci, v, colors, x, x2, b, 0.9, direction), kh.get_gs_handle().last_kernel())

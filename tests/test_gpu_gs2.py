@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 import torch
 
+import exact_ref as R
 from test_oracle_gs2 import dd_matrix
 
 pytestmark = pytest.mark.gpu
@@ -49,6 +50,8 @@ def test_oracle_parity(cuda, oracle, dtype, compact):
                                  outer_sweeps=outer, gamma=dtype(gamma))
                 err = np.max(np.abs(x.astype(np.float64) - xo.astype(np.float64)))
                 assert err <= tol * 20 * max(1.0, np.max(np.abs(xo))), (inner, gamma, outer, direction, omega, init_zero, err)
+                ex, bnd = R.gs2_ref(rp, ci, v, ncols, x0, b, init_zero, omega, num_iter, direction, compact, inner, outer, gamma)
+                R.assert_within(x, ex, bnd, str((inner, gamma, outer, direction, omega, init_zero)))
         kh.destroy_gs_handle()
 
 
@@ -82,6 +85,8 @@ def test_reference_unit_test_and_multivectors(cuda, oracle):
             xo = np.zeros(n)
             oracle.gs2_apply(rp, ci, v, n, xo, np.ascontiguousarray(Y[:, j]), True, 0.9, 2, direction)
             assert np.allclose(X[:, j], xo, rtol=0, atol=1e-13)
+            ex, bnd = R.gs2_ref(rp, ci, v, n, np.zeros(n), np.ascontiguousarray(Y[:, j]), True, 0.9, 2, direction)
+            R.assert_within(X[:, j], ex, bnd, f"direction {direction} column {j}")
     kh.set_gs_twostage(False, n)  # the classic (sptrsv) form: tests/test_gpu_sptrsv.py; switching resets the phases
     assert not kh.get_twostage_gs_handle().isTwoStage() and not kh.get_twostage_gs_handle().is_symbolic_called()
     kh2 = sp.KokkosKernelsHandle()

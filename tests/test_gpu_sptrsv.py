@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 import torch
 
+import exact_ref as R
 from test_oracle_gs2 import dd_matrix
 from test_oracle_sptrsv import REFERENCE_FIXTURES, fixture_crs, triangle
 
@@ -193,6 +194,8 @@ def test_classic_two_stage_gauss_seidel(cuda, oracle, dtype, compact):
                                          inverse_diagonal=given)
                 err = np.max(np.abs(x.astype(np.float64) - xo.astype(np.float64)))
                 assert err <= tol * 20 * max(1.0, np.max(np.abs(xo))), (given is not None, direction, init_zero, num_iter, err)
+                ex, bnd = R.gs2_ref(rp, ci, v, ncols, x0, b, init_zero, 1.0, num_iter, direction, compact, 0, 2, 1.0, False, given)
+                R.assert_within(x, ex, bnd, str((given is not None, direction, init_zero, num_iter)))
         # omega != 1 is refused, as the reference's apply throws (twostage_gauss_seidel_impl.hpp:886-893)
         with pytest.raises(sp.B200SparseError):
             sp.forward_sweep_gauss_seidel_apply(kh, n, ncols, rpd, cid, vd, t(x0), bd, False, True, 0.9, 1)
