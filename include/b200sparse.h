@@ -221,7 +221,8 @@ int b200sp_spmm_f32_i32(b200sp_spmv_plan* plan, void* stream, char mode, int m, 
  * copies; without a plan, or LayoutLeft with k < 4, one thread per (row, column) computes the entry.  On those item paths
  * the result has the same bits as b200sp_spmm_f32_i32 on the widened inputs, rounded to binary16.  T / H add the exact
  * products into a zeroed fp32 scratch (the plan's, or a stream-ordered temporary without a plan) with atomics and round
- * each entry once.  B200SP_SPMM_KERNEL (row / split / tile) does not apply to this entry point. */
+ * each entry once.  b200sp_spmm_f32_i32 and b200sp_spmm_f64_i32 dispatch the same way, except that without a plan their
+ * row-major X and Y take a kernel of row groups. */
 int b200sp_spmm_f16_i32(b200sp_spmv_plan* plan, void* stream, char mode, int m, int n, int64_t nnz, int k, float alpha,
                         const int* row_ptr, const int* col_idx, const uint16_t* vals, const uint16_t* X, int64_t ldx,
                         int x_row_major, float beta, uint16_t* Y, int64_t ldy, int y_row_major);

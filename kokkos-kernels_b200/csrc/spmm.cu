@@ -6,17 +6,21 @@
 //   TPL     cusparseSpMM                 sparse/tpls/KokkosSparse_spmv_mv_tpl_spec_decl.hpp:97-196
 //
 // Kernels:
-//   spmm_rowmajor_kernel  X, Y LayoutRight: a group of KT lanes owns one row of
-//                         A and one strip of <= KT columns; (col,val) pairs are
-//                         loaded coalesced KT at a time and broadcast by shuffle,
-//                         X rows are read as contiguous KT*sizeof(S) segments.
-//                         One pass over A per 32-column strip, no reduction.
+//   spmm_item_coop_kernel X, Y LayoutRight with a plan: length-sorted runs of
+//                         <= LMAX entries of one row (DESIGN.md 4.2), pieces
+//                         of longer rows added up by spmm_item_reduce_kernel.
+//   spmm_rowmajor_kernel  X, Y LayoutRight without a plan: a group of KT lanes
+//                         owns one row of A and one strip of <= KT columns;
+//                         (col,val) pairs are loaded coalesced KT at a time and
+//                         broadcast by shuffle, X rows are read as contiguous
+//                         KT*sizeof(S) segments.  One pass over A per 32-column
+//                         strip, no reduction.
 //   spmm_general_kernel   any LayoutLeft / LayoutRight mix: thread per (row, j).
 //   spmm_transpose_kernel T/H modes: Y pre-scaled, atomicAdd scatter.
 // Column-major (LayoutLeft) X with k >= 4 goes through a transposed copy so the
 // gather touches one segment per nonzero instead of k sectors (DESIGN.md 3.4).
-// binary16 (b200sp_spmm_f16_i32, spmm_impl_f16): the item, general and relayout kernels with fp32 accumulators, and an fp32
-// scratch for T/H (DESIGN.md 4.3).
+// binary16 (b200sp_spmm_f16_i32): the item, general and relayout kernels with fp32 accumulators, and an fp32 scratch for
+// T/H (DESIGN.md 4.3).
 #include <limits.h>
 #include "spmv_plan.h"
 #include <algorithm>
@@ -203,121 +207,8 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// ---------------------------------------------------------------------------
-// nnz-split kernel (power-law rows): a group of KT lanes (one per column of the strip) walks a chunk
-// of Q consecutive nonzeros; rows that lie inside the chunk are stored directly, the (at most two)
-// rows cut by the chunk borders are pre-scaled by spmm_prescale_split_rows and accumulated with
-// atomicAdd.  chunk_row[c] = row holding nonzero c*Q (built once per matrix, cached in the plan).
-// ---------------------------------------------------------------------------
-__global__ void build_chunk_rows_kernel(int m, const int* __restrict__ row_ptr, int n_chunks, int Q,
-                                        int* __restrict__ chunk_row) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= n_chunks) return;
-  // first row r with row_ptr[r+1] > c*Q
-  const int64_t pos = (int64_t)c * Q;
-  int lo = 0, hi = m;
-  while (lo < hi) {
-    const int mid = lo + ((hi - lo) >> 1);
-    if ((int64_t)row_ptr[mid + 1] <= pos) lo = mid + 1;
-    else hi = mid;
-  }
-  chunk_row[c] = lo;
-}
-
-template <typename S>
-__global__ void spmm_prescale_split_rows(int m, int k, int Q, const int* __restrict__ row_ptr, S beta,
-                                         S* __restrict__ Y, int64_t ldy) {
-  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < m; r += gridDim.x * blockDim.x) {
-    const int s = row_ptr[r], e = row_ptr[r + 1];
-    if (e > s && (s / Q) != ((e - 1) / Q)) {
-      S* yp = Y + (int64_t)r * ldy;
-      for (int j = 0; j < k; ++j) yp[j] = (beta == S(0)) ? S(0) : beta * yp[j];
-    }
-  }
-}
-
-template <typename S, int KT>
-__global__ void __launch_bounds__(256)
-    spmm_split_kernel(int m, int k, int64_t nnz, int Q, int n_chunks, const int* __restrict__ chunk_row,
-                      const int* __restrict__ row_ptr, const int* __restrict__ col_idx, const S* __restrict__ vals,
-                      const S* __restrict__ X, int64_t ldx, S* __restrict__ Y, int64_t ldy, S alpha, S beta) {
-  constexpr int GPW = 32 / KT;
-  const int lane = threadIdx.x & 31;
-  const int grp = lane / KT, t = lane % KT;
-  const unsigned gmask = (KT == 32) ? 0xffffffffu : (((1u << KT) - 1u) << (grp * KT));
-  const int gbase = grp * KT;  // shuffle source lanes are absolute
-  const int nstrips = (k + KT - 1) / KT;
-  const int64_t gid = ((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5) * GPW + grp;
-  const int64_t ngroups = (((int64_t)gridDim.x * blockDim.x) >> 5) * GPW;
-  const int64_t work_total = (int64_t)n_chunks * nstrips;
-  for (int64_t w = gid; w < work_total; w += ngroups) {
-    const int chunk = (int)(w / nstrips);
-    const int j = (int)(w % nstrips) * KT + t;
-    const bool jok = j < k;
-    // chunk 0 starts at the first entry of row 0: the windows of the 64-bit-offset path (spmv64.cu) pass relative row maps
-    // that start at 1..3, and the entries before row_ptr[0] belong to the previous window's last row
-    const int64_t cq = (int64_t)chunk * Q;
-    const int64_t c0 = (chunk == 0) ? (int64_t)row_ptr[0] : cq;
-    const int64_t c1 = (cq + Q < nnz) ? cq + Q : nnz;
-    int row = (chunk == 0) ? 0 : chunk_row[chunk];
-    // cache of KT row ends: lane t holds row_ptr[ebase + 1 + t]
-    int ebase = row;
-    int ends = row_ptr[min(ebase + 1 + t, m)];
-    int64_t row_start = row_ptr[row];
-    int64_t next_end = __shfl_sync(gmask, ends, gbase);
-    S acc = S(0);
-    auto flush = [&]() {
-      // row `row` ends at next_end; acc holds this chunk's share of it
-      if (jok) {
-        S* yp = Y + (int64_t)row * ldy + j;
-        const S a = alpha * acc;
-        if (row_start >= c0 && next_end <= c1) *yp = (beta == S(0)) ? a : beta * *yp + a;
-        else atomicAdd(yp, a);
-      }
-      acc = S(0);
-      row_start = next_end;
-      ++row;
-      if (row - ebase == KT) {
-        ebase = row;
-        ends = row_ptr[min(ebase + 1 + t, m)];
-      }
-      next_end = __shfl_sync(gmask, ends, gbase + (row - ebase));
-    };
-    for (int64_t b = c0; b < c1; b += KT) {
-      const int64_t e = b + t;
-      int c = 0;
-      S v = S(0);
-      if (e < c1) {
-        c = ld_stream(col_idx + e);
-        v = ld_stream(vals + e);
-      }
-      const int nb = (int)((c1 - b < KT) ? (c1 - b) : KT);
-      S xv[KT];
-#pragma unroll
-      for (int u = 0; u < KT; ++u) {
-        const int cu = __shfl_sync(gmask, c, gbase + u);
-        xv[u] = (u < nb && jok) ? ldg(X + (int64_t)cu * ldx + j) : S(0);
-      }
-#pragma unroll
-      for (int u = 0; u < KT; ++u) {
-        const S vu = __shfl_sync(gmask, v, gbase + u);
-        if (u < nb) {
-          while (b + u >= next_end) flush();  // uniform within the group
-          acc += vu * xv[u];
-        }
-      }
-    }
-    // rows ending inside (or exactly at the end of) this chunk, incl. empty rows
-    while (row < m && next_end <= c1) flush();
-    // a row that continues into the next chunk: its share goes in atomically
-    if (row < m && row_start < c1 && jok) atomicAdd(Y + (int64_t)row * ldy + j, alpha * acc);
-  }
-}
-
-
-// Vectorised variant: every lane owns VW adjacent columns (one 16-byte load of the X row per nonzero),
-// a group of KT lanes covers KT*VW columns, so a warp advances 32/KT chunks at once.  Needs k, ldx,
-// ldy multiples of VW and 16-byte aligned X / Y.
+// 16-byte loads and stores of VW adjacent columns of a row-major X or Y row.  Needs k, ldx, ldy multiples of VW and 16-byte
+// aligned X / Y (items_vec).
 template <typename S> struct VecOf;
 template <> struct VecOf<float> { using type = float4; static constexpr int W = 4; };
 template <> struct VecOf<double> { using type = double2; static constexpr int W = 2; };
@@ -342,15 +233,7 @@ __device__ __forceinline__ uint4 vec_pack(const __half* a) {
   return make_uint4(w[0], w[1], w[2], w[3]);
 }
 
-// ---------------------------------------------------------------------------
-// Tile kernel (B200SP_SPMM_KERNEL=tile|tilev; row-major X and Y): the matrix is streamed ONCE, whatever k,
-// through the same TMA-fed shared-memory ring as the rank-1 kernel (tile_ring.cuh); a group of KTL lanes
-// owns one row at a time (rows dealt round-robin to the groups like spmv_tile_kernel does), every lane
-// accumulates VW adjacent columns in registers: per nonzero a broadcast read of (col, val) from shared
-// memory, one gather of the X row segment (VW = 1: 4/8-byte, VW = 4/2: 16-byte loads) and VW FMAs -- no
-// shuffles, no atomics, no row bookkeeping in the inner loop, deterministic.  Rows longer than the tile
-// row limit are cut into segments (plan_analyse_mm) and done by spmm_seg_kernel.
-// ---------------------------------------------------------------------------
+// the VW adjacent columns a lane accumulates in registers
 template <typename S, int VW>
 struct Acc {
   S a[VW];
@@ -358,7 +241,7 @@ struct Acc {
 
 // beta*y + alpha*acc as alpha*acc rounded, then one fused multiply-add.  Written out so that every instantiation rounds the
 // same way: left to the compiler, the contraction of this expression differed between the 16-byte-load (VW > 1) and the
-// scalar variants of the item and tile kernels, and misaligned operands then gave other bits than aligned ones.
+// scalar variants of the item kernel, and misaligned operands then gave other bits than aligned ones.
 __device__ __forceinline__ float axpby_rn(float alpha, float acc, float beta, float y) { return fmaf(beta, y, __fmul_rn(alpha, acc)); }
 __device__ __forceinline__ double axpby_rn(double alpha, double acc, double beta, double y) { return fma(beta, y, __dmul_rn(alpha, acc)); }
 
@@ -421,240 +304,6 @@ __device__ __forceinline__ void item_epilogue(AccT<S>* o, const Acc<AccT<S>, VW>
   }
 }
 
-template <typename S, int VW, int KTL, int NW, int STAGES, int CAP, int UNR>
-__global__ void __launch_bounds__((NW + 1) * 32)
-    spmm_tile_kernel(int m, int k, int64_t nnz, int n_tiles, int LMAX, const int4* __restrict__ tiles,
-                     const int* __restrict__ row_ptr, const int* __restrict__ col_idx, const S* __restrict__ vals,
-                     const S* __restrict__ X, int64_t ldx, S* __restrict__ Y, int64_t ldy, S alpha, S beta) {
-  using Ring = CsrTileRing<S, CAP, STAGES>;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  Ring& sm = *reinterpret_cast<Ring*>(smem_raw);
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  tile_ring_init(sm, NW);
-  if (warp == NW) {
-    tile_ring_produce(sm, lane, m, nnz, 1, n_tiles, tiles, row_ptr, col_idx, vals);
-    return;
-  }
-  constexpr int RPW = 32 / KTL;  // rows per warp
-  const int sub = lane / KTL, t = lane % KTL;
-  const int nstrips = (k + KTL * VW - 1) / (KTL * VW);
-  for (int it = 0; tile_ring_more(it, n_tiles); ++it) {
-    const TileView tv = tile_ring_acquire<4, 4>(sm, it);
-    const int stage = tv.stage, r0 = tv.r0, r1 = tv.r1, s_al = tv.s_al;
-    const S* sv = sm.vals[stage];
-    const int* sc = sm.cols[stage];
-    const int g_first = r0 / RPW;
-    int g = g_first + ((warp - g_first % NW) + NW) % NW;
-    for (; g * RPW < r1; g += NW) {
-      const int r = g * RPW + sub;
-      const bool valid = (r >= r0) && (r < r1);
-      int rs = 0, re = 0;
-      if (valid) tile_row_bounds(sm, stage, row_ptr, r, r - tv.r0_al, rs, re);
-      const bool is_long = (re - rs) > LMAX;
-      if (is_long) re = rs;
-      const int jbeg = rs - s_al, jend = re - s_al;
-      for (int strip = 0; strip < nstrips; ++strip) {
-        const int j = (strip * KTL + t) * VW;
-        const bool jok = j < k;  // k % VW == 0: a lane's VW columns are all in or all out
-        Acc<S, VW> acc;
-#pragma unroll
-        for (int q = 0; q < VW; ++q) acc.a[q] = S(0);
-        for (int e0 = jbeg; e0 < jend; e0 += UNR) {
-          int c[UNR];
-          S av[UNR];
-          Acc<S, VW> xv[UNR];
-#pragma unroll
-          for (int u = 0; u < UNR; ++u) {
-            const bool ok = e0 + u < jend;
-            c[u] = ok ? sc[e0 + u] : 0;
-            av[u] = ok ? sv[e0 + u] : S(0);
-          }
-#pragma unroll
-          for (int u = 0; u < UNR; ++u) {
-            if (jok && e0 + u < jend) {
-              xv[u] = load_x<S, VW>(X + (int64_t)c[u] * ldx + j);
-            } else {
-#pragma unroll
-              for (int q = 0; q < VW; ++q) xv[u].a[q] = S(0);
-            }
-          }
-#pragma unroll
-          for (int u = 0; u < UNR; ++u)
-#pragma unroll
-            for (int q = 0; q < VW; ++q) acc.a[q] += av[u] * xv[u].a[q];
-        }
-        if (valid && !is_long && jok) {
-          S* yp = Y + (int64_t)r * ldy + j;
-          S o[VW];
-          if (beta == S(0)) {
-#pragma unroll
-            for (int q = 0; q < VW; ++q) o[q] = alpha * acc.a[q];
-          } else {
-            const Acc<S, VW> old = load_x<S, VW>(yp);
-#pragma unroll
-            for (int q = 0; q < VW; ++q) o[q] = axpby_rn(alpha, acc.a[q], beta, old.a[q]);
-          }
-          if constexpr (VW == 1) {
-            yp[0] = o[0];
-          } else {
-            using V = typename VecOf<S>::type;
-            *reinterpret_cast<V*>(yp) = vec_pack(o);
-          }
-        }
-      }
-    }
-    tile_ring_release(sm, stage, lane);
-  }
-}
-
-// rows of several segments: y_row = beta*y_row before the pieces are added atomically
-template <typename S>
-__global__ void __launch_bounds__(256)
-    spmm_seg_prescale_kernel(const int4* __restrict__ segs, const int* __restrict__ n_seg_ptr, int k, S beta,
-                             S* __restrict__ Y, int64_t ldy) {
-  const int n_seg = *n_seg_ptr;
-  const int64_t total = (int64_t)n_seg * k;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int4 d = segs[i / k];
-    if ((d.w & 3) == 3) {
-      S* yp = Y + (int64_t)d.x * ldy + (i % k);
-      *yp = (beta == S(0)) ? S(0) : beta * *yp;
-    }
-  }
-}
-
-// one CTA (256 threads = 256/KT groups of KT lanes) per segment of a long row
-template <typename S, int KT>
-__global__ void __launch_bounds__(256)
-    spmm_seg_kernel(const int4* __restrict__ segs, const int* __restrict__ n_seg_ptr, int k,
-                    const int* __restrict__ col_idx, const S* __restrict__ vals, const S* __restrict__ X, int64_t ldx,
-                    S* __restrict__ Y, int64_t ldy, S alpha, S beta) {
-  constexpr int G = 256 / KT;
-  constexpr int UNR = 4;
-  __shared__ S red[G][KT];
-  const int grp = threadIdx.x / KT, t = threadIdx.x % KT;
-  const int n_seg = *n_seg_ptr;
-  const int nstrips = (k + KT - 1) / KT;
-  for (int q = blockIdx.x; q < n_seg; q += gridDim.x) {
-    const int4 d = segs[q];
-    const int row = d.x, e0 = d.y, e1 = d.z;
-    const bool multi = (d.w & 1) != 0;
-    for (int strip = 0; strip < nstrips; ++strip) {
-      const int j = strip * KT + t;
-      const bool jok = j < k;
-      S acc = S(0);
-      for (int e = e0 + grp; e < e1; e += G * UNR) {
-        int c[UNR];
-        S av[UNR], xv[UNR];
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-          const int ee = e + u * G;
-          const bool ok = ee < e1;
-          c[u] = ok ? ld_stream(col_idx + ee) : 0;
-          av[u] = ok ? ld_stream(vals + ee) : S(0);
-        }
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) xv[u] = (jok && e + u * G < e1) ? ldg(X + (int64_t)c[u] * ldx + j) : S(0);
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) acc += av[u] * xv[u];
-      }
-      red[grp][t] = acc;
-      __syncthreads();
-      if (grp == 0 && jok) {
-        S sum = S(0);
-#pragma unroll 4
-        for (int gg = 0; gg < G; ++gg) sum += red[gg][t];
-        S* yp = Y + (int64_t)row * ldy + j;
-        const S a = alpha * sum;
-        if (multi) atomicAdd(yp, a);
-        else *yp = (beta == S(0)) ? a : beta * *yp + a;
-      }
-      __syncthreads();
-    }
-  }
-}
-
-// 16-byte-load flavour of spmm_seg_kernel (opt-in, B200SP_SPMM_SEG=vec): groups of KTL lanes with VW adjacent columns
-// each (the tile kernel's vec layout), so that a 256-thread CTA keeps 256/KTL nonzeros' X rows in flight per step
-// instead of 256/KT; partial sums are reduced by shuffles inside a warp and through shared memory across the 8 warps.
-template <typename S, int KTL>
-__global__ void __launch_bounds__(256)
-    spmm_seg_vec_kernel(const int4* __restrict__ segs, const int* __restrict__ n_seg_ptr, int k,
-                        const int* __restrict__ col_idx, const S* __restrict__ vals, const S* __restrict__ X, int64_t ldx,
-                        S* __restrict__ Y, int64_t ldy, S alpha, S beta) {
-  constexpr int VW = VecOf<S>::W;
-  constexpr int G = 256 / KTL;       // groups per CTA
-  constexpr int GPW = 32 / KTL;      // groups per warp
-  constexpr int UNR = 4;
-  __shared__ S red[8][KTL * VW];
-  const int grp = threadIdx.x / KTL, t = threadIdx.x % KTL;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_seg = *n_seg_ptr;
-  const int nstrips = (k + KTL * VW - 1) / (KTL * VW);
-  for (int q = blockIdx.x; q < n_seg; q += gridDim.x) {
-    const int4 d = segs[q];
-    const int row = d.x, e0 = d.y, e1 = d.z;
-    const bool multi = (d.w & 1) != 0;
-    for (int strip = 0; strip < nstrips; ++strip) {
-      const int j = (strip * KTL + t) * VW;
-      const bool jok = j < k;
-      Acc<S, VW> acc;
-#pragma unroll
-      for (int c = 0; c < VW; ++c) acc.a[c] = S(0);
-      for (int e = e0 + grp; e < e1; e += G * UNR) {
-        int c[UNR];
-        S av[UNR];
-        Acc<S, VW> xv[UNR];
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-          const int ee = e + u * G;
-          const bool ok = ee < e1;
-          c[u] = ok ? ld_stream(col_idx + ee) : 0;
-          av[u] = ok ? ld_stream(vals + ee) : S(0);
-        }
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-          if (jok && e + u * G < e1) {
-            xv[u] = load_x<S, VW>(X + (int64_t)c[u] * ldx + j);
-          } else {
-#pragma unroll
-            for (int cc = 0; cc < VW; ++cc) xv[u].a[cc] = S(0);
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < UNR; ++u)
-#pragma unroll
-          for (int cc = 0; cc < VW; ++cc) acc.a[cc] += av[u] * xv[u].a[cc];
-      }
-      // groups of one warp: lanes with the same t are KTL apart
-#pragma unroll
-      for (int o = KTL; o < 32; o <<= 1)
-#pragma unroll
-        for (int cc = 0; cc < VW; ++cc) acc.a[cc] += __shfl_xor_sync(0xffffffffu, acc.a[cc], o);
-      if (lane < KTL) {
-#pragma unroll
-        for (int cc = 0; cc < VW; ++cc) red[warp][lane * VW + cc] = acc.a[cc];
-      }
-      __syncthreads();
-      if (threadIdx.x < KTL && jok) {
-        S* yp = Y + (int64_t)row * ldy + j;
-#pragma unroll
-        for (int cc = 0; cc < VW; ++cc) {
-          S sum = S(0);
-#pragma unroll
-          for (int w = 0; w < 8; ++w) sum += red[w][threadIdx.x * VW + cc];
-          const S a = alpha * sum;
-          if (multi) atomicAdd(yp + cc, a);
-          else yp[cc] = (beta == S(0)) ? a : beta * yp[cc] + a;
-        }
-      }
-      __syncthreads();
-    }
-  }
-  (void)GPW;
-}
-
 template <typename S>
 static int launch_rowmajor(cudaStream_t st, int m, int k, const int* row_ptr, const int* col_idx, const S* vals,
                            const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
@@ -682,370 +331,14 @@ static int launch_rowmajor(cudaStream_t st, int m, int k, const int* row_ptr, co
   return B200SP_OK;
 }
 
-template <typename S, int KT>
-__global__ void __launch_bounds__(256)
-    spmm_split_vec_kernel(int m, int k, int64_t nnz, int Q, int n_chunks, const int* __restrict__ chunk_row,
-                          const int* __restrict__ row_ptr, const int* __restrict__ col_idx, const S* __restrict__ vals,
-                          const S* __restrict__ X, int64_t ldx, S* __restrict__ Y, int64_t ldy, S alpha, S beta) {
-  using V = typename VecOf<S>::type;
-  constexpr int VW = VecOf<S>::W;
-  constexpr int GPW = 32 / KT;
-  constexpr int EB = (KT >= 8) ? 1 : (8 / KT);  // entries per lane per batch
-  constexpr int BATCH = KT * EB;
-  const int lane = threadIdx.x & 31;
-  const int grp = lane / KT, t = lane % KT;
-  const unsigned gmask = (KT == 32) ? 0xffffffffu : (((1u << KT) - 1u) << (grp * KT));
-  const int gbase = grp * KT;
-  const int strip_cols = KT * VW;
-  const int nstrips = (k + strip_cols - 1) / strip_cols;
-  const int64_t gid = ((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5) * GPW + grp;
-  const int64_t ngroups = (((int64_t)gridDim.x * blockDim.x) >> 5) * GPW;
-  const int64_t work_total = (int64_t)n_chunks * nstrips;
-  for (int64_t w = gid; w < work_total; w += ngroups) {
-    const int chunk = (int)(w / nstrips);
-    const int j = (int)(w % nstrips) * strip_cols + t * VW;
-    const bool jok = j < k;  // k % VW == 0: a lane's VW columns are all in or all out
-    const int64_t c0 = (int64_t)chunk * Q;
-    const int64_t c1 = (c0 + Q < nnz) ? c0 + Q : nnz;
-    int row = (chunk == 0) ? 0 : chunk_row[chunk];
-    int ebase = row;
-    int ends = row_ptr[min(ebase + 1 + t, m)];
-    int64_t row_start = row_ptr[row];
-    int64_t next_end = __shfl_sync(gmask, ends, gbase);
-    S acc[VW];
-#pragma unroll
-    for (int q = 0; q < VW; ++q) acc[q] = S(0);
-    auto flush = [&]() {
-      if (jok) {
-        S* yp = Y + (int64_t)row * ldy + j;
-        if (row_start >= c0 && next_end <= c1) {
-          S o[VW];
-          if (beta == S(0)) {
-#pragma unroll
-            for (int q = 0; q < VW; ++q) o[q] = alpha * acc[q];
-          } else {
-            S old[VW];
-            vec_unpack(*reinterpret_cast<const V*>(yp), old);
-#pragma unroll
-            for (int q = 0; q < VW; ++q) o[q] = beta * old[q] + alpha * acc[q];
-          }
-          *reinterpret_cast<V*>(yp) = vec_pack(o);
-        } else {
-#pragma unroll
-          for (int q = 0; q < VW; ++q) atomicAdd(yp + q, alpha * acc[q]);
-        }
-      }
-#pragma unroll
-      for (int q = 0; q < VW; ++q) acc[q] = S(0);
-      row_start = next_end;
-      ++row;
-      if (row - ebase == KT) {
-        ebase = row;
-        ends = row_ptr[min(ebase + 1 + t, m)];
-      }
-      next_end = __shfl_sync(gmask, ends, gbase + (row - ebase));
-    };
-    for (int64_t b = c0; b < c1; b += BATCH) {
-      int c[EB];
-      S v[EB];
-#pragma unroll
-      for (int i = 0; i < EB; ++i) {
-        const int64_t e = b + i * KT + t;
-        c[i] = 0;
-        v[i] = S(0);
-        if (e < c1) {
-          c[i] = ld_stream(col_idx + e);
-          v[i] = ld_stream(vals + e);
-        }
-      }
-      const int nb = (int)((c1 - b < BATCH) ? (c1 - b) : BATCH);
-      V xv[BATCH];
-#pragma unroll
-      for (int u = 0; u < BATCH; ++u) {
-        const int cu = __shfl_sync(gmask, c[u / KT], gbase + (u % KT));
-        if (u < nb && jok) xv[u] = __ldg(reinterpret_cast<const V*>(X + (int64_t)cu * ldx + j));
-      }
-#pragma unroll
-      for (int u = 0; u < BATCH; ++u) {
-        const S vu = __shfl_sync(gmask, v[u / KT], gbase + (u % KT));
-        if (u < nb) {
-          while (b + u >= next_end) flush();  // uniform within the group
-          if (jok) {
-            S xs[VW];
-            vec_unpack(xv[u], xs);
-#pragma unroll
-            for (int q = 0; q < VW; ++q) acc[q] += vu * xs[q];
-          }
-        }
-      }
-    }
-    while (row < m && next_end <= c1) flush();
-    if (row < m && row_start < c1 && jok) {
-      S* yp = Y + (int64_t)row * ldy + j;
-#pragma unroll
-      for (int q = 0; q < VW; ++q) atomicAdd(yp + q, alpha * acc[q]);
-    }
-  }
-}
-
-// the chunk table of the plan (once per matrix and Q)
-static int chunk_table(SpmmState& mm, cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int Q) {
-  const PlanKey key{row_ptr, nullptr, m, -1, nnz, Q};
-  if (mm.chunk_key == key) return B200SP_OK;
-  mm.chunk_key = PlanKey();
-  mm.n_chunks = std::max<int>(1, (int)((nnz + Q - 1) / Q));
-  B200SP_CUDA_TRY(mm.chunk_row.alloc((size_t)mm.n_chunks, st));
-  build_chunk_rows_kernel<<<(mm.n_chunks + 255) / 256, 256, 0, st>>>(m, row_ptr, mm.n_chunks, Q, mm.chunk_row);
-  B200SP_LAUNCH_CHECK();
-  mm.chunk_key = key;
-  return B200SP_OK;
-}
-
-template <typename S>
-static int launch_split(b200sp_spmv_plan* p, cudaStream_t st, int m, int k, int64_t nnz, const int* row_ptr,
-                        const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta,
-                        const char** name) {
-  const int Q = 256;
-  int rc = chunk_table(p->mm, st, m, nnz, row_ptr, Q);
-  if (rc) return rc;
-  const int* chunk_row = p->mm.chunk_row;
-  const int n_chunks = p->mm.n_chunks;
-  {
-    const int blocks = std::max(1, std::min((m + 255) / 256, sm_count() * 8));
-    spmm_prescale_split_rows<S><<<blocks, 256, 0, st>>>(m, k, Q, row_ptr, beta, Y, ldy);
-    B200SP_LAUNCH_CHECK();
-  }
-  {
-    constexpr int VW = 16 / (int)sizeof(S);
-    const bool vec_ok = (k % VW == 0) && (ldx % VW == 0) && (ldy % VW == 0) &&
-                        ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0 && getenv("B200SP_SPMM_VEC") != nullptr;
-    // opt-in: slower than the scalar-lane kernel on config 3 when it was tuned -- fewer lanes per chunk means fewer
-    // chunks in flight per SM at its register count; kept for the tuning round
-    *name = vec_ok ? "split_vec" : "split";
-    if (vec_ok) {
-      int KTv = 1;
-      while (KTv * VW < k && KTv < 32) KTv <<= 1;
-      const int gpwv = 32 / KTv;
-      const int nstripsv = (k + KTv * VW - 1) / (KTv * VW);
-      const int64_t workv = (int64_t)n_chunks * nstripsv;
-      int blocksv = (int)std::min<int64_t>((workv + 8 * gpwv - 1) / (8 * gpwv), (int64_t)sm_count() * 16);
-      if (blocksv < 1) blocksv = 1;
-#define B200SP_SPLITV(K)                                                                                          \
-  case K:                                                                                                         \
-    spmm_split_vec_kernel<S, K><<<blocksv, 256, 0, st>>>(m, k, nnz, Q, n_chunks, chunk_row, row_ptr, col_idx, vals, X, \
-                                                         ldx, Y, ldy, alpha, beta);                               \
-    break;
-      switch (KTv) {
-        B200SP_SPLITV(1)
-        B200SP_SPLITV(2)
-        B200SP_SPLITV(4)
-        B200SP_SPLITV(8)
-        B200SP_SPLITV(16)
-        B200SP_SPLITV(32)
-      }
-#undef B200SP_SPLITV
-      B200SP_LAUNCH_CHECK();
-      return B200SP_OK;
-    }
-  }
-  int KT = 1;
-  while (KT < k && KT < 32) KT <<= 1;
-  const int gpw = 32 / KT;
-  const int nstrips = (k + KT - 1) / KT;
-  const int64_t work = (int64_t)n_chunks * nstrips;
-  int blocks = (int)std::min<int64_t>((work + 8 * gpw - 1) / (8 * gpw), (int64_t)sm_count() * 16);
-  if (blocks < 1) blocks = 1;
-#define B200SP_SPLIT(K)                                                                                       \
-  case K:                                                                                                     \
-    spmm_split_kernel<S, K><<<blocks, 256, 0, st>>>(m, k, nnz, Q, n_chunks, chunk_row, row_ptr, col_idx, vals, X, ldx, \
-                                                    Y, ldy, alpha, beta);                                     \
-    break;
-  switch (KT) {
-    B200SP_SPLIT(1)
-    B200SP_SPLIT(2)
-    B200SP_SPLIT(4)
-    B200SP_SPLIT(8)
-    B200SP_SPLIT(16)
-    B200SP_SPLIT(32)
-  }
-#undef B200SP_SPLIT
-  B200SP_LAUNCH_CHECK();
-  return B200SP_OK;
-}
-
-// Segments of the rows the rank-2 tile kernel leaves out (longer than LMAX): {row, first entry, end entry,
-// flags}; flags bit 0 = the row has several segments (its pieces are combined with atomics), bit 1 = first
-// segment of its row.  One thread per long row.
-__global__ void build_segments_kernel(const int* __restrict__ long_rows, const int* __restrict__ n_long,
-                                      const int* __restrict__ row_ptr, int SEG, int4* __restrict__ segs,
-                                      int* __restrict__ n_seg) {
-  const int nl = *n_long;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nl; i += gridDim.x * blockDim.x) {
-    const int r = long_rows[i];
-    const int s = row_ptr[r], e = row_ptr[r + 1];
-    const int nseg = (e - s + SEG - 1) / SEG;
-    const int base = atomicAdd(n_seg, nseg);
-    for (int q = 0; q < nseg; ++q)
-      segs[base + q] = make_int4(r, s + q * SEG, min(e, s + (q + 1) * SEG), (nseg > 1 ? 1 : 0) | (q == 0 ? 2 : 0));
-  }
-}
-
-void SpmmState::release_tiles(cudaStream_t st) {
-  tiles.release(st);
-  segs.release(st);
-  n_seg.release(st);
-  tiles_key = PlanKey();
-}
-
-void SpmmState::reset(cudaStream_t st) {
-  release_tiles(st);
-  items.release(st);
-  chunk_row.release(st);
-  n_chunks = 0;
-  chunk_key = PlanKey();
-}
-
-void SpmmState::release(cudaStream_t st) {
-  reset(st);
-  xt.release(st);
-  yt.release(st);
-}
-
-// Tile analysis of the rank-2 tile kernel: same descriptors as the rank-1 kernel's, with its own stage capacity and row
-// limit, + the segments of its long rows; cached per matrix in the plan; stream-ordered, no host synchronisation.
-static int plan_analyse_mm(SpmmState& mm, cudaStream_t st, int cap, int lmax, int seg, int m, int64_t nnz, const int* row_ptr) {
-  const PlanKey key{row_ptr, nullptr, m, -1, nnz, cap, lmax};
-  if (mm.tiles_key == key) return B200SP_OK;
-  mm.release_tiles(st);
-  const int rc = tile_analyse(st, m, nnz, row_ptr, cap, lmax, &mm.tiles);
-  if (rc != B200SP_OK) return rc;
-  const int long_cap = mm.tiles.long_cap;
-  B200SP_CUDA_TRY(mm.segs.alloc((size_t)(nnz / seg) + long_cap + 1, st));
-  B200SP_CUDA_TRY(mm.n_seg.alloc(1, st));
-  B200SP_CUDA_TRY(cudaMemsetAsync(mm.n_seg, 0, sizeof(int), st));
-  build_segments_kernel<<<std::max(1, std::min((long_cap + 255) / 256, sm_count() * 4)), 256, 0, st>>>(
-      mm.tiles.long_rows, mm.tiles.n_long, row_ptr, seg, mm.segs, mm.n_seg);
-  B200SP_LAUNCH_CHECK();
-  mm.tiles_key = key;
-  return B200SP_OK;
-}
-
-template <typename S, int VW, int KTL, int NW, int STAGES, int CAP, int UNR>
-static int launch_mm_tile_k(cudaStream_t st, const TileAnalysis& tv, int m, int k, int64_t nnz, const int* row_ptr,
-                            const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
-  using Ring = CsrTileRing<S, CAP, STAGES>;
-  auto kern = spmm_tile_kernel<S, VW, KTL, NW, STAGES, CAP, UNR>;
-  const size_t smem = sizeof(Ring) + 128;
-  static KernelSetup ks;  // per instantiation and device: attribute set + occupancy queried once
-  int occ = 1;
-  if (int rc = kernel_setup(ks, kern, (NW + 1) * 32, smem, &occ)) return rc;
-  int grid = std::min(tv.n_tiles, sm_count() * occ);
-  if (grid < 1) grid = 1;
-  kern<<<grid, (NW + 1) * 32, smem, st>>>(m, k, nnz, tv.n_tiles, tv.LMAX, tv.tiles, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
-  B200SP_LAUNCH_CHECK();
-  return B200SP_OK;
-}
-
-// ring / unroll configurations of the tile kernel.  0 is the default; 1-3 exist for the 16-byte-load path only
-// (B200SP_SPMM_CFG, tuning sweeps): 1 = small ring (8 consumer warps, 1024-entry stages: 5 CTAs per SM for fp32),
-// 2 = default ring with twice the gathers in flight per lane, 3 = small ring with 16 consumer warps.
-template <typename S, int VW, int KTL>
-static int launch_mm_tile_cfg(int cfg, cudaStream_t st, const TileAnalysis& tv, int m, int k, int64_t nnz, const int* row_ptr,
-                              const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta) {
-  if constexpr (VW > 1) {
-    switch (cfg) {
-      case 1: return launch_mm_tile_k<S, VW, KTL, 8, 4, 1024, 4>(st, tv, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
-      case 2: return launch_mm_tile_k<S, VW, KTL, 16, 4, 2048, 8>(st, tv, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
-      case 3: return launch_mm_tile_k<S, VW, KTL, 16, 3, 1024, 4>(st, tv, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
-      default: break;
-    }
-  }
-  return launch_mm_tile_k<S, VW, KTL, 16, 4, 2048, (VW == 1 ? 8 : 4)>(st, tv, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
-}
-
-template <typename S>
-static int launch_mm_tile(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m, int k, int64_t nnz, const int* row_ptr,
-                          const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, S alpha, S beta,
-                          const char** name) {
-  constexpr int SEG = 2048;
-  int cfg = 0;
-  if (const char* e = getenv("B200SP_SPMM_CFG")) cfg = atoi(e);
-  if (!vec || cfg < 0 || cfg > 3) cfg = 0;
-  const int CAP = (cfg == 1 || cfg == 3) ? 1024 : 2048;
-  int LMAX = 256;  // rows longer than this leave the tiles for the segment kernel (B200SP_SPMM_LMAX: 16..512)
-  if (const char* e = getenv("B200SP_SPMM_LMAX")) {
-    const int v = atoi(e);
-    if (v >= 16 && v <= 512) LMAX = v;
-  }
-  int rc = plan_analyse_mm(p->mm, st, CAP, LMAX, SEG, m, nnz, row_ptr);
-  if (rc) return rc;
-  const TileAnalysis& tv = p->mm.tiles;
-  const int4* segs = p->mm.segs;
-  const int* n_seg = p->mm.n_seg;
-  constexpr int W = VecOf<S>::W;
-  const int lanes_needed = vec ? (k + W - 1) / W : k;
-  int KTL = 1;
-  while (KTL < lanes_needed && KTL < 32) KTL <<= 1;
-#define B200SP_MMT(V, L)                                                                                                    \
-  case L:                                                                                                                   \
-    rc = launch_mm_tile_cfg<S, V, L>(cfg, st, tv, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);          \
-    break;
-  if (vec) {
-    switch (KTL) {
-      B200SP_MMT(W, 1) B200SP_MMT(W, 2) B200SP_MMT(W, 4) B200SP_MMT(W, 8) B200SP_MMT(W, 16) B200SP_MMT(W, 32)
-    }
-  } else {
-    switch (KTL) {
-      B200SP_MMT(1, 1) B200SP_MMT(1, 2) B200SP_MMT(1, 4) B200SP_MMT(1, 8) B200SP_MMT(1, 16) B200SP_MMT(1, 32)
-    }
-  }
-#undef B200SP_MMT
-  if (rc) return rc;
-  // long rows: segments of <= SEG entries, one CTA each
-  const int grid = sm_count() * 4;
-  spmm_seg_prescale_kernel<S><<<grid, 256, 0, st>>>(segs, n_seg, k, beta, Y, ldy);
-  B200SP_LAUNCH_CHECK();
-  *name = vec ? "tile_vec" : "tile";
-  if (vec) {
-    const char* e = getenv("B200SP_SPMM_SEG");
-    if (e && e[0] == 'v') {
-      *name = "tile_vec+seg_vec";
-#define B200SP_SEGV(L)                                                                                               \
-  case L:                                                                                                            \
-    spmm_seg_vec_kernel<S, L><<<grid, 256, 0, st>>>(segs, n_seg, k, col_idx, vals, X, ldx, Y, ldy, alpha, beta); \
-    break;
-      switch (KTL) {
-        B200SP_SEGV(1) B200SP_SEGV(2) B200SP_SEGV(4) B200SP_SEGV(8) B200SP_SEGV(16) B200SP_SEGV(32)
-      }
-#undef B200SP_SEGV
-      B200SP_LAUNCH_CHECK();
-      return B200SP_OK;
-    }
-  }
-  int KT = 1;
-  while (KT < k && KT < 32) KT <<= 1;
-#define B200SP_SEG(K)                                                                                              \
-  case K:                                                                                                          \
-    spmm_seg_kernel<S, K><<<grid, 256, 0, st>>>(segs, n_seg, k, col_idx, vals, X, ldx, Y, ldy, alpha, beta); \
-    break;
-  switch (KT) {
-    B200SP_SEG(1) B200SP_SEG(2) B200SP_SEG(4) B200SP_SEG(8) B200SP_SEG(16) B200SP_SEG(32)
-  }
-#undef B200SP_SEG
-  B200SP_LAUNCH_CHECK();
-  return B200SP_OK;
-}
-
 // ---------------------------------------------------------------------------
-// Item kernel (default for row-major X and Y with a plan; B200SP_SPMM_KERNEL=items): the gather-bound formulation.
-// On power-law matrices the tile kernel's row groups of one warp run loops of very different lengths and wait for
-// the longest; here the unit of work is an ITEM -- a run of <= LMAX consecutive entries of one row (MMItems, spmv_plan.h) --
-// and the items are sorted by length, longest first.  A group of KTL lanes (VW adjacent columns each, one 16-byte
-// load of the X row segment per lane and entry) owns one item, so the 32/KTL groups of a warp run loops of equal
-// length with 4 independent gathers in flight per lane, nothing waits, and the long items are scheduled first.
-// (col, val) are read straight from global memory (every lane of the group the same address: one request).
-// Single-item rows write Y; the pieces of longer rows write partial sums that spmm_item_reduce_kernel adds up in
-// piece order (no atomics: deterministic).  Per entry the sum order is the storage order.
+// Item kernel (row-major X and Y with a plan): the gather-bound formulation.  On power-law matrices row groups of one
+// warp that each own a whole row run loops of very different lengths and wait for the longest; here the unit of work is
+// an ITEM -- a run of <= LMAX consecutive entries of one row (MMItems, spmv_plan.h) -- and the items are sorted by length,
+// longest first.  A group of KTL lanes (VW adjacent columns each, one 16-byte load of the X row segment per lane and
+// entry) owns one item, so the 32/KTL groups of a warp run loops of equal length, nothing waits, and the long items are
+// scheduled first.  Single-item rows write Y; the pieces of longer rows write partial sums that spmm_item_reduce_kernel
+// adds up in piece order (no atomics: deterministic).  Per entry the sum order is the storage order.
 // ---------------------------------------------------------------------------
 static constexpr int MMI_MAXL = 256;
 static constexpr int MMI_LONG_PIECES = 64;  // rows of more pieces are added up by a whole CTA (spmm_item_reduce_long_kernel)
@@ -1157,84 +450,14 @@ static int plan_analyse_items(MMItems* mi, cudaStream_t st, int lmax, int m, int
   return B200SP_OK;
 }
 
-template <typename S, int VW, int KTL>
-__global__ void __launch_bounds__(256)
-    spmm_item_kernel(int n_items, const int4* __restrict__ items, int k, const int* __restrict__ col_idx,
-                     const S* __restrict__ vals, const S* __restrict__ X, int64_t ldx, S* __restrict__ Y, int64_t ldy,
-                     AccT<S>* __restrict__ partial, AccT<S> alpha, AccT<S> beta) {
-  using A = AccT<S>;
-  const int64_t gt = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  const int64_t q = gt / KTL;
-  const int t = (int)(gt % KTL);
-  if (q >= n_items) return;
-  // the matrix, the item list and Y pass through once: evict-first in L2, which then belongs to the gathered rows of X
-  const uint64_t once = l2_policy_evict_first();
-  const int4 it = ld_once(items + q, once);
-  const int row = it.x, e0 = it.y, len = it.z, slot = it.w;
-  const int nstrips = (k + KTL * VW - 1) / (KTL * VW);
-  for (int strip = 0; strip < nstrips; ++strip) {
-    const int j = (strip * KTL + t) * VW;
-    if (j >= k) break;  // k % VW == 0: a lane's VW columns are all in or all out
-    Acc<A, VW> acc;
-#pragma unroll
-    for (int c = 0; c < VW; ++c) acc.a[c] = A(0);
-    const S* xb = X + j;
-    int e = e0;
-    const int e4 = e0 + (len & ~3);
-    for (; e < e4; e += 4) {
-      int c[4];
-      A av[4];
-      Acc<A, VW> xv[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        c[u] = ld_once(col_idx + e + u, once);
-        av[u] = wide(ld_once(vals + e + u, once));
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) xv[u] = load_x<S, VW>(xb + (int64_t)c[u] * ldx);
-#pragma unroll
-      for (int u = 0; u < 4; ++u)
-#pragma unroll
-        for (int cc = 0; cc < VW; ++cc) acc.a[cc] += av[u] * xv[u].a[cc];
-    }
-    for (; e < e0 + len; ++e) {
-      const int c = ld_once(col_idx + e, once);
-      const A av = wide(ld_once(vals + e, once));
-      const Acc<A, VW> xv = load_x<S, VW>(xb + (int64_t)c * ldx);
-#pragma unroll
-      for (int cc = 0; cc < VW; ++cc) acc.a[cc] += av * xv.a[cc];
-    }
-    A o[VW];
-    if constexpr (std::is_same<S, A>::value) {  // fp32 / fp64: Y and the partial sums share a type, one store
-      S* dst;
-      if (slot < 0) {
-        dst = Y + (int64_t)row * ldy + j;
-        item_epilogue<S, VW>(o, acc, alpha, beta, dst);
-      } else {
-        dst = partial + (int64_t)slot * k + j;  // raw sums; alpha and beta are applied by the reduce kernel
-#pragma unroll
-        for (int cc = 0; cc < VW; ++cc) o[cc] = acc.a[cc];
-      }
-      st_vec_once<VW>(dst, o, once);
-    } else if (slot < 0) {  // fp16: Y in S, the partial sums in A
-      S* dst = Y + (int64_t)row * ldy + j;
-      item_epilogue<S, VW>(o, acc, alpha, beta, dst);
-      st_vec_once<VW>(dst, o, once);
-    } else {
-      st_vec_once<VW>(partial + (int64_t)slot * k + j, acc.a, once);
-    }
-  }
-}
-
-// Cooperative variant (default; B200SP_SPMM_ITEM_COOP=0 selects the kernel above): the same items, the same order of
-// additions (bit-identical Y), but the KTL lanes of a group no longer read the same (col, val) address each -- that
-// costs one L1 wavefront per group and entry for the column, one for the value and one for the X row: 3 per
-// nonzero at 8 groups per warp, and the kernel is bound by exactly that (one wavefront per SM and clock).  Here the
-// group reads a batch of EB consecutive entries with ONE load per lane (adjacent lanes, adjacent entries: the group's
-// EB/KTL loads cover a contiguous 32..64-byte run) and passes them round with shuffles, which run on a different
-// pipe: 1 + 2 * 4/32 wavefronts per nonzero for k = 16 fp32, with EB gathers of X in flight per lane (EB = 4: 40 registers,
-// 6 CTAs per SM; EB = 8: 80 registers, 3 CTAs -- the same number of gathers in flight per SM, and 4 was faster when tuned).
-template <typename S, int VW, int KTL, int EB /* entries per batch: 4 or 8 */>
+// Cooperative loads: the KTL lanes of a group do not each read the same (col, val) address -- that costs one L1 wavefront
+// per group and entry for the column, one for the value and one for the X row: 3 per nonzero at 8 groups per warp, and a
+// kernel that did so was bound by exactly that (one wavefront per SM and clock).  The group reads a batch of EB
+// consecutive entries with ONE load per lane (adjacent lanes, adjacent entries: the group's EB/KTL loads cover a
+// contiguous 32..64-byte run) and passes them round with shuffles, which run on a different pipe: 1 + 2 * 4/32
+// wavefronts per nonzero for k = 16 fp32, with EB gathers of X in flight per lane (EB = 4: 40 registers, 6 CTAs per SM;
+// EB = 8, 80 registers and 3 CTAs, was slower when tuned).
+template <typename S, int VW, int KTL, int EB /* entries per batch */>
 __global__ void __launch_bounds__(256)
     spmm_item_coop_kernel(int n_items, const int4* __restrict__ items, int k, const int* __restrict__ col_idx,
                           const S* __restrict__ vals, const S* __restrict__ X, int64_t ldx, S* __restrict__ Y, int64_t ldy,
@@ -1425,8 +648,16 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// the 16-byte item kernels can take row-major X and Y: k, ldx and ldy multiples of the vector width, X and Y 16-byte aligned
 template <typename S>
-static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m, int k, int64_t nnz, const int* row_ptr,
+static bool items_vec(int k, int64_t ldx, int64_t ldy, const S* X, const S* Y) {
+  constexpr int W = VecOf<S>::W;
+  return (k % W == 0) && (ldx % W == 0) && (ldy % W == 0) && ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0;
+}
+
+// the item path on row-major X and Y: the plan's items (built once per matrix), the item kernel, then the reduce kernels
+template <typename S>
+static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, int m, int k, int64_t nnz, const int* row_ptr,
                            const int* col_idx, const S* vals, const S* X, int64_t ldx, S* Y, int64_t ldy, AccT<S> alpha, AccT<S> beta) {
   using A = AccT<S>;
   int LMAX = 64;  // entries per item (B200SP_SPMM_ITEM_LMAX: 16..256); 64 was the best of 32..256 on R-MAT scale 23 when tuned
@@ -1438,6 +669,7 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   int rc = plan_analyse_items(mi, st, LMAX, m, nnz, row_ptr);
   if (rc) return rc;
   B200SP_CUDA_TRY(mi->partial.grow(sizeof(A) * (size_t)mi->n_partial * (size_t)k, st));
+  const bool vec = items_vec(k, ldx, ldy, X, Y);
   constexpr int W = VecOf<S>::W;
   const int lanes_needed = vec ? (k + W - 1) / W : k;
   int KTL = 1;
@@ -1445,21 +677,10 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   const int64_t threads = (int64_t)mi->n_items * KTL;
   const unsigned grid = (unsigned)((threads + 255) / 256);
   if (grid > 0) {
-    static const int coop = [] {  // B200SP_SPMM_ITEM_COOP=0: every lane reads (col, val) itself (the first item kernel); 4 (default) | 8: batch
-      const char* e = getenv("B200SP_SPMM_ITEM_COOP");
-      return e && e[0] == '0' ? 0 : (e && e[0] == '8' ? 8 : 4);  // 4 was the fastest of 0 / 4 / 8 on R-MAT scale 23 x 16 when tuned
-    }();
 #define B200SP_MMI(V, L)                                                                                                   \
   case L:                                                                                                                  \
-    if (coop == 8)                                                                                                         \
-      spmm_item_coop_kernel<S, V, L, 8><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,    \
-                                                              mi->partial.as<A>(), alpha, beta);                               \
-    else if (coop == 4)                                                                                                    \
-      spmm_item_coop_kernel<S, V, L, 4><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,    \
-                                                              mi->partial.as<A>(), alpha, beta);                               \
-    else                                                                                                                   \
-      spmm_item_kernel<S, V, L><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,            \
-                                                      mi->partial.as<A>(), alpha, beta);                                       \
+    spmm_item_coop_kernel<S, V, L, 4><<<grid, 256, 0, st>>>(mi->n_items, mi->items, k, col_idx, vals, X, ldx, Y, ldy,      \
+                                                            mi->partial.as<A>(), alpha, beta);                             \
     break;
     if (vec) {
       switch (KTL) { B200SP_MMI(W, 1) B200SP_MMI(W, 2) B200SP_MMI(W, 4) B200SP_MMI(W, 8) B200SP_MMI(W, 16) B200SP_MMI(W, 32) }
@@ -1483,31 +704,16 @@ static int launch_mm_items(b200sp_spmv_plan* p, cudaStream_t st, bool vec, int m
   return B200SP_OK;
 }
 
-// which rank-2 kernel: 0 = row per group, 1 = nnz-split, 2 = tile, 3 = tile with 16-byte X loads (default: about twice
-// as fast as the split kernel on R-MAT scale 21 x 16 columns when it was tuned).
-// B200SP_SPMM_KERNEL=row|split|tile|tilev overrides.
-static int mm_kernel_choice(b200sp_spmv_plan* p) {
-  if (!p) return 0;  // the others need a plan (chunk table / tile analysis)
-  const char* e = getenv("B200SP_SPMM_KERNEL");
-  if (e && e[0] == 'r') return 0;
-  if (e && e[0] == 's') return 1;
-  if (e && e[0] == 't') return (e[1] == 'i' && e[2] == 'l' && e[3] == 'e' && e[4] == 'v') ? 3 : 2;
-  if (e && e[0] == 'i') return 4;
-  return 4;  // items (B200SP_SPMM_KERNEL=items)
-}
-
-static bool use_split_kernel(b200sp_spmv_plan* p) {
-  // needs a plan (chunk table); B200SP_SPMM_KERNEL=row|split overrides for experiments
-  if (!p) return false;
-  const char* e = getenv("B200SP_SPMM_KERNEL");
-  if (e && e[0] == 'r') return false;
-  return true;
-}
-
+// Y = beta*Y + alpha*op(A)*X for S = double, float and __half (binary16 A, X and Y with fp32 products, sums and epilogue:
+// include/b200sparse.h, DESIGN.md 4.3).  Mode N with a plan takes the item path, through row-major copies for LayoutLeft
+// operands when k >= 4; without a plan, LayoutRight X and Y take spmm_rowmajor_kernel (fp32 / fp64) and everything else
+// spmm_general_kernel.  T/H scatter with atomics.
 template <typename S>
-static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int n, int64_t nnz, int k, S alpha,
+static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int n, int64_t nnz, int k, AccT<S> alpha,
                      const int* row_ptr, const int* col_idx, const S* vals, const S* X, int64_t ldx, int xrm,
-                     S beta, S* Y, int64_t ldy, int yrm) {
+                     AccT<S> beta, S* Y, int64_t ldy, int yrm) {
+  using A = AccT<S>;
+  constexpr bool f16 = std::is_same<S, __half>::value;
   B200SP_REQUIRE(m >= 0 && n >= 0 && nnz >= 0 && k >= 0, "spmm: negative dimension");
   bool trans;
   switch (mode) {
@@ -1522,8 +728,8 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   B200SP_REQUIRE(Y != nullptr, "spmm: Y is null");
   B200SP_REQUIRE((xrm ? ldx >= k : ldx >= xrows) && (yrm ? ldy >= k : ldy >= yrows), "spmm: leading dimension too small");
   const int grid_elem = (int)std::min<int64_t>((yrows * k + 255) / 256, (int64_t)sm_count() * 16);
-  if (alpha == S(0) || m == 0 || n == 0 || nnz == 0) {
-    if (beta != S(1)) {
+  if (alpha == A(0) || m == 0 || n == 0 || nnz == 0) {
+    if (beta != A(1)) {
       scale2d_kernel<S><<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, beta, Y, yr, yc);
       B200SP_LAUNCH_CHECK();
     }
@@ -1531,155 +737,39 @@ static int spmm_impl(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int
   }
   B200SP_REQUIRE(row_ptr && col_idx && vals && X, "spmm: null pointer argument");
   if (trans) {
-    if (beta != S(1)) {
-      scale2d_kernel<S><<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, beta, Y, yr, yc);
-      B200SP_LAUNCH_CHECK();
-    }
     const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
-    spmm_transpose_kernel<S><<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, Y, yr, yc, alpha);
-    B200SP_LAUNCH_CHECK();
-    set_last_kernel(p, "spmm_transpose");
-    return B200SP_OK;
-  }
-  const bool split = use_split_kernel(p);
-  const int choice = mm_kernel_choice(p);
-  if (xrm && yrm) {
-    if (choice == 4) {
-      constexpr int W = VecOf<S>::W;
-      const bool vec = (k % W == 0) && (ldx % W == 0) && (ldy % W == 0) && ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0;
-      set_last_kernel(p, vec ? "spmm_items_vec" : "spmm_items");
-      return launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
-    }
-    const char* name = "rowmajor";
-    int rc;
-    if (choice >= 2 && (((uintptr_t)vals | (uintptr_t)col_idx | (uintptr_t)row_ptr) & 15u) == 0) {
-      constexpr int W = VecOf<S>::W;
-      const bool vec = choice == 3 && (k % W == 0) && (ldx % W == 0) && (ldy % W == 0) && ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0;
-      rc = launch_mm_tile<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta, &name);
-    } else if (split) {
-      rc = launch_split<S>(p, st, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta, &name);
-    } else {
-      rc = launch_rowmajor<S>(st, m, k, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
-    }
-    if (rc) return rc;
-    char label[48];
-    snprintf(label, sizeof(label), "spmm_%s", name);
-    set_last_kernel(p, label);
-    return B200SP_OK;
-  }
-  // LayoutLeft operands: with a plan and k >= 4, relayout to row-major scratch and use the row-major kernel
-  if (p && k >= 4) {
-    B200SP_CUDA_TRY(p->mm.xt.grow(xrm ? 0 : sizeof(S) * (size_t)xrows * k, st));
-    B200SP_CUDA_TRY(p->mm.yt.grow(yrm ? 0 : sizeof(S) * (size_t)yrows * k, st));
-    S* xt = p->mm.xt.as<S>();
-    S* yt = p->mm.yt.as<S>();
-    int rc;
-    const int tb = 256;
-    auto rl_grid = [](int64_t rows) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>((rows + 127) / 128, (int64_t)sm_count() * 16)); };
-    const S* Xr = X;
-    int64_t ldxr = ldx;
-    if (!xrm) {
-      relayout_kernel<S, true><<<rl_grid(xrows), tb, 0, st>>>(xrows, k, xt, X, nullptr, xr, xc);
+    if constexpr (f16) {  // fp32 scratch, then one rounding per entry of Y
+      DevTmp tmp(st);
+      float* acc = nullptr;
+      const size_t acc_bytes = sizeof(float) * (size_t)yrows * (size_t)k;
+      if (p) {
+        B200SP_CUDA_TRY(p->mm.yt.grow(acc_bytes, st));
+        acc = p->mm.yt.as<float>();
+      } else {
+        B200SP_CUDA_TRY(tmp.alloc(&acc, (size_t)yrows * (size_t)k));
+      }
+      B200SP_CUDA_TRY(cudaMemsetAsync(acc, 0, acc_bytes, st));
+      spmm_transpose_acc_kernel<<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, acc);
       B200SP_LAUNCH_CHECK();
-      Xr = xt;
-      ldxr = k;
-    }
-    S* Yr = Y;
-    int64_t ldyr = ldy;
-    if (!yrm) {
-      Yr = yt;
-      ldyr = k;
-      if (beta != S(0)) {
-        relayout_kernel<S, true><<<rl_grid(yrows), tb, 0, st>>>(yrows, k, Yr, Y, nullptr, yr, yc);
+      spmm_acc_epilogue_kernel<<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, acc, alpha, beta, Y, yr, yc);
+      B200SP_LAUNCH_CHECK();
+    } else {
+      if (beta != A(1)) {
+        scale2d_kernel<S><<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, beta, Y, yr, yc);
         B200SP_LAUNCH_CHECK();
       }
-    }
-    const bool tile_ok = choice >= 2 && (choice == 4 || (((uintptr_t)vals | (uintptr_t)col_idx | (uintptr_t)row_ptr) & 15u) == 0);
-    const char* name = choice == 4 ? "items" : split ? "split" : "rowmajor";
-    if (choice == 4) {
-      constexpr int W = VecOf<S>::W;
-      const bool vec = (k % W == 0) && (ldxr % W == 0) && (ldyr % W == 0) && ((((uintptr_t)Xr) | ((uintptr_t)Yr)) & 15u) == 0;
-      rc = launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta);
-    } else if (tile_ok) {
-      constexpr int W = VecOf<S>::W;
-      const bool vec = choice == 3 && (k % W == 0) && (ldxr % W == 0) && (ldyr % W == 0) && ((((uintptr_t)Xr) | ((uintptr_t)Yr)) & 15u) == 0;
-      rc = launch_mm_tile<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta, &name);
-    } else {
-      rc = split ? launch_split<S>(p, st, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta, &name)
-                 : launch_rowmajor<S>(st, m, k, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta);
-    }
-    if (rc) return rc;
-    if (!yrm) {
-      relayout_kernel<S, false><<<rl_grid(yrows), tb, 0, st>>>(yrows, k, Yr, nullptr, Y, yr, yc);
+      spmm_transpose_kernel<S><<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, Y, yr, yc, alpha);
       B200SP_LAUNCH_CHECK();
     }
-    char label[48];
-    snprintf(label, sizeof(label), "spmm_relayout+%s", name);
-    set_last_kernel(p, label);
-    return B200SP_OK;
-  }
-  const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
-  spmm_general_kernel<S><<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, Y, yr, yc, alpha, beta);
-  B200SP_LAUNCH_CHECK();
-  set_last_kernel(p, "spmm_general");
-  return B200SP_OK;
-}
-
-// binary16 A, X and Y with fp32 products, sums and epilogue (include/b200sparse.h, DESIGN.md 4.3).  The item path and its
-// relayout serve mode N with a plan; B200SP_SPMM_KERNEL does not apply.  Without a plan, or for LayoutLeft with k < 4:
-// spmm_general_kernel.  T/H: fp32 scratch + one epilogue.
-static int spmm_impl_f16(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m, int n, int64_t nnz, int k, float alpha,
-                         const int* row_ptr, const int* col_idx, const __half* vals, const __half* X, int64_t ldx, int xrm,
-                         float beta, __half* Y, int64_t ldy, int yrm) {
-  using S = __half;
-  B200SP_REQUIRE(m >= 0 && n >= 0 && nnz >= 0 && k >= 0, "spmm: negative dimension");
-  bool trans;
-  switch (mode) {
-    case 'N': case 'n': case 'C': case 'c': trans = false; break;
-    case 'T': case 't': case 'H': case 'h': trans = true; break;
-    default: set_error("Invalid transpose mode %c for KokkosSparse::spmv()", mode); return B200SP_ERR_INVALID_ARGUMENT;
-  }
-  const int64_t xrows = trans ? m : n, yrows = trans ? n : m;
-  const int64_t xr = xrm ? ldx : 1, xc = xrm ? 1 : ldx;
-  const int64_t yr = yrm ? ldy : 1, yc = yrm ? 1 : ldy;
-  if (k == 0 || yrows == 0) return B200SP_OK;
-  B200SP_REQUIRE(Y != nullptr, "spmm: Y is null");
-  B200SP_REQUIRE((xrm ? ldx >= k : ldx >= xrows) && (yrm ? ldy >= k : ldy >= yrows), "spmm: leading dimension too small");
-  const int grid_elem = (int)std::min<int64_t>((yrows * k + 255) / 256, (int64_t)sm_count() * 16);
-  if (alpha == 0.0f || m == 0 || n == 0 || nnz == 0) {
-    if (beta != 1.0f) {
-      scale2d_kernel<S><<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, beta, Y, yr, yc);
-      B200SP_LAUNCH_CHECK();
-    }
-    return B200SP_OK;
-  }
-  B200SP_REQUIRE(row_ptr && col_idx && vals && X, "spmm: null pointer argument");
-  if (trans) {
-    DevTmp tmp(st);
-    float* acc = nullptr;
-    const size_t acc_bytes = sizeof(float) * (size_t)yrows * (size_t)k;
-    if (p) {
-      B200SP_CUDA_TRY(p->mm.yt.grow(acc_bytes, st));
-      acc = p->mm.yt.as<float>();
-    } else {
-      B200SP_CUDA_TRY(tmp.alloc(&acc, (size_t)yrows * (size_t)k));
-    }
-    B200SP_CUDA_TRY(cudaMemsetAsync(acc, 0, acc_bytes, st));
-    const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
-    spmm_transpose_acc_kernel<<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, acc);
-    B200SP_LAUNCH_CHECK();
-    spmm_acc_epilogue_kernel<<<std::max(grid_elem, 1), 256, 0, st>>>(yrows, k, acc, alpha, beta, Y, yr, yc);
-    B200SP_LAUNCH_CHECK();
     set_last_kernel(p, "spmm_transpose");
     return B200SP_OK;
   }
-  constexpr int W = VecOf<S>::W;
   if (p && xrm && yrm) {
-    const bool vec = (k % W == 0) && (ldx % W == 0) && (ldy % W == 0) && ((((uintptr_t)X) | ((uintptr_t)Y)) & 15u) == 0;
-    set_last_kernel(p, vec ? "spmm_items_vec" : "spmm_items");
-    return launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
+    set_last_kernel(p, items_vec(k, ldx, ldy, X, Y) ? "spmm_items_vec" : "spmm_items");
+    return launch_mm_items<S>(p, st, m, k, nnz, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);
   }
-  if (p && k >= 4) {  // LayoutLeft operands: row-major copies in the plan's scratch, as for fp32
+  // LayoutLeft operands: with a plan and k >= 4, relayout to row-major scratch and take the item path
+  if (p && k >= 4) {
     B200SP_CUDA_TRY(p->mm.xt.grow(xrm ? 0 : sizeof(S) * (size_t)xrows * k, st));
     B200SP_CUDA_TRY(p->mm.yt.grow(yrm ? 0 : sizeof(S) * (size_t)yrows * k, st));
     S* xt = p->mm.xt.as<S>();
@@ -1698,19 +788,21 @@ static int spmm_impl_f16(b200sp_spmv_plan* p, cudaStream_t st, char mode, int m,
     if (!yrm) {
       Yr = yt;
       ldyr = k;
-      if (beta != 0.0f) {
+      if (beta != A(0)) {
         relayout_kernel<S, true><<<rl_grid(yrows), 256, 0, st>>>(yrows, k, Yr, Y, nullptr, yr, yc);
         B200SP_LAUNCH_CHECK();
       }
     }
-    const bool vec = (k % W == 0) && (ldxr % W == 0) && (ldyr % W == 0) && ((((uintptr_t)Xr) | ((uintptr_t)Yr)) & 15u) == 0;
-    if (int rc = launch_mm_items<S>(p, st, vec, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta)) return rc;
+    if (int rc = launch_mm_items<S>(p, st, m, k, nnz, row_ptr, col_idx, vals, Xr, ldxr, Yr, ldyr, alpha, beta)) return rc;
     if (!yrm) {
       relayout_kernel<S, false><<<rl_grid(yrows), 256, 0, st>>>(yrows, k, Yr, nullptr, Y, yr, yc);
       B200SP_LAUNCH_CHECK();
     }
     set_last_kernel(p, "spmm_relayout+items");
     return B200SP_OK;
+  }
+  if constexpr (!f16) {
+    if (xrm && yrm) return launch_rowmajor<S>(st, m, k, row_ptr, col_idx, vals, X, ldx, Y, ldy, alpha, beta);  // no plan
   }
   const int g = (int)std::min<int64_t>(((int64_t)m * k + 255) / 256, (int64_t)sm_count() * 16);
   spmm_general_kernel<S><<<std::max(g, 1), 256, 0, st>>>(m, k, row_ptr, col_idx, vals, X, xr, xc, Y, yr, yc, alpha, beta);
@@ -1740,7 +832,7 @@ int b200sp_spmm_f16_i32(b200sp_spmv_plan* plan, void* stream, char mode, int m, 
                         const int* row_ptr, const int* col_idx, const uint16_t* vals, const uint16_t* X, int64_t ldx,
                         int x_row_major, float beta, uint16_t* Y, int64_t ldy, int y_row_major) {
   static_assert(sizeof(__half) == sizeof(uint16_t), "binary16 bit patterns");
-  return spmm_impl_f16(plan, (cudaStream_t)stream, mode, m, n, nnz, k, alpha, row_ptr, col_idx, reinterpret_cast<const __half*>(vals),
-                       reinterpret_cast<const __half*>(X), ldx, x_row_major, beta, reinterpret_cast<__half*>(Y), ldy, y_row_major);
+  return spmm_impl<__half>(plan, (cudaStream_t)stream, mode, m, n, nnz, k, alpha, row_ptr, col_idx, reinterpret_cast<const __half*>(vals),
+                           reinterpret_cast<const __half*>(X), ldx, x_row_major, beta, reinterpret_cast<__half*>(Y), ldy, y_row_major);
 }
 }

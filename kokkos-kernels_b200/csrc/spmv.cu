@@ -355,7 +355,7 @@ __global__ void find_long_rows_kernel(int m, const int* __restrict__ row_ptr, in
     if (row_ptr[r + 1] - row_ptr[r] > LMAX) long_rows[atomicAdd(n_long, 1)] = r;
 }
 
-// The tiles and long rows of the tile kernels (spmv_tile_kernel, spmm_tile_kernel, the BSR ones of bsr.cu with blocks for
+// The tiles and long rows of the tile kernels (spmv_tile_kernel, the BSR ones of bsr.cu with blocks for
 // entries) for a stage of cap entries and a row limit of lmax.  *out owns what it allocated, also on an error.
 int tile_analyse(cudaStream_t st, int m, int64_t nnz, const int* row_ptr, int cap, int lmax, TileAnalysis* out) {
   out->LMAX = lmax;

@@ -134,21 +134,14 @@ struct MMItems {
 
 // rank-2 state (spmm.cu)
 struct SpmmState {
-  // tile kernel: its own tile analysis (smaller row limit) + segments {row, e0, e1, flags} of the long rows (flags bit 0:
-  // the row has several segments, bit 1: first segment)
-  TileAnalysis tiles;
-  DevArray<int4> segs;
-  DevArray<int> n_seg;
-  PlanKey tiles_key;
   MMItems items;  // item kernel
-  // nnz-chunk -> row table of the split kernel
-  DevArray<int> chunk_row;
-  int n_chunks = 0;
-  PlanKey chunk_key;
   DevArray<char> xt, yt;  // row-major copies of LayoutLeft operands: size-only, kept by reset()
-  void release_tiles(cudaStream_t st);
-  void reset(cudaStream_t st);
-  void release(cudaStream_t st);
+  void reset(cudaStream_t st) { items.release(st); }
+  void release(cudaStream_t st) {
+    reset(st);
+    xt.release(st);
+    yt.release(st);
+  }
 };
 
 // cached transpose (B200SP_SPMV_OPT_CACHE_TRANSPOSE): structure of A^T + source entry of each of its entries, values

@@ -1,7 +1,7 @@
 // tile_ring.cuh -- the shared-memory ring of row-aligned tiles that a producer warp fills with 1-D TMA bulk copies
-// (cp.async.bulk + mbarrier) for the consumer warps of the tile kernels: spmv_tile_kernel (spmv.cu, DESIGN.md 3.1),
-// spmm_tile_kernel (spmm.cu) and the BsrMatrix tile kernels (bsr.cu), whose entries are blocks of bs*bs values.  The
-// tile descriptors are made once for all of them by tile_analyse (build_tiles_kernel, spmv.cu).
+// (cp.async.bulk + mbarrier) for the consumer warps of the tile kernels: spmv_tile_kernel (spmv.cu, DESIGN.md 3.1) and
+// the BsrMatrix tile kernels (bsr.cu), whose entries are blocks of bs*bs values.  The tile descriptors are made once for
+// all of them by tile_analyse (build_tiles_kernel, spmv.cu).
 #pragma once
 #include "common.cuh"
 
@@ -132,7 +132,7 @@ __device__ __forceinline__ void tile_ring_issue(Ring& sm, int stage, int4 d, con
   if (ts.nrp > 0) bulk_g2s(sm.rows[stage], row_ptr + ts.r0_al, (uint32_t)(ts.nrp * 4), &sm.full[stage], pol);
 }
 
-// The producer of spmm_tile_kernel and the BSR tile kernels (vpe values per entry: 1 for CSR, bs*bs for BSR).
+// The producer of the BSR tile kernels (vpe values per entry: bs*bs).
 // spmv_tile_kernel has its own, which also streams its 16-bit column forms.
 template <typename Ring>
 __device__ __forceinline__ void tile_ring_produce(Ring& sm, int lane, int m, int64_t nnz, int vpe, int n_tiles,

@@ -3,18 +3,16 @@ shared by the emulated-kernel tests and the GPU tests.  Every builder takes a se
 (rp, ci, v, ncols); values are mixed-sign and span a few binades, so that dropping, repeating or misplacing a term shows.
 
 The thresholds (csrc/spmm.cu):
-  * cooperative item kernel: batches of EB = 4 or 8 entries, then a remainder of 0..EB-1;
+  * cooperative item kernel: batches of EB = 4 entries, then a remainder of 0..EB-1;
   * items of LMAX entries (B200SP_SPMM_ITEM_LMAX, 16..256, default 64): longer rows are split into pieces;
-  * rows of more than MMI_LONG_PIECES = 64 pieces are reduced by a CTA instead of a warp;
-  * tile kernel: rows longer than its row limit (B200SP_SPMM_LMAX, default 256) go to the segment kernels, in segments
-    of 2048 entries (several segments: pre-scaled row plus atomics)."""
+  * rows of more than MMI_LONG_PIECES = 64 pieces are reduced by a CTA instead of a warp."""
 import numpy as np
 
 # row lengths straddling every threshold above, at the default LMAX values
-THRESHOLD_LENGTHS = [0, 1, 3, 4, 5, 7, 8, 9,          # EB = 4 / 8 batch remainders
-                     15, 16, 17, 255, 256, 257,       # item LMAX extremes; tile row limit
+THRESHOLD_LENGTHS = [0, 1, 3, 4, 5, 7, 8, 9,          # EB = 4 batch remainders
+                     15, 16, 17, 255, 256, 257,       # item LMAX extremes
                      63, 64, 65, 127, 128, 129,       # item pieces at LMAX = 64
-                     2047, 2048, 2049, 4097,          # one / several segments of 2048
+                     2047, 2048, 2049, 4097,          # long rows of many pieces
                      4096]                            # exactly 64 pieces of 64 (warp reduce); 4097 is the CTA reduce
 
 

@@ -165,18 +165,17 @@ def test_spmv_cached_transpose(emu, oracle):
 
 
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])
-@pytest.mark.parametrize("kernel,extra", [("items", {}), ("items", {"B200SP_SPMM_ITEM_LMAX": "16"}), ("tilev", {}), ("tile", {}), ("split", {}),
-                                          ("row", {}), ("tilev", {"B200SP_SPMM_SEG": "vec"}), ("tilev", {"B200SP_SPMM_LMAX": "64"})])
-def test_spmm_kernels_layouts(emu, oracle, dtype, kernel, extra):
+@pytest.mark.parametrize("lmax", [None, "16"], ids=["items", "items16"])
+def test_spmm_kernels_layouts(emu, oracle, dtype, lmax):
     rng = np.random.default_rng(11)
     rows, cols = 1500, 1300
     lens = rng.integers(0, 30, rows)
-    lens[[3, 700]] = [1200, 1100]  # long rows -> the segment kernels
+    lens[[3, 700]] = [1200, 1100]  # long rows -> rows of many pieces
     rp = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
     ci = np.concatenate([np.sort(rng.choice(cols, l, replace=False)) for l in lens]).astype(np.int32)
     v = rng.uniform(-1, 1, len(ci)).astype(dtype)
-    with env(B200SP_SPMM_KERNEL=kernel, **extra):
-        for k in (1, 3, 8, 17, 16, 40) if kernel == "items" else (1, 3, 8, 17):
+    with env(B200SP_SPMM_ITEM_LMAX=lmax):
+        for k in (1, 3, 8, 17, 16, 40):
             for order in "CF":
                 X = np.asarray(rng.random((cols, k)).astype(dtype), order=order)
                 Y0 = np.asarray(rng.random((rows, k)).astype(dtype), order=order)
@@ -192,7 +191,7 @@ def test_spmm_kernels_layouts(emu, oracle, dtype, kernel, extra):
                     for j in range(k):
                         scale = rowwise_scale(rp, ci, v, X[:, j], Y0[:, j], alpha, beta)
                         err = np.abs(Y[:, j].astype(np.float64) - exp[:, j].astype(np.float64))
-                        assert not (err > TOL[v.dtype] * scale + 1e-300).any(), (kernel, extra, k, order, alpha, beta, j)
+                        assert not (err > TOL[v.dtype] * scale + 1e-300).any(), (lmax, k, order, alpha, beta, j)
 
 
 def gen_ab(oracle, m, k, n, nnz, dtype):

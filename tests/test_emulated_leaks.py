@@ -173,7 +173,7 @@ def hostvec(emu, p, mode, m, n, rp, ci, v, x, y, alpha, beta):
 
 def test_spmv_plan_parts_give_everything_back(emu):
     """each part of the SpMV plan that no bracket above reaches: long-row segments, the pattern form's tile table and the cfg's
-    cut again, the rank-2 tile and split kernels, the simple host-vector path, and every part built again after invalidate"""
+    cut again, the simple host-vector path, and every part built again after invalidate"""
     from test_emulated_kernels import env
     import pattern_cases as PC
 
@@ -198,14 +198,6 @@ def test_spmv_plan_parts_give_everything_back(emu):
                 E.spmv(p, "N", len(A[0]) - 1, A[3], A[0], A[1], A[2], np.ones(A[3]), ya, 1.0, 0.0)
             assert ("COLS=pat" in p.kernel()) == (idx16 is None), p.kernel()
         p.close()
-    with balanced(emu, "rank-2 tile and split kernels (segments, chunk table)"):
-        p = E.SpmvPlan()
-        for kern in ("tile", "tilev", "split"):
-            with env(B200SP_SPMM_KERNEL=kern):
-                Y = np.zeros((m, 8))
-                E.spmm(p, "N", m, n, rp, ci, v, np.asarray(rng.random((n, 8))), Y, 1.0, 0.0)
-                assert p.kernel().startswith("spmm_" + kern[:4]), p.kernel()
-        p.close()
     with balanced(emu, "simple host-vector path (staging vectors)"):
         p = E.SpmvPlan()
         for mode, xv, ylen in (("N", x, m), ("T", xt, n), ("N", x, m)):
@@ -221,9 +213,6 @@ def test_spmv_plan_parts_give_everything_back(emu):
             E.spmv(p, "T", m, n, rp, ci, v, xt, np.zeros(n), 1.0, 0.0)
             for order in "CF":
                 E.spmm(p, "N", m, n, rp, ci, v, np.asarray(rng.random((n, 5)), order=order), np.zeros((m, 5), order=order), 1.0, 0.0)
-            for kern in ("tile", "split"):
-                with env(B200SP_SPMM_KERNEL=kern):
-                    E.spmm(p, "N", m, n, rp, ci, v, rng.random((n, 8)), np.zeros((m, 8)), 1.0, 0.0)
             hostvec(emu, p, "N", m, n, rp, ci, v, x, np.zeros(m), 1.0, 0.0)
             E.ok(emu.b200sp_spmv_plan_invalidate(p.h, None))
         p.close()

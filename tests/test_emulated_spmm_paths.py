@@ -10,16 +10,10 @@ import spmm_cases as cases
 from test_emulated_kernels import env
 
 PATHS = {
-    "items": {"B200SP_SPMM_KERNEL": "items"},
-    "items16": {"B200SP_SPMM_KERNEL": "items", "B200SP_SPMM_ITEM_LMAX": "16"},
-    "items256": {"B200SP_SPMM_KERNEL": "items", "B200SP_SPMM_ITEM_LMAX": "256"},
-    "tile": {"B200SP_SPMM_KERNEL": "tile"},
-    "tilev": {"B200SP_SPMM_KERNEL": "tilev"},
-    "tilev_cfg1": {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_CFG": "1"},
-    "tilev_segvec_lmax16": {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_SEG": "vec", "B200SP_SPMM_LMAX": "16"},
-    "split": {"B200SP_SPMM_KERNEL": "split"},
-    "split_vec": {"B200SP_SPMM_KERNEL": "split", "B200SP_SPMM_VEC": "1"},
-    "row": {"B200SP_SPMM_KERNEL": "row"},
+    "items": {},
+    "items16": {"B200SP_SPMM_ITEM_LMAX": "16"},
+    "items64": {"B200SP_SPMM_ITEM_LMAX": "64"},
+    "items256": {"B200SP_SPMM_ITEM_LMAX": "256"},
 }
 KS = [1, 4, 5, 16, 33, 64]
 
@@ -107,3 +101,29 @@ def test_item_path_identities(emu, dtype):
             assert kern_o == "spmm_items", kern_o
         for other in (again, left, Yo):
             assert np.array_equal(np.ascontiguousarray(other).view(np.uint8), ref.view(np.uint8)), (k, kern, kern_l, kern_o)
+
+
+# variables that once selected kernels of spmm.cu; nothing reads them any more
+RETIRED = [dict(B200SP_SPMM_KERNEL=kern, B200SP_SPMM_SEG="vec", B200SP_SPMM_VEC="1", B200SP_SPMM_CFG="2", B200SP_SPMM_LMAX="16")
+           for kern in ("row", "split", "tilev")]
+
+
+@pytest.mark.parametrize("dtype", [np.float64, np.float32, np.float16])
+def test_retired_variables_are_inert(emu, dtype):
+    """With every retired selection variable set, fp64, fp32 and fp16 calls report the default kernel and give the same bits
+    as without them, for LayoutRight and LayoutLeft operands."""
+    from test_emulated_spmm_f16 import case16, run16
+
+    A_np = case16("thresholds") if dtype == np.float16 else cases.thresholds(5, dtype)
+    call = run16 if dtype == np.float16 else run
+    for k in (5, 16):
+        for order in "CF":
+            X, Y0 = operands(A_np, k, dtype, order)
+            ref, kern = call(A_np, X, Y0, 1.5, -0.5)
+            assert kern in ("spmm_items", "spmm_items_vec", "spmm_relayout+items"), kern
+            for retired in RETIRED:
+                with env(**retired):
+                    got, kern_r = call(A_np, X, Y0, 1.5, -0.5)
+                what = f"{np.dtype(dtype).name} k={k} order={order} {retired}"
+                assert kern_r == kern, (what, kern_r, kern)
+                assert np.array_equal(np.ascontiguousarray(got).view(np.uint8), np.ascontiguousarray(ref).view(np.uint8)), what

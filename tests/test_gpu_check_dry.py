@@ -1,6 +1,7 @@
 """tools/gpu_check (the torch-free GPU validation harness) must build and its host side -- generators, oracle calls,
 comparison code of every suite -- must run to completion without a GPU (`--dry`: device buffers live in host memory,
 C-ABI calls are skipped, so every comparison fails by construction but nothing may crash)."""
+import collections
 import json
 import os
 import subprocess
@@ -24,4 +25,6 @@ def test_harness_host_side_runs(tmp_path):
     for s in suites:
         assert "signal=0" in summary[s] and "exit=1" in summary[s], (s, summary[s])  # ran to the end, comparisons failed as they must
     assert res.returncode == len(suites)
-    assert sum(r["suite"] != "summary" for r in recs) > 40
+    # every case of every suite is recorded; spmm_sweep: 4 matrices, each with a plan and without one
+    per_suite = collections.Counter(r["suite"] for r in recs if r["suite"] != "summary")
+    assert per_suite == {"crs": 24, "jacobi": 4, "spmv_t": 4, "spmm_sweep": 8}, per_suite

@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 F16 = np.float16
 EMULATED = os.environ.get("B200SP_TEST_EMULATED") == "1"
-SPMM_VARS = ["B200SP_SPMM_KERNEL", "B200SP_SPMM_ITEM_LMAX", "B200SP_SPMM_CFG", "B200SP_SPMM_LMAX", "B200SP_SPMM_SEG", "B200SP_SPMM_VEC"]
+SPMM_VARS = ["B200SP_SPMM_ITEM_LMAX"]
 LAYOUTS = ["RR", "LL", "RL", "LR"]  # X layout, Y layout: R = LayoutRight (row-major), L = LayoutLeft
 
 

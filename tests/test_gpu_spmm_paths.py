@@ -1,11 +1,9 @@
 """Every rank-2 SpMV kernel path (csrc/spmm.cu) on the GPU, each call checked entry by entry against the exact product
-(tests/exact_ref.py) within a rigorous per-entry rounding bound, in fp32 and fp64.  Paths are selected with the library's
-B200SP_SPMM_* variables (read by getenv on every call), and every test that selects one asserts the handle's
-last_kernel(), so a dispatcher that quietly falls back cannot make a test vacuous."""
+(tests/exact_ref.py) within a rigorous per-entry rounding bound, in fp32 and fp64.  The operands' layouts, strides and alignment and the
+presence of a plan select the path, B200SP_SPMM_ITEM_LMAX (read by getenv on every call) the item length, and every test
+that runs with a plan asserts the handle's last_kernel(), so a dispatcher that quietly falls back cannot make a test
+vacuous."""
 import os
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
@@ -19,7 +17,7 @@ pytestmark = pytest.mark.gpu
 DTYPES = [np.float32, np.float64]
 TDT = {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64}
 LAYOUTS = ["RR", "LL", "RL", "LR"]  # X layout, Y layout: R = LayoutRight (row-major), L = LayoutLeft
-SPMM_VARS = ["B200SP_SPMM_KERNEL", "B200SP_SPMM_ITEM_LMAX", "B200SP_SPMM_CFG", "B200SP_SPMM_LMAX", "B200SP_SPMM_SEG", "B200SP_SPMM_VEC"]
+SPMM_VARS = ["B200SP_SPMM_ITEM_LMAX"]
 EMULATED = os.environ.get("B200SP_TEST_EMULATED") == "1"
 
 
@@ -69,24 +67,15 @@ def kernel(h):
     return h.last_kernel() if h is not None else "no plan"
 
 
-def expected_kernel(env, k, dtype, layout, ld_vec=True):
-    """The label spmm_impl reports for these settings (16-byte aligned operands, a plan).  ld_vec=False: a LayoutRight
-    operand has a leading dimension that is not a multiple of the vector width, which rules out the 16-byte kernels."""
+def expected_kernel(k, dtype, layout, ld_vec=True):
+    """The label spmm_impl reports for these operands (16-byte aligned, a plan).  ld_vec=False: a LayoutRight operand has a
+    leading dimension that is not a multiple of the vector width, which rules out the 16-byte kernels."""
     if k == 1:
         layout = "RR"  # a single column is passed as LayoutRight whatever its strides
-    if layout != "RR" and k < 4:
-        return "spmm_general"
+    if layout != "RR":
+        return "spmm_relayout+items" if k >= 4 else "spmm_general"
     vec = k % (4 if np.dtype(dtype) == np.float32 else 2) == 0 and ld_vec
-    kern = env.get("B200SP_SPMM_KERNEL", "items")
-    if kern == "items":
-        name = "items_vec" if vec and layout == "RR" else "items"
-    elif kern in ("tile", "tilev"):
-        name = "tile_vec" + ("+seg_vec" if env.get("B200SP_SPMM_SEG") == "vec" else "") if kern == "tilev" and vec else "tile"
-    elif kern == "split":
-        name = "split_vec" if env.get("B200SP_SPMM_VEC") and vec else "split"
-    else:
-        name = "rowmajor"
-    return ("spmm_" if layout == "RR" else "spmm_relayout+") + name
+    return "spmm_items_vec" if vec else "spmm_items"
 
 
 def check(got, A_np, X, Y0, alpha, beta, trans, what):
@@ -104,31 +93,19 @@ def operands(A_np, k, dtype, trans=False, seed=0):
 
 # ---- (a) each path ---------------------------------------------------------------------------------------------------
 PATHS = [
-    {"B200SP_SPMM_KERNEL": "items", "B200SP_SPMM_ITEM_LMAX": "16"},
-    {"B200SP_SPMM_KERNEL": "items", "B200SP_SPMM_ITEM_LMAX": "64"},
-    {"B200SP_SPMM_KERNEL": "items", "B200SP_SPMM_ITEM_LMAX": "256"},
-    {"B200SP_SPMM_KERNEL": "tile"},
-    {"B200SP_SPMM_KERNEL": "tile", "B200SP_SPMM_LMAX": "16"},
-    {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_CFG": "0"},
-    {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_CFG": "1"},
-    {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_CFG": "2"},
-    {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_CFG": "3"},
-    {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_LMAX": "16"},
-    {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_LMAX": "512"},
-    {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_SEG": "vec"},
-    {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_SEG": "vec", "B200SP_SPMM_LMAX": "16"},
-    {"B200SP_SPMM_KERNEL": "split"},
-    {"B200SP_SPMM_KERNEL": "split", "B200SP_SPMM_VEC": "1"},
-    {"B200SP_SPMM_KERNEL": "row"},
+    {},
+    {"B200SP_SPMM_ITEM_LMAX": "16"},
+    {"B200SP_SPMM_ITEM_LMAX": "64"},
+    {"B200SP_SPMM_ITEM_LMAX": "256"},
 ]
-PATH_IDS = ["-".join(f"{k.replace('B200SP_SPMM_', '').lower()}={v}" for k, v in p.items()) for p in PATHS]
+PATH_IDS = ["-".join(f"{k.replace('B200SP_SPMM_', '').lower()}={v}" for k, v in p.items()) or "default" for p in PATHS]
 PATH_KS = [1, 5, 16, 36, 132]
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("env", PATHS, ids=PATH_IDS)
 def test_each_path(cuda, monkeypatch, env, dtype):
-    """The threshold matrix (row lengths around every batch, item, tile and segment limit) through one kernel path, with a
+    """The threshold matrix (row lengths around every batch and item limit) through the item path at one item length, with a
     fresh handle, for k crossing the vector width and the 32-lane strips, LayoutRight and LayoutLeft (relayout)."""
     from kokkos_kernels_b200 import sparse as sp
 
@@ -143,7 +120,7 @@ def test_each_path(cuda, monkeypatch, env, dtype):
         bound = R.spmm_bound(*A_np[:3], X, Y0, 2.5, -0.5)
         for layout in ("RR", "LL"):
             got = spmv(h, "N", 2.5, A, dev(cuda, X, layout[0] == "R"), -0.5, dev(cuda, Y0, layout[1] == "R"))
-            assert h.last_kernel() == expected_kernel(env, k, dtype, layout), (env, k, layout, h.last_kernel())
+            assert h.last_kernel() == expected_kernel(k, dtype, layout), (env, k, layout, h.last_kernel())
             R.assert_within(got, exact, bound, f"{h.last_kernel()} {env} k={k} {layout} {np.dtype(dtype).name}")
 
 
@@ -172,11 +149,12 @@ def test_transpose_every_layout(cuda, mode, dtype):
 
 @pytest.mark.parametrize("dtype", DTYPES)
 def test_no_plan_paths(cuda, dtype):
-    """handle=None: spmm_rowmajor_kernel for LayoutRight X and Y, spmm_general_kernel for any other mix."""
+    """handle=None: spmm_rowmajor_kernel for LayoutRight X and Y (k from 1 to 33: every group width KT from 1 to 32),
+    spmm_general_kernel for any other mix."""
     for name in ("thresholds", "small_mod1", "duplicates", "cancelling"):
         A_np = matrix(name, dtype)
         A = dev_matrix(cuda, *A_np)
-        for k in (1, 3, 8, 33):
+        for k in (1, 2, 3, 5, 8, 16, 17, 33):
             X, Y0 = operands(A_np, k, dtype)
             exact = R.spmm_exact(*A_np[:3], X, Y0, -1.0, 1.0)
             bound = R.spmm_bound(*A_np[:3], X, Y0, -1.0, 1.0)
@@ -204,7 +182,7 @@ def test_k_sweep(cuda, dtype):
         for layout in LAYOUTS:
             h = sp.SPMVHandle()
             got = spmv(h, "N", 1.5, A, dev(cuda, X, layout[0] == "R"), 0.5, dev(cuda, Y0, layout[1] == "R"))
-            assert h.last_kernel() == expected_kernel({}, k, dtype, layout), (k, layout, h.last_kernel())
+            assert h.last_kernel() == expected_kernel(k, dtype, layout), (k, layout, h.last_kernel())
             R.assert_within(got, exact, bound, f"{h.last_kernel()} k={k} {layout} {np.dtype(dtype).name}")
 
 
@@ -228,17 +206,12 @@ def padded(cuda, a, rowmajor, extra_cols, extra_rows=5):
 
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("pad", [4, 3], ids=["ld_vector", "ld_odd"])
-@pytest.mark.parametrize("env", [{}, {"B200SP_SPMM_KERNEL": "tilev"}, {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_SEG": "vec"},
-                                 {"B200SP_SPMM_KERNEL": "split", "B200SP_SPMM_VEC": "1"}, {"B200SP_SPMM_KERNEL": "row"}],
-                         ids=["items", "tilev", "tilev_segvec", "split_vec", "row"])
-def test_strided_views(cuda, monkeypatch, env, pad, dtype):
+def test_strided_views(cuda, pad, dtype):
     """X and Y as slices of wider tensors in both layouts: correct, and nothing outside Y's view is written.  Padding
     LayoutRight rows by 4 keeps ld a multiple of the vector width, so the 16-byte kernels run with ld > k (a vector store
     past k would land in the padding); padding by 3 makes ld odd and selects the scalar kernels."""
     from kokkos_kernels_b200 import sparse as sp
 
-    for k_, v_ in env.items():
-        monkeypatch.setenv(k_, v_)
     A_np = matrix("thresholds", dtype)
     A = dev_matrix(cuda, *A_np)
     for k in (4, 6, 16, 36, 132):
@@ -251,9 +224,9 @@ def test_strided_views(cuda, monkeypatch, env, pad, dtype):
             Yv, Yb = padded(cuda, Y0, layout[1] == "R", pad)
             before = Yb.cpu().numpy().copy()
             got = spmv(h, "N", 2.5, A, Xv, -0.5, Yv)
-            what = f"{h.last_kernel()} {env} k={k} {layout} strided pad={pad}"
+            what = f"{h.last_kernel()} k={k} {layout} strided pad={pad}"
             ld_vec = pad % (4 if np.dtype(dtype) == np.float32 else 2) == 0 or layout == "LL"  # LL: row-major scratch, ld = k
-            assert h.last_kernel() == expected_kernel(env, k, dtype, layout, ld_vec), what
+            assert h.last_kernel() == expected_kernel(k, dtype, layout, ld_vec), what
             R.assert_within(got, exact, bound, what)
             after = Yb.cpu().numpy()
             outside = np.ones(after.shape, bool)
@@ -271,19 +244,13 @@ def offset_by_one(cuda, a):
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("env", [{}, {"B200SP_SPMM_KERNEL": "tilev"}, {"B200SP_SPMM_KERNEL": "split", "B200SP_SPMM_VEC": "1"}],
-                         ids=["items", "tilev", "split_vec"])
-def test_misaligned_operands(cuda, monkeypatch, env, dtype):
-    """X / Y one element off 16-byte alignment: the scalar kernel, and for the item and tile kernels the same bits as the
-    aligned vector kernel (per column the additions come in the same order).  The tile path adds the segments of rows
-    longer than 2048 entries with atomics: those rows are held to the bound only."""
+def test_misaligned_operands(cuda, dtype):
+    """X / Y one element off 16-byte alignment: the scalar item kernel, with the same bits as the aligned vector kernel (per
+    column the additions come in the same order)."""
     from kokkos_kernels_b200 import sparse as sp
 
-    for k_, v_ in env.items():
-        monkeypatch.setenv(k_, v_)
     A_np = matrix("thresholds", dtype)
     A = dev_matrix(cuda, *A_np)
-    rows = slice(None) if not env else np.diff(A_np[0]) <= 2048
     for k in (4, 16, 132):
         X, Y0 = operands(A_np, k, dtype)
         exact = R.spmm_exact(*A_np[:3], X, Y0, 2.5, -0.5)
@@ -291,26 +258,23 @@ def test_misaligned_operands(cuda, monkeypatch, env, dtype):
         h = sp.SPMVHandle()
         ref = spmv(h, "N", 2.5, A, dev(cuda, X, True), -0.5, dev(cuda, Y0, True))
         vec_kernel = h.last_kernel()
-        assert vec_kernel == expected_kernel(env, k, dtype, "RR")
+        assert vec_kernel == expected_kernel(k, dtype, "RR")
         for xoff, yoff in ((True, False), (False, True), (True, True)):
             Xd = offset_by_one(cuda, X) if xoff else dev(cuda, X, True)
             Yd = offset_by_one(cuda, Y0) if yoff else dev(cuda, Y0, True)
             got = spmv(h, "N", 2.5, A, Xd, -0.5, Yd)
-            what = f"{h.last_kernel()} {env} k={k} offsets x={xoff} y={yoff}"
-            assert h.last_kernel() == vec_kernel.replace("_vec", "").replace("+seg", ""), what
+            what = f"{h.last_kernel()} k={k} offsets x={xoff} y={yoff}"
+            assert h.last_kernel() == "spmm_items", what
             R.assert_within(got, exact, bound, what)
-            if env.get("B200SP_SPMM_KERNEL") != "split":  # the split kernels add rows cut by a chunk border with atomics
-                assert np.array_equal(bits(got[rows]), bits(ref[rows])), what + ": differs from the aligned vector kernel"
+            assert np.array_equal(bits(got), bits(ref)), what + ": differs from the aligned vector kernel"
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("kern", ["tile", "tilev"])
-def test_misaligned_matrix_arrays(cuda, monkeypatch, kern, dtype):
-    """vals / col_idx one element off 16-byte alignment: the TMA-fed tile kernel cannot take them; the fallback must be
-    taken and be right, in both layouts."""
+def test_misaligned_matrix_arrays(cuda, dtype):
+    """vals / col_idx one element off 16-byte alignment: the item path reads them entry by entry, so it takes them and must
+    be right, in both layouts."""
     from kokkos_kernels_b200 import sparse as sp
 
-    monkeypatch.setenv("B200SP_SPMM_KERNEL", kern)
     rp, ci, v, ncols = A_np = matrix("thresholds", dtype)
     A = sp.CrsMatrix(torch.from_numpy(rp).to(cuda), offset_by_one(cuda, ci[:, None])[:, 0], offset_by_one(cuda, v[:, None])[:, 0], ncols)
     assert A.entries.data_ptr() % 16 != 0 and A.values.data_ptr() % 16 != 0
@@ -321,10 +285,7 @@ def test_misaligned_matrix_arrays(cuda, monkeypatch, kern, dtype):
         for layout in ("RR", "LL"):
             h = sp.SPMVHandle()
             got = spmv(h, "N", 2.5, A, dev(cuda, X, layout[0] == "R"), -0.5, dev(cuda, Y0, layout[1] == "R"))
-            if layout == "RR":
-                assert h.last_kernel() == "spmm_split", h.last_kernel()
-            else:
-                assert h.last_kernel() in ("spmm_relayout+split", "spmm_general"), h.last_kernel()
+            assert h.last_kernel() == expected_kernel(k, dtype, layout), h.last_kernel()
             R.assert_within(got, exact, bound, f"{h.last_kernel()} k={k} {layout} misaligned vals/col_idx")
 
 
@@ -333,13 +294,10 @@ SCALARS = [(1.0, 0.0), (-1.0, 1.0), (2.5, -0.5), (0.0, 2.5), (0.0, 0.0), (1.0, 1
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("env", [{}, {"B200SP_SPMM_KERNEL": "tilev"}, {"B200SP_SPMM_KERNEL": "split"}], ids=["items", "tilev", "split"])
-def test_scalars(cuda, monkeypatch, env, dtype):
+def test_scalars(cuda, dtype):
     """Every (alpha, beta) pair; beta == 0 over a Y of NaN; alpha == 0 over an X of NaN gives exactly beta*Y0."""
     from kokkos_kernels_b200 import sparse as sp
 
-    for k_, v_ in env.items():
-        monkeypatch.setenv(k_, v_)
     for name in ("thresholds", "cancelling", "small_mod2", "no_columns"):
         A_np = matrix(name, dtype)
         A = dev_matrix(cuda, *A_np)
@@ -358,21 +316,16 @@ def test_scalars(cuda, monkeypatch, env, dtype):
                         assert h.last_kernel() == "none", what
                         assert torch.equal(torch.from_numpy(got).to(cuda), expect0), what
                     else:
-                        assert h.last_kernel() == expected_kernel(env, k, dtype, layout), what
+                        assert h.last_kernel() == expected_kernel(k, dtype, layout), what
                         R.assert_within(got, R.spmm_exact(*A_np[:3], X, Y0, alpha, beta), R.spmm_bound(*A_np[:3], X, Y0, alpha, beta), what)
 
 
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("env", [{}, {"B200SP_SPMM_KERNEL": "tile"}, {"B200SP_SPMM_KERNEL": "tilev", "B200SP_SPMM_SEG": "vec"},
-                                 {"B200SP_SPMM_KERNEL": "split", "B200SP_SPMM_VEC": "1"}, {"B200SP_SPMM_KERNEL": "row"}],
-                         ids=["items", "tile", "tilev_segvec", "split_vec", "row"])
-def test_single_inf_reaches_exactly_its_rows(cuda, monkeypatch, env, dtype):
+def test_single_inf_reaches_exactly_its_rows(cuda, dtype):
     """One Inf in X(c, j): exactly the rows of A that reference column c turn non-finite in column j (the reference
     says which: +-Inf, or NaN where terms of both signs meet); every other entry stays finite and within its bound."""
     from kokkos_kernels_b200 import sparse as sp
 
-    for k_, v_ in env.items():
-        monkeypatch.setenv(k_, v_)
     rp, ci, v, ncols = A_np = matrix("thresholds", dtype)
     A = dev_matrix(cuda, *A_np)
     counts = np.bincount(ci, minlength=ncols)
@@ -388,94 +341,41 @@ def test_single_inf_reaches_exactly_its_rows(cuda, monkeypatch, env, dtype):
             for layout in ("RR", "LL"):
                 h = sp.SPMVHandle()
                 got = spmv(h, "N", 1.5, A, dev(cuda, Xi, layout[0] == "R"), 0.5, dev(cuda, Y0, layout[1] == "R"))
-                assert h.last_kernel() == expected_kernel(env, k, dtype, layout), h.last_kernel()
+                assert h.last_kernel() == expected_kernel(k, dtype, layout), h.last_kernel()
                 R.assert_within(got, exact, R.spmm_bound(rp, ci, v, Xi, Y0, 1.5, 0.5), f"{h.last_kernel()} Inf at X({c},{j}) k={k} {layout}")
 
 
 # ---- (e) determinism and the stated identities -----------------------------------------------------------------------
 @pytest.mark.parametrize("dtype", DTYPES)
-def test_items_and_tile_are_deterministic(cuda, monkeypatch, dtype):
-    """The item and tile kernels use no atomics: a second call through the same handle gives the same bits; and the
-    item path gives the same bits for LayoutLeft as for LayoutRight (the relayout only moves data).  The tile path hands
-    rows of several 2048-entry segments to the segment kernel, which adds the segments with atomics: those rows are
-    checked against the bound only."""
+def test_items_are_deterministic(cuda, dtype):
+    """The item path uses no atomics: a second call through the same handle gives the same bits; and it gives the same bits
+    for LayoutLeft as for LayoutRight (the relayout only moves data)."""
     from kokkos_kernels_b200 import sparse as sp
 
     A_np = matrix("thresholds", dtype)
     A = dev_matrix(cuda, *A_np)
-    single_segment = np.diff(A_np[0]) <= 2048
-    for kern in ("items", "tile", "tilev"):
-        monkeypatch.setenv("B200SP_SPMM_KERNEL", kern)
-        for k in (3, 16, 132):
-            X, Y0 = operands(A_np, k, dtype)
-            h = sp.SPMVHandle()
-            outs = {}
-            for layout in ("RR", "RR", "LL", "RL", "LR"):
-                got = spmv(h, "N", 1.5, A, dev(cuda, X, layout[0] == "R"), -0.5, dev(cuda, Y0, layout[1] == "R"))
-                check(got, A_np, X, Y0, 1.5, -0.5, False, f"{h.last_kernel()} k={k} {layout}")
-                if layout in outs:
-                    rows = slice(None) if kern == "items" else single_segment
-                    assert np.array_equal(bits(got[rows]), bits(outs[layout][rows])), (kern, k, "second call differs")
-                outs[layout] = got
-            if kern == "items" and k >= 4:  # below 4 columns LayoutLeft operands take spmm_general_kernel
-                for layout in ("LL", "RL", "LR"):
-                    assert np.array_equal(bits(outs[layout]), bits(outs["RR"])), (k, layout, "differs from RR")
-
-
-_CHILD = r"""
-import sys
-import numpy as np
-sys.path[:0] = [{root!r}, {tests!r}]
-import torch
-import spmm_cases
-from kokkos_kernels_b200 import sparse as sp
-dtype = np.dtype({dtype!r}).type
-rp, ci, v, ncols = spmm_cases.thresholds(5, dtype)
-dev = torch.device("cuda:0")
-A = sp.CrsMatrix(torch.from_numpy(rp).to(dev), torch.from_numpy(ci).to(dev), torch.from_numpy(v).to(dev), ncols)
-rng = np.random.default_rng(3)
-h = sp.SPMVHandle()
-outs = []
-for k in (5, 16, 132):
-    X = spmm_cases.dense_operands(rng, ncols, k, dtype)
-    Y0 = spmm_cases.dense_operands(rng, len(rp) - 1, k, dtype)
-    Y = torch.from_numpy(Y0).to(dev)
-    sp.spmv(h, "N", 1.5, A, torch.from_numpy(X).to(dev), -0.5, Y)
-    assert h.last_kernel().startswith("spmm_items"), h.last_kernel()
-    outs.append(Y.cpu().numpy().ravel())
-np.save({out!r}, np.concatenate(outs))
-"""
-
-
-@pytest.mark.skipif(EMULATED, reason="runs the library on the GPU in child processes")
-@pytest.mark.parametrize("dtype", DTYPES)
-def test_item_kernels_give_the_same_bits(cuda, dtype):
-    """The first item kernel (B200SP_SPMM_ITEM_COOP=0) and the cooperative ones with batches of 4 and 8: the same items and
-    the same order of additions, so the same Y (DESIGN.md 4.2).  The variable is read once per process, so each setting
-    runs in a child process of its own."""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    res = {}
-    with tempfile.TemporaryDirectory() as tmp:
-        for coop in ("0", "4", "8"):
-            out = os.path.join(tmp, f"y{coop}.npy")
-            code = _CHILD.format(root=root, tests=os.path.join(root, "tests"), dtype=np.dtype(dtype).name, out=out)
-            env = dict(os.environ, B200SP_SPMM_ITEM_COOP=coop)
-            p = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=600)
-            assert p.returncode == 0, p.stderr[-3000:]
-            res[coop] = np.load(out)
-    assert np.array_equal(res["0"].view(np.uint8), res["4"].view(np.uint8))
-    assert np.array_equal(res["0"].view(np.uint8), res["8"].view(np.uint8))
+    for k in (3, 16, 132):
+        X, Y0 = operands(A_np, k, dtype)
+        h = sp.SPMVHandle()
+        outs = {}
+        for layout in ("RR", "RR", "LL", "RL", "LR"):
+            got = spmv(h, "N", 1.5, A, dev(cuda, X, layout[0] == "R"), -0.5, dev(cuda, Y0, layout[1] == "R"))
+            check(got, A_np, X, Y0, 1.5, -0.5, False, f"{h.last_kernel()} k={k} {layout}")
+            if layout in outs:
+                assert np.array_equal(bits(got), bits(outs[layout])), (k, "second call differs")
+            outs[layout] = got
+        if k >= 4:  # below 4 columns LayoutLeft operands take spmm_general_kernel
+            for layout in ("LL", "RL", "LR"):
+                assert np.array_equal(bits(outs[layout]), bits(outs["RR"])), (k, layout, "differs from RR")
 
 
 # ---- (f) one handle, changing shapes ---------------------------------------------------------------------------------
 @pytest.mark.parametrize("dtype", DTYPES)
-@pytest.mark.parametrize("kern", ["items", "tilev", "split"])
-def test_one_handle_growing_and_shrinking_k(cuda, monkeypatch, kern, dtype):
+def test_one_handle_growing_and_shrinking_k(cuda, dtype):
     """k = 16, 129, 4, 64 through one handle and one matrix, layouts RR, LL, RL, LR in turn, beta alternating between 0
     and not: the plan's partial sums and relayout scratch are re-grown and reused."""
     from kokkos_kernels_b200 import sparse as sp
 
-    monkeypatch.setenv("B200SP_SPMM_KERNEL", kern)
     A_np = matrix("thresholds", dtype)
     A = dev_matrix(cuda, *A_np)
     h = sp.SPMVHandle()
@@ -487,7 +387,7 @@ def test_one_handle_growing_and_shrinking_k(cuda, monkeypatch, kern, dtype):
             step += 1
             Yin = np.full_like(Y0, np.nan) if beta == 0 else Y0
             got = spmv(h, "N", -2.0, A, dev(cuda, X, layout[0] == "R"), beta, dev(cuda, Yin, layout[1] == "R"))
-            assert h.last_kernel() == expected_kernel({"B200SP_SPMM_KERNEL": kern}, k, dtype, layout), (k, layout, h.last_kernel())
+            assert h.last_kernel() == expected_kernel(k, dtype, layout), (k, layout, h.last_kernel())
             check(got, A_np, X, Y0, -2.0, beta, False, f"{h.last_kernel()} k={k} {layout} b={beta}")
 
 
@@ -505,7 +405,7 @@ def test_reduce_kernels_wrap(cuda, dtype, k):
         X, Y0 = operands(A_np, k, dtype)
         h = sp.SPMVHandle()
         got = spmv(h, "N", 1.5, A, dev(cuda, X, layout[0] == "R"), -0.5, dev(cuda, Y0, layout[1] == "R"))
-        assert h.last_kernel() == expected_kernel({}, k, dtype, layout), h.last_kernel()
+        assert h.last_kernel() == expected_kernel(k, dtype, layout), h.last_kernel()
         check(got, A_np, X, Y0, 1.5, -0.5, False, f"{h.last_kernel()} {name} k={k} {layout}")
 
 
@@ -523,7 +423,7 @@ def test_relayout_and_scale_wrap(cuda, dtype):
         for layout in ("LL", "RL", "LR"):
             h = sp.SPMVHandle()
             got = spmv(h, "N", 2.5, A, dev(cuda, X, layout[0] == "R"), -0.5, dev(cuda, Y0, layout[1] == "R"))
-            assert h.last_kernel() == expected_kernel({}, k, dtype, layout), h.last_kernel()
+            assert h.last_kernel() == expected_kernel(k, dtype, layout), h.last_kernel()
             check(got, A_np, X, Y0, 2.5, -0.5, False, f"{h.last_kernel()} tall k={k} {layout}")
             Yd = dev(cuda, Y0, layout[1] == "R")
             expect = Yd * 0.5

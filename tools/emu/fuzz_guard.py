@@ -194,25 +194,18 @@ def op_spmm(rng, orc, verbose):
     X = np.asarray(rng.uniform(-1, 1, (nx, k)).astype(dtype), order=order)
     Y0 = np.asarray(rng.uniform(-1, 1, (ny, k)).astype(dtype), order=order)
     alpha, beta = [(1.0, 0.0), (-2.0, 0.5), (1.0, 1.0)][rng.integers(0, 3)]
-    kern_env = ["tilev", "tile", "split", "row"][rng.integers(0, 4)]
-    os.environ["B200SP_SPMM_KERNEL"] = kern_env
-    if rng.random() < 0.3:
-        os.environ["B200SP_SPMM_SEG"] = "vec"
-    else:
-        os.environ.pop("B200SP_SPMM_SEG", None)
     grp, gci, gv = g(rp, rng), g(ci, rng), g(v, rng)
     gX, gY = E.guarded(X, 16 if rng.random() < 0.6 else None), E.guarded(Y0, 16 if rng.random() < 0.6 else None)
     plan = E.SpmvPlan()
     E.spmm(plan, mode, m, n, grp, gci, gv, gX, gY, alpha, beta)
+    kern = plan.kernel()
     plan.close()
-    os.environ.pop("B200SP_SPMM_KERNEL", None)
-    os.environ.pop("B200SP_SPMM_SEG", None)
     Yc = Y0.copy(order=order)
     exp = orc.spmv_mv_transpose(rp, ci, v, n, X, Yc, alpha, beta) if trans else orc.spmv_mv(rp, ci, v, n, X, Yc, alpha, beta)
     ok = True
     for j in range(k):
         ok &= scaled_ok(gY[:, j], exp[:, j], row_scale(rp, ci, v, X[:, j], Y0[:, j], alpha, beta, n, trans), TOL[np.dtype(dtype)])
-    return ok, f"spmm {mode} {np.dtype(dtype).name} {m}x{n} k={k} {order} kernel={kern_env}"
+    return ok, f"spmm {mode} {np.dtype(dtype).name} {m}x{n} k={k} {order} kernel={kern}"
 
 
 def op_spgemm(rng, orc, verbose):

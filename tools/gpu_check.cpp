@@ -865,7 +865,7 @@ static void suite_crs_big() {
 }
 
 // ------------------------------------------------------------------------------------------------
-// suite: spmm -- kernel variants of the rank-2 product (B200SP_SPMM_KERNEL) against the oracle + timing
+// suite: spmm -- the rank-2 product's default path (the item kernel) against the oracle + timing
 // ------------------------------------------------------------------------------------------------
 static int g_timeout_scale = 1;  // --timeout-scale N: the emulated build is orders of magnitude slower
 static int g_spmm_scale = 0;  // --spmm-scale N (default 18, 21 with --big; 23 = BASELINE.json config 3)
@@ -902,7 +902,7 @@ static void suite_spmm() {
   } else {
     Rng r(1);
     for (int i = 0; i < 3000; ++i) sample.push_back(r.below(n));
-    // the longest rows (segment path) are part of the sample
+    // the longest rows (the most pieces) are part of the sample
     std::vector<int> order(n);
     std::iota(order.begin(), order.end(), 0);
     std::partial_sort(order.begin(), order.begin() + 40, order.end(), [&](int a, int b) { return rp[a + 1] - rp[a] > rp[b + 1] - rp[b]; });
@@ -932,47 +932,23 @@ static void suite_spmm() {
   Dev<int> drp(rp), dci(ci);
   Dev<float> dv(v), dX(X), dY((size_t)n * k);
   const double balg = 8.0 * nnz + 4.0 * (n + 1) + 4.0 * (double)n * k * 3;
-  struct Var {
-    const char* kernel;
-    const char* lmax;
-    const char* cfg;
-  };
-  const Var vars[] = {{"split", nullptr, nullptr}, {"tile", nullptr, nullptr},  {"tilev", nullptr, nullptr}, {"tilev", "64", nullptr},
-                      {"tilev", "128", nullptr},   {"tilev", "512", nullptr},   {"tilev", nullptr, "1"},     {"tilev", nullptr, "2"},
-                      {"tilev", nullptr, "3"},     {"tilev", "128", "1"},       {"tilev", "128", "2"},       {"tilev", "128", "segvec"},
-                      {"tilev", "64", "segvec"},   {"row", nullptr, nullptr}};
-  for (const Var& vr : vars) {
-    if (!strcmp(vr.kernel, "row") && scale > 21) continue;  // far the slowest at scale 21: not worth the slot
-    setenv("B200SP_SPMM_KERNEL", vr.kernel, 1);
-    if (vr.lmax) setenv("B200SP_SPMM_LMAX", vr.lmax, 1);
-    else unsetenv("B200SP_SPMM_LMAX");
-    unsetenv("B200SP_SPMM_CFG");
-    unsetenv("B200SP_SPMM_SEG");
-    if (vr.cfg && !strcmp(vr.cfg, "segvec")) setenv("B200SP_SPMM_SEG", "vec", 1);
-    else if (vr.cfg) setenv("B200SP_SPMM_CFG", vr.cfg, 1);
-    b200sp_spmv_plan* plan = nullptr;
-    SP(b200sp_spmv_plan_create(&plan, 0));
-    float best = 1e30f;
-    for (int rep = 0; rep < 5; ++rep) {
-      CK(cudaMemcpy(dY.p, Y0.data(), Y0.size() * sizeof(float), cudaMemcpyHostToDevice));
-      Timer t;
-      t.start();
-      SP(b200sp_spmm_f32_i32(plan, nullptr, 'N', n, n, nnz, k, alpha, drp.p, dci.p, dv.p, dX.p, k, 1, beta, dY.p, k, 1));
-      const float ms = t.stop_ms();
-      if (rep > 0) best = std::min(best, ms);
-    }
-    const double worst = check(dY.host());
-    char nm[96];
-    snprintf(nm, sizeof(nm), "rmat%d_k16_f32/%s%s%s%s%s", scale, vr.kernel, vr.lmax ? "_lmax" : "", vr.lmax ? vr.lmax : "", vr.cfg ? "_cfg" : "",
-             vr.cfg ? vr.cfg : "");
-    record(nm, worst <= 1e-4, "kernel=%s %.3f ms, %.0f GFLOP/s, %.0f GB/s algorithmic, max scaled err %.2e (%s)", b200sp_spmv_last_kernel(plan), best,
-           2.0 * nnz * k / (best * 1e-3) / 1e9, balg / (best * 1e-3) / 1e9, worst, full_check ? "all rows" : "sampled + longest rows");
-    b200sp_spmv_plan_destroy(plan, nullptr);
+  b200sp_spmv_plan* plan = nullptr;
+  SP(b200sp_spmv_plan_create(&plan, 0));
+  float best = 1e30f;
+  for (int rep = 0; rep < 5; ++rep) {
+    CK(cudaMemcpy(dY.p, Y0.data(), Y0.size() * sizeof(float), cudaMemcpyHostToDevice));
+    Timer t;
+    t.start();
+    SP(b200sp_spmm_f32_i32(plan, nullptr, 'N', n, n, nnz, k, alpha, drp.p, dci.p, dv.p, dX.p, k, 1, beta, dY.p, k, 1));
+    const float ms = t.stop_ms();
+    if (rep > 0) best = std::min(best, ms);
   }
-  unsetenv("B200SP_SPMM_KERNEL");
-  unsetenv("B200SP_SPMM_LMAX");
-  unsetenv("B200SP_SPMM_CFG");
-  unsetenv("B200SP_SPMM_SEG");
+  const double worst = check(dY.host());
+  char nm[96];
+  snprintf(nm, sizeof(nm), "rmat%d_k16_f32/default", scale);
+  record(nm, worst <= 1e-4, "kernel=%s %.3f ms, %.0f GFLOP/s, %.0f GB/s algorithmic, max scaled err %.2e (%s)", b200sp_spmv_last_kernel(plan), best,
+         2.0 * nnz * k / (best * 1e-3) / 1e9, balg / (best * 1e-3) / 1e9, worst, full_check ? "all rows" : "sampled + longest rows");
+  b200sp_spmv_plan_destroy(plan, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1431,11 +1407,7 @@ static void spmm_sweep_matrix(const char* name, const Csr<S>& A) {
   Csr<S> Aabs = A;
   for (auto& t : Aabs.v) t = std::fabs(t);
   const double tol = sizeof(S) == 8 ? 1e-13 : 2e-5;
-  for (const char* kern : {"tilev", "tile", "split", "tilev+segvec"}) {
-    const bool segvec = strstr(kern, "segvec") != nullptr;
-    setenv("B200SP_SPMM_KERNEL", segvec ? "tilev" : kern, 1);
-    if (segvec) setenv("B200SP_SPMM_SEG", "vec", 1);
-    else unsetenv("B200SP_SPMM_SEG");
+  for (const bool with_plan : {true, false}) {
     int bad = 0, runs = 0;
     double worst = 0;
     std::string last;
@@ -1458,11 +1430,11 @@ static void spmm_sweep_matrix(const char* name, const Csr<S>& A) {
               for (int j = 0; j < k; ++j) Yin[(size_t)r * ldy + j] = std::numeric_limits<S>::quiet_NaN();
           Dev<S> dX(X), dY(Yin);
           b200sp_spmv_plan* plan = nullptr;
-          SP(b200sp_spmv_plan_create(&plan, 0));
+          if (with_plan) SP(b200sp_spmv_plan_create(&plan, 0));
           SP(gspmm(plan, A.m, A.n, A.nnz(), k, al, rp.p, ci.p, v.p, dX.p, ldx, be, dY.p, ldy));
           CK(cudaDeviceSynchronize());
-          last = b200sp_spmv_last_kernel(plan);
-          b200sp_spmv_plan_destroy(plan, nullptr);
+          last = with_plan ? b200sp_spmv_last_kernel(plan) : "no plan";
+          if (plan) b200sp_spmv_plan_destroy(plan, nullptr);
           auto got = dY.host();
           ++runs;
           bool ok = true;
@@ -1486,12 +1458,10 @@ static void spmm_sweep_matrix(const char* name, const Csr<S>& A) {
       }
     }
     char nm[128];
-    snprintf(nm, sizeof(nm), "%s/%s", name, kern);
+    snprintf(nm, sizeof(nm), "%s/%s", name, with_plan ? "plan" : "no_plan");
     record(nm, bad == 0, "%d runs (13 column counts x 2 leading dimensions x beta in {0, -0.5}), %d bad, max scaled err %.2e, last kernel %s",
            runs, bad, worst, last.c_str());
   }
-  unsetenv("B200SP_SPMM_KERNEL");
-  unsetenv("B200SP_SPMM_SEG");
 }
 
 static void suite_spmm_sweep() {

@@ -3,7 +3,7 @@
 instruction count comes from.  Uses the object files of the in-tree build (compiled with -lineinfo).
 
   python tools/sass_lines.py spgemm num_hash_kernel 'double, (int)128, (int)4096'
-  python tools/sass_lines.py spmm spmm_tile_kernel 'float, (int)4, (int)4'
+  python tools/sass_lines.py spmm spmm_item_coop_kernel 'float, (int)4, (int)4'
 
 Prints `line  #instructions  source text` for the kernel whose demangled name contains every given substring
 (first match), plus totals per opcode class.  Weigh the lines with the trip counts of the case at hand."""
